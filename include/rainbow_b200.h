@@ -206,8 +206,13 @@ typedef struct rb_head_grads {   /* gradients are OVERWRITTEN (not accumulated) 
  * s1 is the larger of the two layer-1 implementations' factors (tensor-core kernel, csrc/rb_head_tc.cu; FFMA kernel). */
 int rb_head_splits(int conv_features, int hidden, int* s1, int* s2);
 int rb_head_ticket_count(void);
+/* Whether the fused head takes this shape, without touching the device: RB_OK, or the code rb_head_forward over `rows`
+ * rows (rows > 0) and rb_head_backward over `backward_batch` rows (backward_batch > 0) would return for it with valid
+ * pointers.  rows == 0 / backward_batch == 0 leave that call out.  Both calls check these limits before they launch
+ * anything: a refused backward writes nothing. */
+int rb_head_supported(int conv_features, int hidden, int atoms, int actions, int rows, int backward_batch);
 /* probes / tests only: bit 0 skips the layer-1 launch of rb_head_forward, bit 1 the layer-2 launch, bit 2 forces the FFMA
- * layer-1 kernel instead of the tensor-core one (0 = normal) */
+ * layer-1 kernel instead of the tensor-core one, bit 3 the split-K layer-2 kernel instead of the single-pass one (0 = normal) */
 int rb_head_debug(int flags);
 
 /* Forward over M = m_lo + m_hi rows (x_lo: [m_lo][conv_features], x_hi: [m_hi][conv_features] or NULL).
@@ -222,7 +227,8 @@ int rb_head_forward(const rb_head_params* p, const float* x_lo, int m_lo, const 
 /* q[M][actions][atoms] = zv + za - mean_a(za) (model.py:75) from z. */
 int rb_head_logits(const float* z, int M, int actions, int atoms, float* q, rb_stream_t stream);
 
-/* Backward for B <= 32 rows: given dz[B][atoms*(1+actions)] (value block first), x[B][conv_features] and h[B][2*hidden]
+/* Backward for B <= 32 rows, hidden <= 1024 and actions * atoms small enough for the dh kernel's shared memory (about
+ * 1060; rb_head_supported says which shapes): given dz[B][atoms*(1+actions)] (value block first), x[B][conv_features] and h[B][2*hidden]
  * writes all 16 parameter gradients through `g` and dx[B][conv_features].  dh_scratch: float32[(B + 32) * 2*hidden]
  * (dh [B][2*hidden], then its transpose [2*hidden][32] for the layer-1 kernel).
  * relu_mask_x != 0 additionally zeroes dx where x <= 0, i.e. folds in the backward of the ReLU that produced the conv

@@ -331,7 +331,8 @@ class Agent:
     # ---- the update ------------------------------------------------------------------------------
     def _fused_path(self, B):
         on = self.online_net
-        return self.use_fused_head and B <= 32 and on.training and on.fused_ok(2 * B) and self.target_net.fused_ok(B)
+        return (self.use_fused_head and B <= 32 and on.training and on.fused_ok(2 * B, backward_batch=B) and
+                self.target_net.fused_ok(B))
 
     @staticmethod
     def _adjacent(states, next_states):

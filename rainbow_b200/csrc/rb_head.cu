@@ -990,6 +990,30 @@ k_conv_wgrad_reduce(const float* __restrict__ part, int n_part, int n_w, int n_b
   }
 }
 
+// Every shape limit of rb_head_forward (rows > 0) and rb_head_backward (backward: over bwd_batch rows), checked before
+// anything is launched; rb_head_supported exports it so callers can pick another path instead of meeting the error
+// mid-update.
+int head_shape_check(int K1, int H, int Z, int A, int rows, int bwd_batch, bool backward) {
+  if (K1 <= 0 || H <= 0 || Z <= 1 || A <= 0 || rows < 0) return rbi::fail(RB_ERR_INVAL, "rb_head: bad size");
+  if (K1 % 32 || H % 64) return rbi::fail(RB_ERR_RANGE, "rb_head: conv_features % 32 == 0 and hidden % 64 == 0 required");
+  if (rows > 0) {
+    const int MT = (rows > 32) ? 64 : 32;
+    const long long mt = (rows + MT - 1) / MT;
+    const long long tiles1 = 2 * H / NT, tiles2 = (Z + NT - 1) / NT + ((long long)A * Z + NT - 1) / NT;
+    if (mt > 65535 || mt * tiles1 > 2048 || mt * tiles2 > 2048) return rbi::fail(RB_ERR_RANGE, "rb_head_forward: too many rows");
+  }
+  if (backward) {
+    if (bwd_batch <= 0 || bwd_batch > 32)
+      return rbi::fail(RB_ERR_RANGE, "rb_head_backward: 1 <= B <= 32 required (larger batches use the library GEMM path)");
+    const long long ns_max = (long long)A * Z > Z ? (long long)A * Z : Z;
+    const long long ld_dz = ns_max | 1;
+    const long long smem = (32 * ld_dz + 2 * ((ns_max + 3) & ~3ll) * DH_KB) * (long long)sizeof(float);
+    if (smem > 200 * 1024 || H % DH_KB) return rbi::fail(RB_ERR_RANGE, "rb_head_backward: actions * atoms too large for the dh kernel");
+    if (H > 1024) return rbi::fail(RB_ERR_RANGE, "rb_head_backward: hidden <= 1024 required");
+  }
+  return RB_OK;
+}
+
 int head_check(const rb_head_params* p, const char* who) {
   if (!p) return rbi::fail(RB_ERR_INVAL, who);
   for (int s = 0; s < 2; ++s)
@@ -1008,7 +1032,6 @@ int head_check(const rb_head_params* p, const char* who) {
                            (uintptr_t)p->eps_out1[s] | (uintptr_t)p->eps_in2[s];
     if (bits & 15) return rbi::fail(RB_ERR_INVAL, "rb_head: weight / bias / factor pointers must be 16-byte aligned");
   }
-  if (p->conv_features % 32 || p->hidden % 64) return rbi::fail(RB_ERR_RANGE, "rb_head: conv_features % 32 == 0 and hidden % 64 == 0 required");
   return RB_OK;
 }
 
@@ -1046,6 +1069,10 @@ int rb_head_splits(int conv_features, int hidden, int* s1, int* s2) {
 
 int rb_head_ticket_count(void) { return 4096; }
 
+int rb_head_supported(int conv_features, int hidden, int atoms, int actions, int rows, int backward_batch) {
+  return head_shape_check(conv_features, hidden, atoms, actions, rows, backward_batch, backward_batch != 0);
+}
+
 static int g_head_debug = 0;   // bit 0: skip the layer-1 launch, bit 1: skip the layer-2 launch (timing probes only); bit 2: FFMA layer 1; bit 3: split-K layer 2
 int rb_head_debug(int flags) {
   g_head_debug = flags;
@@ -1059,6 +1086,8 @@ int rb_head_forward(const rb_head_params* p, const float* x_lo, int m_lo, const 
   const int M = m_lo + m_hi;
   if (!x_lo || m_lo <= 0 || m_hi < 0 || (m_hi > 0 && !x_hi) || !part1 || !part2 || !tickets || !h || !z)
     return rbi::fail(RB_ERR_INVAL, "rb_head_forward: bad argument");
+  rc = head_shape_check(p->conv_features, p->hidden, p->atoms, p->actions, M, 0, false);
+  if (rc != RB_OK) return rc;
   const HeadDesc d = to_desc(p);
   int s1, s2, ks1, ks2;
   head_splits(d.K1, d.H, &s1, &s2, &ks1, &ks2);
@@ -1066,7 +1095,6 @@ int rb_head_forward(const rb_head_params* p, const float* x_lo, int m_lo, const 
   const int MT = (M > 32) ? 64 : 32;
   const int mt = (M + MT - 1) / MT;
   const int tiles1 = 2 * d.H / NT, tiles2 = (d.Z + NT - 1) / NT + (d.A * d.Z + NT - 1) / NT;
-  if (mt > 65535 || mt * tiles1 > 2048 || mt * tiles2 > 2048) return rbi::fail(RB_ERR_RANGE, "rb_head_forward: too many rows");
   const size_t smem64 = (size_t)FC_STAGES * (64 + 2 * NT) * (KT + 4) * sizeof(float);
   const size_t smem32 = (size_t)FC_STAGES * (32 + 2 * NT) * (KT + 4) * sizeof(float);
   rc = rbi::ensure_dynamic_smem(k_head_fc<64, 1>, smem64, "rb_head_forward");
@@ -1119,7 +1147,8 @@ int rb_head_backward(const rb_head_params* p, const rb_head_grads* gr, const flo
   if ((parts & 7) == 0) return rbi::fail(RB_ERR_INVAL, "rb_head_backward: parts must select at least one of RB_HEAD_BWD_*");
   if (rc != RB_OK) return rc;
   if (!gr || !x || !h || !dz || !dh_scratch || !dx) return rbi::fail(RB_ERR_INVAL, "rb_head_backward: null pointer");
-  if (B <= 0 || B > 32) return rbi::fail(RB_ERR_RANGE, "rb_head_backward: 1 <= B <= 32 required (larger batches use the library GEMM path)");
+  rc = head_shape_check(p->conv_features, p->hidden, p->atoms, p->actions, 0, B, true);   // all limits, whatever `parts` selects
+  if (rc != RB_OK) return rc;
   HeadGrads g;
   for (int s = 0; s < 2; ++s) {
     if (!gr->w1_mu[s] || !gr->w1_sigma[s] || !gr->b1_mu[s] || !gr->b1_sigma[s] || !gr->w2_mu[s] || !gr->w2_sigma[s] ||
@@ -1141,8 +1170,7 @@ int rb_head_backward(const rb_head_params* p, const rb_head_grads* gr, const flo
   if (parts & RB_HEAD_BWD_DH) {
     const int ns_max = d.A * d.Z > d.Z ? d.A * d.Z : d.Z;
     const int ld_dz = ns_max | 1;                       // odd row stride: the 32 rows of a column hit 32 different banks
-    const size_t smem = ((size_t)32 * ld_dz + 2 * (size_t)((ns_max + 3) & ~3) * DH_KB) * sizeof(float);
-    if (smem > 200 * 1024 || d.H % DH_KB) return rbi::fail(RB_ERR_RANGE, "rb_head_backward: actions * atoms too large for the dh kernel");
+    const size_t smem = ((size_t)32 * ld_dz + 2 * (size_t)((ns_max + 3) & ~3) * DH_KB) * sizeof(float);   // <= 200 KB: head_shape_check
     rc = rbi::ensure_dynamic_smem(k_head_dh, smem, "rb_head_backward");
     if (rc != RB_OK) return rc;
     dim3 grid(d.H / DH_KB, 2);
@@ -1151,8 +1179,7 @@ int rb_head_backward(const rb_head_params* p, const rb_head_grads* gr, const flo
   }
   rc = rbi::check_launch("rb_head_backward(dh)");
   if (rc != RB_OK) return rc;
-  if (parts & RB_HEAD_BWD_LAYER1) {
-    if (d.H > 1024) return rbi::fail(RB_ERR_RANGE, "rb_head_backward: hidden <= 1024 required");
+  if (parts & RB_HEAD_BWD_LAYER1) {   // hidden <= 1024 (EoAll holds H / 2 factors): head_shape_check
     dim3 grid(d.K1 / B1_K, 4);
     rbi::ProfScope prof_(RB_K_HEAD_BWD1, st);
     const size_t smem_b1 = (size_t)B1_STAGES * B1_STAGE * sizeof(float);

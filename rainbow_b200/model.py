@@ -18,6 +18,7 @@ plain torch path (composed weights + F.linear) so autograd works as in the refer
 rainbow_b200.agent drives the fused forward AND backward kernels itself.
 """
 import ctypes as C
+import functools
 import math
 
 import torch
@@ -90,6 +91,11 @@ def resample_noise(layers, seed, rng_counter, x_in=None, x_out=None):
                                              _lib.ptr(rng_counter), _lib.stream()))
 
 
+@functools.lru_cache(maxsize=None)
+def _head_shape_rc(conv_features, hidden, atoms, actions, rows, backward_batch):
+    return _lib.load().rb_head_supported(conv_features, hidden, atoms, actions, rows, backward_batch)
+
+
 class FusedHead:
     """Launcher of the fused noisy dueling head kernels for one DQN (csrc/rb_head.cu)."""
 
@@ -106,9 +112,11 @@ class FusedHead:
         self._tickets = None
 
     @staticmethod
-    def supported(net):
-        return (net.conv_output_size % 32 == 0 and net.hidden_size % 64 == 0 and net.atoms <= 128 and
-                next(net.parameters()).is_cuda)
+    def supported(net, rows=1, backward_batch=0):
+        """Whether the fused kernels take this net's head over `rows` forward rows and, if backward_batch > 0, a backward
+        over that many rows (rb_head_supported); atoms <= 128 is what rb_q_values and the fused C51 loss take."""
+        return (net.atoms <= 128 and next(net.parameters()).is_cuda and
+                _head_shape_rc(net.conv_output_size, net.hidden_size, net.atoms, net.action_space, rows, backward_batch) == 0)
 
     def params(self, noisy=None):
         net = self.net
@@ -301,8 +309,9 @@ class DQN(nn.Module):
             self._head = FusedHead(self)
         return self._head
 
-    def fused_ok(self, rows):
-        return self.use_fused_head and rows <= FusedHead.MAX_ROWS and FusedHead.supported(self)
+    def fused_ok(self, rows, backward_batch=0):
+        """The fused head serves a forward over `rows` rows (and a backward over `backward_batch` rows, if > 0)."""
+        return self.use_fused_head and rows <= FusedHead.MAX_ROWS and FusedHead.supported(self, rows, backward_batch)
 
     def features(self, x):
         return self.convs(x).view(-1, self.conv_output_size)

@@ -74,6 +74,32 @@ def test_abi_argument_validation_without_gpu():
     assert lib.rb_peer_scratch_bytes() >= (2 * 592 + 2) * 8
 
 
+def test_head_supported_without_gpu():
+    """rb_head_supported is host arithmetic: the fused head's shape limits, answerable before any device exists."""
+    from rainbow_b200 import _lib
+    lib = _lib.load()
+    assert lib.rb_head_supported(3136, 512, 51, 6, 64, 32) == 0           # canonical learner
+    assert lib.rb_head_supported(576, 256, 51, 18, 64, 32) == 0           # data-efficient learner
+    assert lib.rb_head_supported(576, 64, 101, 18, 64, 0) == 0            # forward only: acting at A 18, Z 101
+    # dh kernel: (32 (A Z | 1) + 2 A Z 8) floats of shared memory must fit in 200 KB
+    assert lib.rb_head_supported(576, 64, 59, 18, 64, 32) == 0            # 204 160 B
+    assert lib.rb_head_supported(576, 64, 60, 18, 64, 32) == -34          # 207 488 B
+    assert lib.rb_head_supported(576, 64, 101, 10, 64, 32) == 0
+    assert lib.rb_head_supported(576, 64, 101, 11, 64, 32) == -34
+    assert lib.rb_head_supported(576, 64, 101, 18, 64, 32) == -34
+    assert lib.rb_head_supported(576, 1024, 51, 6, 64, 32) == 0
+    assert lib.rb_head_supported(576, 1088, 51, 6, 64, 32) == -34         # hidden <= 1024 for the backward
+    assert lib.rb_head_supported(576, 2048, 51, 6, 64, 32) == -34
+    assert lib.rb_head_supported(576, 2048, 51, 6, 64, 0) == 0
+    assert lib.rb_head_supported(576, 1024, 51, 6, 4096, 0) == 0          # 64 row tiles x 32 layer-1 tiles = 2048 tickets
+    assert lib.rb_head_supported(576, 2048, 51, 6, 4096, 0) == -34        # 64 x 64 > 2048
+    assert lib.rb_head_supported(576, 256, 51, 6, 64, 33) == -34          # backward batch > 32
+    assert lib.rb_head_supported(576, 96, 51, 6, 64, 0) == -34            # hidden % 64
+    assert lib.rb_head_supported(48, 256, 51, 6, 64, 0) == -34            # conv_features % 32
+    assert lib.rb_head_supported(576, 256, 1, 6, 64, 0) == -22            # atoms > 1
+    assert lib.rb_head_supported(576, 256, 51, 6, -1, 0) == -22
+
+
 def test_no_cpu_fallback():
     from rainbow_b200 import RainbowB200Error, _lib
     from rainbow_b200.agent import Agent
