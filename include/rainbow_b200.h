@@ -73,7 +73,7 @@ enum {
   RB_K_TREE_UPDATE = 0, RB_K_TREE_FIND, RB_K_TREE_SAMPLE, RB_K_GATHER, RB_K_ITER_STATES, RB_K_APPEND, RB_K_C51,
   RB_K_NOISY_RESAMPLE, RB_K_NOISY_COMPOSE, RB_K_SQNORM, RB_K_CLIP_ADAM, RB_K_HEAD_FC1, RB_K_HEAD_FC2, RB_K_HEAD_LOGITS,
   RB_K_HEAD_WGRAD2, RB_K_HEAD_DH, RB_K_HEAD_BWD1, RB_K_NOISE_FACTORS, RB_K_C51_DUELING, RB_K_BIAS_GRAD, RB_K_Q_VALUES,
-  RB_K_HEAD_REDUCE1, RB_K_CONV_WGRAD, RB_KERNEL_COUNT
+  RB_K_HEAD_REDUCE1, RB_K_CONV_WGRAD, RB_K_HEAD_BWD1_WGRAD, RB_K_HEAD_BWD1_DX, RB_KERNEL_COUNT
 };
 
 int rb_abi_version(void);
@@ -242,6 +242,18 @@ int rb_head_logits(const float* z, int M, int actions, int atoms, float* q, rb_s
 #define RB_HEAD_BWD_ALL 7
 int rb_head_backward(const rb_head_params* p, const rb_head_grads* g, const float* x, const float* h, const float* dz, int B,
                      float* dh_scratch, float* dx, int relu_mask_x, int parts, rb_stream_t stream);
+
+/* What rb_head_backward_large returns for this shape with valid pointers, without touching the device: RB_OK for
+ * 1 <= B <= 512, hidden <= 1024 and the dh kernel's actions * atoms limit (the same as rb_head_backward's). */
+int rb_head_large_supported(int conv_features, int hidden, int atoms, int actions, int B);
+/* The same backward as rb_head_backward (same outputs, `parts` bits and relu_mask_x) for 1 <= B <= 512 rows: layer 1 runs
+ * as two GEMM-shaped tensor-core launches (weight gradients reduced over the batch, dx reduced over both streams' rows)
+ * instead of k_head_bwd1's single pass.  dh_scratch: float32[(B + Bp) * 2*hidden], Bp = B rounded up to a multiple of 32
+ * (dh [B][2*hidden], then its transpose [2*hidden][Bp] with the columns past B zero); at B <= 32 the layout of
+ * rb_head_backward.  It runs its own layer-1 kernels at every B.  The shape check runs before any launch: a refused call
+ * writes nothing. */
+int rb_head_backward_large(const rb_head_params* p, const rb_head_grads* g, const float* x, const float* h, const float* dz,
+                           int B, float* dh_scratch, float* dx, int relu_mask_x, int parts, rb_stream_t stream);
 
 /* agent.py:53-55 Agent.act / :110-112 evaluate_q after the network body, for M states at once: from the head output
  * z[M][atoms*(1+actions)] computes q[m][a] = sum_z support_z * softmax_z(zv + za[a] - mean_a za) (model.py:75-79) and its

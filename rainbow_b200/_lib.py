@@ -52,6 +52,8 @@ SIGNATURES = {
     "rb_head_forward": (C.c_int, [_hp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rb_head_logits": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp]),
     "rb_head_backward": (C.c_int, [_hp, _hg, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _vp]),
+    "rb_head_large_supported": (C.c_int, [_i32, _i32, _i32, _i32, _i32]),
+    "rb_head_backward_large": (C.c_int, [_hp, _hg, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _vp]),
     "rb_bias_grad": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp]),
     "rb_conv_wgrad_scratch_elems": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _i32]),
     "rb_conv_wgrad": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
@@ -119,7 +121,8 @@ def stream():
 
 KERNEL_IDS = ["tree_update", "tree_find", "tree_sample", "gather", "iter_states", "append", "c51", "noisy_resample",
               "noisy_compose", "sqnorm", "clip_adam", "head_fc1", "head_fc2", "head_logits", "head_wgrad2", "head_dh",
-              "head_bwd1", "noise_factors", "c51_dueling", "bias_grad", "q_values", "head_reduce1", "conv_wgrad"]  # order of the enum in include/rainbow_b200.h
+              "head_bwd1", "noise_factors", "c51_dueling", "bias_grad", "q_values", "head_reduce1", "conv_wgrad",
+              "head_bwd1_wgrad", "head_bwd1_dx"]  # order of the enum in include/rainbow_b200.h
 
 
 class KernelTimer:

@@ -26,7 +26,7 @@ import torch
 from . import _lib
 from .dist import GradSync
 from .memory import ReplayMemory, _SampleWorkspace
-from .model import DQN
+from .model import DQN, FusedHead
 
 
 def c51_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax,
@@ -331,7 +331,7 @@ class Agent:
     # ---- the update ------------------------------------------------------------------------------
     def _fused_path(self, B):
         on = self.online_net
-        return (self.use_fused_head and B <= 32 and on.training and on.fused_ok(2 * B, backward_batch=B) and
+        return (self.use_fused_head and on.training and on.fused_ok(2 * B, backward_batch=B) and
                 self.target_net.fused_ok(B))
 
     @staticmethod
@@ -428,7 +428,7 @@ class Agent:
                     after_loss(loss)
                     wb_done = torch.cuda.Event()
                     wb_done.record(s_ns)
-            dh = torch.empty((B + 32, 2 * on.hidden_size), dtype=torch.float32, device=self.device)   # dh, then its transpose
+            dh = torch.empty((FusedHead.dh_rows(B), 2 * on.hidden_size), dtype=torch.float32, device=self.device)   # dh, then its transpose
             dx = torch.empty_like(xs_d)
             if manual:
                 # dx comes back already masked by the last conv layer's ReLU; conv gradients are overwritten.

@@ -13,8 +13,9 @@
 // are weight-bandwidth bound at this batch size, not tensor-core work.
 //
 // Kernels: k_head_fc<MT,LAYER> (forward, split-K partials), k_head_logits (bias + dueling combine),
-//          k_head_wgrad2 / k_head_dh (layer-2 backward), k_head_bwd1 (layer-1 dW + dx, CTA-pair cluster
-//          reducing dx over distributed shared memory), k_noise_factors (Philox factor vectors).
+//          k_head_wgrad2 / k_head_dh (layer-2 backward), k_head_bwd1 (layer-1 dW + dx for B <= 32, CTA-pair cluster
+//          reducing dx over distributed shared memory), k_head_bwd1_wgrad / k_head_bwd1_dx (layer-1 dW and dx for
+//          B <= 512 as two tensor-core GEMMs), k_noise_factors (Philox factor vectors).
 
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
@@ -504,12 +505,13 @@ k_head_wgrad2(const __grid_constant__ HeadDesc d, const __grid_constant__ HeadGr
 }
 
 // Layer-2 backward, input gradient with the ReLU mask of layer 1 folded in:
-// dh[m][s*H + k] = (h > 0) * sum_o dz[m][col(o)] * W2_s[o][k].   B <= 32 rows.
+// dh[m][s*H + k] = (h > 0) * sum_o dz[m][col(o)] * W2_s[o][k].
 // The layer is tiny (1.5 MB of weights) and sits on the critical path between the loss and the layer-1 backward, so the
-// kernel is organised around ONE memory round trip: grid = 2 streams x H/8 CTAs; a CTA stages the stream's whole dz block
-// [32][Ns] and its 8-column slab of W2 (mu and sigma rows, 32 contiguous bytes each) with cp.async, all in flight at once,
-// composes the noisy weights in place, and thread (m, k) runs one Ns-long dot product out of shared memory.
-// Writes dh [B][2H] and its transpose dhT [2H][32] (rows past B zero) for k_head_bwd1.
+// kernel is organised around ONE memory round trip: grid = 2 streams x H/8 CTAs x 32-row batch tiles; a CTA stages its
+// tile's dz block [32][Ns] and its 8-column slab of W2 (mu and sigma rows, 32 contiguous bytes each) with cp.async, all in
+// flight at once, composes the noisy weights in place, and thread (m, k) runs one Ns-long dot product out of shared memory.
+// Writes dh [B][2H] and its transpose dhT [2H][ldT] (ldT = B rounded up to 32, columns past B zero) for the layer-1
+// kernels; at B <= 32 that is one batch tile and ldT = 32.
 constexpr int DH_KB = 8;    // hidden units per CTA
 constexpr int DH_T = 256;   // 32 batch rows x 8 hidden units
 
@@ -525,10 +527,15 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.com
 
 __global__ void __launch_bounds__(DH_T)
 k_head_dh(const __grid_constant__ HeadDesc d, const float* __restrict__ dz, const float* __restrict__ h, int B,
-          float* __restrict__ dh, float* __restrict__ dhT, int ld_dz) {
+          float* __restrict__ dh, float* __restrict__ dhT, int ld_dz, int ldT) {
   extern __shared__ __align__(16) float smem_dh[];
-  const int s = blockIdx.y, k0 = blockIdx.x * DH_KB;
+  const int s = blockIdx.y, k0 = blockIdx.x * DH_KB, m0 = blockIdx.z * 32;
   const int Ns = n2_of(d, s), colbase = col2_of(d, s), ncols = d.Z + d.A * d.Z, H = d.H;
+  dz += (size_t)m0 * ncols;                             // this CTA's 32-row batch tile
+  h += (size_t)m0 * (2 * H);
+  dh += (size_t)m0 * (2 * H);
+  dhT += m0;
+  B = min(B - m0, 32);
   float* Dz = smem_dh;                                  // [32][ld_dz]   dz block of this stream
   float* Wm = Dz + 32 * ld_dz;                          // [Ns][DH_KB]   mu slab, composed in place
   float* Wsg = Wm + (size_t)((Ns + 3) & ~3) * DH_KB;    // [Ns][DH_KB]   sigma slab
@@ -595,7 +602,7 @@ k_head_dh(const __grid_constant__ HeadDesc d, const float* __restrict__ dz, cons
   }
   const float v = (m < B && hv > 0.f) ? ((a0 + a1) + (a2 + a3)) : 0.0f;
   if (m < B) dh[(size_t)m * (2 * H) + s * H + k0 + k] = v;
-  dhT[(size_t)(s * H + k0 + k) * 32 + m] = v;
+  dhT[(size_t)(s * H + k0 + k) * ldT + m] = v;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -813,6 +820,255 @@ k_head_bwd1(const __grid_constant__ HeadDesc d, const __grid_constant__ HeadGrad
 }
 
 // ------------------------------------------------------------------------------------------------
+// Layer-1 backward for 1 <= B <= 512 rows (rb_head_backward_large).  At these batch sizes the two products are real GEMMs
+// (3.3 GFLOP each at conv_features 3136, hidden 512, B 512), and the dh chunk alone would need 128 KB per ring stage in
+// k_head_bwd1's one-pass structure, so they run as two launches, both as error-compensated TF32 on mma.sync (the same
+// arithmetic as k_head_bwd1) with fp32 accumulation:
+//   k_head_bwd1_wgrad: g[o][k] = sum_m dhT[o][m] * x[m][k] per stream, g_sigma = g * eps_out[o] eps_in[k]; CTA tile
+//                      64 o x 64 k; the batch is reduced in 32-row steps through a 3-stage cp.async ring, inside the CTA in
+//                      a fixed order (no atomics, no split across CTAs).  The k-tile-0 CTAs also write the bias gradients.
+//   k_head_bwd1_dx:    dx[m][k] = sum_s sum_o dh[m][s*H + o] * W1_s[o][k]; CTA tile 64 m x 64 k; the 2H weight rows are
+//                      reduced in 32-row chunks, W = mu + sigma * (eps_out (outer) eps_in) composed in place as the chunks
+//                      land.  blockIdx.x walks the m tiles, so the CTAs that read the same W1 columns are resident together
+//                      and all but the first find them in L2 (W1 mu + sigma is 25.7 MB at conv_features 3136, hidden 512).
+// Operands are read straight from k_head_dh's dh [B][2H] and dhT [2H][Bp] (Bp = B rounded up to 32, columns past B zero),
+// x [B][K1] and W1 [H][K1]: for mma.sync every tile is staged in its natural orientation, nothing is transposed.
+// 128 threads = 4 warps in a 2 x 2 grid of 32 x 32 warp tiles (2 x 4 mma.m16n8k8 blocks each).
+// ------------------------------------------------------------------------------------------------
+constexpr int BL_T = 128;        // threads
+constexpr int BL_MT = 64;        // output rows per CTA (o for the weight gradient, m for dx)
+constexpr int BL_NT = 64;        // output columns per CTA (k)
+constexpr int BL_R = 32;         // reduction rows per ring stage
+constexpr int BL_STAGES = 3;
+constexpr int BL_MAX_B = 512;
+constexpr int BL_LDA = BL_R + 4;     // A tiles [row][r]: stride = 4 (mod 32), conflict-free fragment loads
+constexpr int BL_LDB = BL_NT + 8;    // B tiles [r][k]:   stride = 8 (mod 32)
+constexpr int BLW_STAGE = BL_MT * BL_LDA + BL_R * BL_LDB;       // floats per stage: dhT tile | x tile
+constexpr int BLX_STAGE = BL_MT * BL_LDA + 2 * BL_R * BL_LDB;   // floats per stage: dh tile | W mu (composed in place) | W sigma
+
+// acc += A [32 rows][BL_R] x B [BL_R][32 columns] of one warp tile, 3xTF32 (lo*hi, hi*lo, hi*hi per block, as mma3_block).
+// A: row stride BL_LDA, rows = output rows.  B: row stride BL_LDB, rows = reduction index.  acc[mb][nb]: 16-row block mb,
+// 8-column block nb (C fragment: rows gid, gid + 8; columns 2 tig, 2 tig + 1).  The stage's product is accumulated on its
+// own and then added to acc in fp32: the tensor cores accumulate coarser than round-to-nearest, and a chain of 768 MMAs
+// into one accumulator (dx at hidden 1024) came within 4 % of the bound the tests hold dx to on an H100.
+__device__ __forceinline__ void bl_mma_stage(float (&acc)[2][4][4], const float* A, const float* Bt, int gid, int tig) {
+  float part[2][4][4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) part[i][j][q] = 0.0f;
+#pragma unroll
+  for (int ks = 0; ks < BL_R / 8; ++ks) {
+    uint32_t ahi[2][4], alo[2][4], bhi[4][2], blo[4][2];
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+      const float* a = A + (16 * mb) * BL_LDA + 8 * ks;
+      tf32_split(a[gid * BL_LDA + tig], ahi[mb][0], alo[mb][0]);
+      tf32_split(a[(gid + 8) * BL_LDA + tig], ahi[mb][1], alo[mb][1]);
+      tf32_split(a[gid * BL_LDA + tig + 4], ahi[mb][2], alo[mb][2]);
+      tf32_split(a[(gid + 8) * BL_LDA + tig + 4], ahi[mb][3], alo[mb][3]);
+    }
+#pragma unroll
+    for (int nb = 0; nb < 4; ++nb) {
+      tf32_split(Bt[(8 * ks + tig) * BL_LDB + 8 * nb + gid], bhi[nb][0], blo[nb][0]);
+      tf32_split(Bt[(8 * ks + tig + 4) * BL_LDB + 8 * nb + gid], bhi[nb][1], blo[nb][1]);
+    }
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+      for (int nb = 0; nb < 4; ++nb) {
+        mma_tf32(part[mb][nb], alo[mb], bhi[nb]);
+        mma_tf32(part[mb][nb], ahi[mb], blo[nb]);
+        mma_tf32(part[mb][nb], ahi[mb], bhi[nb]);
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[i][j][q] += part[i][j][q];
+}
+
+// grid = (ceil(K1 / 64), 2H / 64): blockIdx.y = 64-row tile of both streams' W1 rows (hidden % 64 == 0: never straddles)
+__global__ void __launch_bounds__(BL_T)
+k_head_bwd1_wgrad(const __grid_constant__ HeadDesc d, const __grid_constant__ HeadGrads g, const float* __restrict__ x,
+                  const float* __restrict__ dhT, int B, int Bp) {
+  extern __shared__ __align__(16) float bl_ring[];   // [BL_STAGES][BLW_STAGE]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
+  const int wr = (warp >> 1) * 32, wc = (warp & 1) * 32;   // warp tile origin in the CTA tile
+  const int K = d.K1, H = d.H;
+  const int k0 = blockIdx.x * BL_NT, r0 = blockIdx.y * BL_MT, s = r0 / H, o0 = r0 - s * H;
+  const int n_steps = Bp / BL_R;
+  auto As = [&](int st) { return bl_ring + (size_t)st * BLW_STAGE; };                    // dhT tile [o][m]
+  auto Bs = [&](int st) { return bl_ring + (size_t)st * BLW_STAGE + BL_MT * BL_LDA; };   // x tile [m][k]
+  auto issue = [&](int c) {   // batch step c -> stage c % BL_STAGES (always commits, possibly an empty group)
+    if (c < n_steps) {
+      const int st = c % BL_STAGES, mb = c * BL_R;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {   // dhT [64 o][32 m]: columns past B are zeros k_head_dh wrote
+        const int idx = tid + j * BL_T, row = idx >> 3, cc = (idx & 7) * 4;
+        cp_async16_zfill(As(st) + row * BL_LDA + cc, dhT + (size_t)(r0 + row) * Bp + mb + cc, true);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {   // x [32 m][64 k]: rows past B and columns past K1 zero-filled
+        const int idx = tid + j * BL_T, row = idx >> 4, cc = (idx & 15) * 4, m = mb + row, k = k0 + cc;
+        const bool ok = m < B && k < K;
+        cp_async16_zfill(Bs(st) + row * BL_LDB + cc, ok ? x + (size_t)m * K + k : x, ok);
+      }
+    }
+    cp_async_commit();
+  };
+  float acc[2][4][4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[i][j][q] = 0.0f;
+  float bsum = 0.0f;   // bias gradient (k-tile-0 CTAs): thread t sums row t / 2, columns 16 (t % 2) .. + 15 of every step
+#pragma unroll
+  for (int c = 0; c < BL_STAGES - 1; ++c) issue(c);
+  for (int c = 0; c < n_steps; ++c) {
+    const int st = c % BL_STAGES;
+    cp_async_wait<BL_STAGES - 2>();   // this thread's copies of step c have landed ...
+    __syncthreads();                  // ... and everybody else's; everybody is also done with step c - 1
+    issue(c + BL_STAGES - 1);         // overwrites the stage step c - 1 used
+    bl_mma_stage(acc, As(st) + wr * BL_LDA, Bs(st) + wc, gid, tig);
+    if (blockIdx.x == 0) {
+      const float* rowp = As(st) + (tid >> 1) * BL_LDA + (tid & 1) * 16;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) bsum += rowp[j];
+    }
+  }
+  cp_async_wait<0>();
+  const float* ei = d.ei1[s];
+  const float* eo = d.eo1[s];
+#pragma unroll
+  for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+    for (int hrow = 0; hrow < 2; ++hrow) {
+      const int o = o0 + wr + 16 * mb + gid + 8 * hrow;
+      const float e = eo ? __ldg(eo + o) : 0.0f;
+#pragma unroll
+      for (int nb = 0; nb < 4; ++nb) {
+        const int k = k0 + wc + 8 * nb + 2 * tig;   // K1 % 32 == 0: k + 1 < K1 whenever k < K1
+        if (k >= K) continue;
+        const size_t off = (size_t)o * K + k;
+        const float g0 = acc[mb][nb][2 * hrow], g1 = acc[mb][nb][2 * hrow + 1];
+        __stcs(reinterpret_cast<float2*>(g.w1_mu[s] + off), make_float2(g0, g1));
+        const float e0 = ei ? __ldg(ei + k) : 0.0f, e1 = ei ? __ldg(ei + k + 1) : 0.0f;
+        __stcs(reinterpret_cast<float2*>(g.w1_sig[s] + off), make_float2(g0 * (e * e0), g1 * (e * e1)));
+      }
+    }
+  if (blockIdx.x == 0) {
+    const float other = __shfl_xor_sync(0xffffffffu, bsum, 1);
+    if ((tid & 1) == 0) {
+      const int o = o0 + (tid >> 1);
+      const float b = bsum + other;
+      g.b1_mu[s][o] = b;
+      g.b1_sig[s][o] = eo ? b * __ldg(eo + o) : 0.0f;
+    }
+  }
+}
+
+// grid = (ceil(B / 64), ceil(K1 / 64))
+__global__ void __launch_bounds__(BL_T)
+k_head_bwd1_dx(const __grid_constant__ HeadDesc d, const float* __restrict__ x, const float* __restrict__ dh, int B,
+               float* __restrict__ dx, int relu_mask_x) {
+  extern __shared__ __align__(16) float bl_ring[];   // [BL_STAGES][BLX_STAGE]
+  __shared__ float EoAll[2 * 1024];                  // eps_out of both streams' rows (hidden <= 1024), fetched once
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
+  const int wr = (warp >> 1) * 32, wc = (warp & 1) * 32;
+  const int K = d.K1, H = d.H;
+  const int m0 = blockIdx.x * BL_MT, k0 = blockIdx.y * BL_NT;
+  const int n_chunks = 2 * H / BL_R;
+  const bool noisy = d.ei1[0] != nullptr;
+  auto Ds = [&](int st) { return bl_ring + (size_t)st * BLX_STAGE; };                                  // dh tile [m][o]
+  auto Wm = [&](int st) { return bl_ring + (size_t)st * BLX_STAGE + BL_MT * BL_LDA; };                 // W mu [o][k]
+  auto Wsg = [&](int st) { return bl_ring + (size_t)st * BLX_STAGE + BL_MT * BL_LDA + BL_R * BL_LDB; }; // W sigma [o][k]
+  auto issue = [&](int c) {   // chunk c of the 2H rows -> stage c % BL_STAGES (always commits)
+    if (c < n_chunks) {
+      const int st = c % BL_STAGES, r = c * BL_R, s = r / H, o = r - s * H;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {   // dh [64 m][32 o]: rows past B zero-filled
+        const int idx = tid + j * BL_T, row = idx >> 3, cc = (idx & 7) * 4, m = m0 + row;
+        const bool ok = m < B;
+        cp_async16_zfill(Ds(st) + row * BL_LDA + cc, ok ? dh + (size_t)m * (2 * H) + r + cc : dh, ok);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {   // W1 rows [32 o][64 k]: columns past K1 zero-filled
+        const int idx = tid + j * BL_T, row = idx >> 4, cc = (idx & 15) * 4, k = k0 + cc;
+        const bool ok = k < K;
+        const size_t off = (size_t)(o + row) * K + k;
+        cp_async16_zfill(Wm(st) + row * BL_LDB + cc, ok ? d.w1_mu[s] + off : d.w1_mu[s], ok);
+        if (noisy) cp_async16_zfill(Wsg(st) + row * BL_LDB + cc, ok ? d.w1_sig[s] + off : d.w1_sig[s], ok);
+      }
+    }
+    cp_async_commit();
+  };
+#pragma unroll
+  for (int c = 0; c < BL_STAGES - 1; ++c) issue(c);
+  for (int i = tid; i < 2 * H; i += BL_T) EoAll[i] = noisy ? __ldg(d.eo1[i / H] + (i % H)) : 0.0f;
+  const int ccol = (tid & 15) * 4;   // the 4 columns every thread composes (BL_T % 16 == 0: the same in each of its chunks)
+  float4 e4s[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+  if (noisy && k0 + ccol < K) {
+    e4s[0] = __ldg(reinterpret_cast<const float4*>(d.ei1[0] + k0 + ccol));
+    e4s[1] = __ldg(reinterpret_cast<const float4*>(d.ei1[1] + k0 + ccol));
+  }
+  float acc[2][4][4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[i][j][q] = 0.0f;
+  for (int c = 0; c < n_chunks; ++c) {
+    const int st = c % BL_STAGES;
+    cp_async_wait<BL_STAGES - 2>();
+    __syncthreads();                  // chunk c complete everywhere (and EoAll, at c = 0); chunk c - 1 consumed
+    issue(c + BL_STAGES - 1);
+    if (noisy) {                      // W = mu + sigma * (eps_out[o] * eps_in[k]) in place   (model.py:39,43)
+      const float4 ek = ((c * BL_R) / H) ? e4s[1] : e4s[0];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int row = (tid + j * BL_T) >> 4;
+        float4 w = *reinterpret_cast<const float4*>(Wm(st) + row * BL_LDB + ccol);
+        const float4 sg4 = *reinterpret_cast<const float4*>(Wsg(st) + row * BL_LDB + ccol);
+        const float e = EoAll[c * BL_R + row];
+        w.x = fmaf(sg4.x, e * ek.x, w.x); w.y = fmaf(sg4.y, e * ek.y, w.y);
+        w.z = fmaf(sg4.z, e * ek.z, w.z); w.w = fmaf(sg4.w, e * ek.w, w.w);
+        *reinterpret_cast<float4*>(Wm(st) + row * BL_LDB + ccol) = w;
+      }
+      __syncthreads();
+    }
+    bl_mma_stage(acc, Ds(st) + wr * BL_LDA, Wm(st) + wc, gid, tig);
+  }
+  cp_async_wait<0>();
+#pragma unroll
+  for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+    for (int hrow = 0; hrow < 2; ++hrow) {
+      const int m = m0 + wr + 16 * mb + gid + 8 * hrow;
+      if (m >= B) continue;
+#pragma unroll
+      for (int nb = 0; nb < 4; ++nb) {
+        const int k = k0 + wc + 8 * nb + 2 * tig;
+        if (k >= K) continue;
+        float2 o2 = make_float2(acc[mb][nb][2 * hrow], acc[mb][nb][2 * hrow + 1]);
+        if (relu_mask_x) {  // x = relu(conv output): fold that ReLU's backward in (x > 0 <=> pre-activation > 0)
+          const float2 xv = __ldg(reinterpret_cast<const float2*>(x + (size_t)m * K + k));
+          o2.x = xv.x > 0.f ? o2.x : 0.f;
+          o2.y = xv.y > 0.f ? o2.y : 0.f;
+        }
+        *reinterpret_cast<float2*>(dx + (size_t)m * K + k) = o2;
+      }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Factor vectors f(eps_in), f(eps_out) of every NoisyLinear of a net: one CTA, same Philox indexing as
 // k_noisy_resample (normal g of stream `which` for draw `ctr`), so factors + outer product == K6.
 // ------------------------------------------------------------------------------------------------
@@ -990,10 +1246,10 @@ k_conv_wgrad_reduce(const float* __restrict__ part, int n_part, int n_w, int n_b
   }
 }
 
-// Every shape limit of rb_head_forward (rows > 0) and rb_head_backward (backward: over bwd_batch rows), checked before
-// anything is launched; rb_head_supported exports it so callers can pick another path instead of meeting the error
-// mid-update.
-int head_shape_check(int K1, int H, int Z, int A, int rows, int bwd_batch, bool backward) {
+// Every shape limit of rb_head_forward (rows > 0) and rb_head_backward (backward: over bwd_batch rows; large: the limits
+// of rb_head_backward_large instead), checked before anything is launched; rb_head_supported / rb_head_large_supported
+// export it so callers can pick another path instead of meeting the error mid-update.
+int head_shape_check(int K1, int H, int Z, int A, int rows, int bwd_batch, bool backward, bool large = false) {
   if (K1 <= 0 || H <= 0 || Z <= 1 || A <= 0 || rows < 0) return rbi::fail(RB_ERR_INVAL, "rb_head: bad size");
   if (K1 % 32 || H % 64) return rbi::fail(RB_ERR_RANGE, "rb_head: conv_features % 32 == 0 and hidden % 64 == 0 required");
   if (rows > 0) {
@@ -1003,8 +1259,10 @@ int head_shape_check(int K1, int H, int Z, int A, int rows, int bwd_batch, bool 
     if (mt > 65535 || mt * tiles1 > 2048 || mt * tiles2 > 2048) return rbi::fail(RB_ERR_RANGE, "rb_head_forward: too many rows");
   }
   if (backward) {
-    if (bwd_batch <= 0 || bwd_batch > 32)
-      return rbi::fail(RB_ERR_RANGE, "rb_head_backward: 1 <= B <= 32 required (larger batches use the library GEMM path)");
+    if (large && (bwd_batch <= 0 || bwd_batch > BL_MAX_B))
+      return rbi::fail(RB_ERR_RANGE, "rb_head_backward_large: 1 <= B <= 512 required");
+    if (!large && (bwd_batch <= 0 || bwd_batch > 32))
+      return rbi::fail(RB_ERR_RANGE, "rb_head_backward: 1 <= B <= 32 required (rb_head_backward_large takes up to 512)");
     const long long ns_max = (long long)A * Z > Z ? (long long)A * Z : Z;
     const long long ld_dz = ns_max | 1;
     const long long smem = (32 * ld_dz + 2 * ((ns_max + 3) & ~3ll) * DH_KB) * (long long)sizeof(float);
@@ -1033,6 +1291,51 @@ int head_check(const rb_head_params* p, const char* who) {
     if (bits & 15) return rbi::fail(RB_ERR_INVAL, "rb_head: weight / bias / factor pointers must be 16-byte aligned");
   }
   return RB_OK;
+}
+
+// The checks and gradient pointers both backward entry points share; the shape check runs before anything is launched.
+int head_bwd_prepare(const rb_head_params* p, const rb_head_grads* gr, const float* x, const float* h, const float* dz, int B,
+                     const float* dh_scratch, const float* dx, int parts, bool large, HeadGrads* g) {
+  const char* who = large ? "rb_head_backward_large: null pointer or bad size" : "rb_head_backward: null pointer or bad size";
+  int rc = head_check(p, who);
+  if ((parts & 7) == 0) return rbi::fail(RB_ERR_INVAL, "rb_head_backward: parts must select at least one of RB_HEAD_BWD_*");
+  if (rc != RB_OK) return rc;
+  if (!gr || !x || !h || !dz || !dh_scratch || !dx) return rbi::fail(RB_ERR_INVAL, "rb_head_backward: null pointer");
+  rc = head_shape_check(p->conv_features, p->hidden, p->atoms, p->actions, 0, B, true, large);   // all limits, whatever `parts` selects
+  if (rc != RB_OK) return rc;
+  for (int s = 0; s < 2; ++s) {
+    if (!gr->w1_mu[s] || !gr->w1_sigma[s] || !gr->b1_mu[s] || !gr->b1_sigma[s] || !gr->w2_mu[s] || !gr->w2_sigma[s] ||
+        !gr->b2_mu[s] || !gr->b2_sigma[s])
+      return rbi::fail(RB_ERR_INVAL, "rb_head_backward: null gradient pointer");
+    g->w1_mu[s] = gr->w1_mu[s]; g->w1_sig[s] = gr->w1_sigma[s]; g->b1_mu[s] = gr->b1_mu[s]; g->b1_sig[s] = gr->b1_sigma[s];
+    g->w2_mu[s] = gr->w2_mu[s]; g->w2_sig[s] = gr->w2_sigma[s]; g->b2_mu[s] = gr->b2_mu[s]; g->b2_sig[s] = gr->b2_sigma[s];
+  }
+  return RB_OK;
+}
+
+// Layer-2 launches of both backward entry points: k_head_wgrad2 (any B) and k_head_dh over ceil(B / 32) batch tiles,
+// writing dh [B][2H] and dhT [2H][ldT] to dh_scratch.
+int head_bwd_layer2(const HeadDesc& d, const HeadGrads& g, const float* dz, const float* h, int B, float* dh_scratch, int ldT,
+                    int parts, cudaStream_t st) {
+  if (parts & RB_HEAD_BWD_WGRAD2) {
+    const int tiles = (d.Z + NT - 1) / NT + (d.A * d.Z + NT - 1) / NT;
+    dim3 grid(tiles, d.H / NT);
+    rbi::ProfScope prof_(RB_K_HEAD_WGRAD2, st);
+    k_head_wgrad2<<<grid, HT, 0, st>>>(d, g, dz, h, B);
+  }
+  int rc = rbi::check_launch("rb_head_backward(wgrad2)");
+  if (rc != RB_OK) return rc;
+  if (parts & RB_HEAD_BWD_DH) {
+    const int ns_max = d.A * d.Z > d.Z ? d.A * d.Z : d.Z;
+    const int ld_dz = ns_max | 1;                       // odd row stride: the 32 rows of a column hit 32 different banks
+    const size_t smem = ((size_t)32 * ld_dz + 2 * (size_t)((ns_max + 3) & ~3) * DH_KB) * sizeof(float);   // <= 200 KB: head_shape_check
+    rc = rbi::ensure_dynamic_smem(k_head_dh, smem, "rb_head_backward");
+    if (rc != RB_OK) return rc;
+    dim3 grid(d.H / DH_KB, 2, (B + 31) / 32);
+    rbi::ProfScope prof_(RB_K_HEAD_DH, st);
+    k_head_dh<<<grid, DH_T, smem, st>>>(d, dz, h, B, dh_scratch, dh_scratch + (size_t)B * 2 * d.H, ld_dz, ldT);
+  }
+  return rbi::check_launch("rb_head_backward(dh)");
 }
 
 void head_splits(int K1, int H, int* s1, int* s2, int* ks1, int* ks2) {
@@ -1143,41 +1446,12 @@ int rb_head_logits(const float* z, int M, int actions, int atoms, float* q, rb_s
 
 int rb_head_backward(const rb_head_params* p, const rb_head_grads* gr, const float* x, const float* h, const float* dz, int B,
                      float* dh_scratch, float* dx, int relu_mask_x, int parts, rb_stream_t stream) {
-  int rc = head_check(p, "rb_head_backward: null pointer or bad size");
-  if ((parts & 7) == 0) return rbi::fail(RB_ERR_INVAL, "rb_head_backward: parts must select at least one of RB_HEAD_BWD_*");
-  if (rc != RB_OK) return rc;
-  if (!gr || !x || !h || !dz || !dh_scratch || !dx) return rbi::fail(RB_ERR_INVAL, "rb_head_backward: null pointer");
-  rc = head_shape_check(p->conv_features, p->hidden, p->atoms, p->actions, 0, B, true);   // all limits, whatever `parts` selects
-  if (rc != RB_OK) return rc;
   HeadGrads g;
-  for (int s = 0; s < 2; ++s) {
-    if (!gr->w1_mu[s] || !gr->w1_sigma[s] || !gr->b1_mu[s] || !gr->b1_sigma[s] || !gr->w2_mu[s] || !gr->w2_sigma[s] ||
-        !gr->b2_mu[s] || !gr->b2_sigma[s])
-      return rbi::fail(RB_ERR_INVAL, "rb_head_backward: null gradient pointer");
-    g.w1_mu[s] = gr->w1_mu[s]; g.w1_sig[s] = gr->w1_sigma[s]; g.b1_mu[s] = gr->b1_mu[s]; g.b1_sig[s] = gr->b1_sigma[s];
-    g.w2_mu[s] = gr->w2_mu[s]; g.w2_sig[s] = gr->w2_sigma[s]; g.b2_mu[s] = gr->b2_mu[s]; g.b2_sig[s] = gr->b2_sigma[s];
-  }
+  int rc = head_bwd_prepare(p, gr, x, h, dz, B, dh_scratch, dx, parts, false, &g);
+  if (rc != RB_OK) return rc;
   const HeadDesc d = to_desc(p);
   cudaStream_t st = (cudaStream_t)stream;
-  if (parts & RB_HEAD_BWD_WGRAD2) {
-    const int tiles = (d.Z + NT - 1) / NT + (d.A * d.Z + NT - 1) / NT;
-    dim3 grid(tiles, d.H / NT);
-    rbi::ProfScope prof_(RB_K_HEAD_WGRAD2, st);
-    k_head_wgrad2<<<grid, HT, 0, st>>>(d, g, dz, h, B);
-  }
-  rc = rbi::check_launch("rb_head_backward(wgrad2)");
-  if (rc != RB_OK) return rc;
-  if (parts & RB_HEAD_BWD_DH) {
-    const int ns_max = d.A * d.Z > d.Z ? d.A * d.Z : d.Z;
-    const int ld_dz = ns_max | 1;                       // odd row stride: the 32 rows of a column hit 32 different banks
-    const size_t smem = ((size_t)32 * ld_dz + 2 * (size_t)((ns_max + 3) & ~3) * DH_KB) * sizeof(float);   // <= 200 KB: head_shape_check
-    rc = rbi::ensure_dynamic_smem(k_head_dh, smem, "rb_head_backward");
-    if (rc != RB_OK) return rc;
-    dim3 grid(d.H / DH_KB, 2);
-    rbi::ProfScope prof_(RB_K_HEAD_DH, st);
-    k_head_dh<<<grid, DH_T, smem, st>>>(d, dz, h, B, dh_scratch, dh_scratch + (size_t)B * 2 * d.H, ld_dz);
-  }
-  rc = rbi::check_launch("rb_head_backward(dh)");
+  rc = head_bwd_layer2(d, g, dz, h, B, dh_scratch, 32, parts, st);
   if (rc != RB_OK) return rc;
   if (parts & RB_HEAD_BWD_LAYER1) {   // hidden <= 1024 (EoAll holds H / 2 factors): head_shape_check
     dim3 grid(d.K1 / B1_K, 4);
@@ -1188,6 +1462,42 @@ int rb_head_backward(const rb_head_params* p, const rb_head_grads* gr, const flo
     k_head_bwd1<<<grid, B1_T, smem_b1, st>>>(d, g, x, dh_scratch, dh_scratch + (size_t)B * 2 * d.H, B, dx, relu_mask_x);
   }
   return rbi::check_launch("rb_head_backward(bwd1)");
+}
+
+int rb_head_large_supported(int conv_features, int hidden, int atoms, int actions, int B) {
+  return head_shape_check(conv_features, hidden, atoms, actions, 0, B, true, true);
+}
+
+int rb_head_backward_large(const rb_head_params* p, const rb_head_grads* gr, const float* x, const float* h, const float* dz,
+                           int B, float* dh_scratch, float* dx, int relu_mask_x, int parts, rb_stream_t stream) {
+  HeadGrads g;
+  int rc = head_bwd_prepare(p, gr, x, h, dz, B, dh_scratch, dx, parts, true, &g);
+  if (rc != RB_OK) return rc;
+  const HeadDesc d = to_desc(p);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Bp = (B + BL_R - 1) / BL_R * BL_R;
+  rc = head_bwd_layer2(d, g, dz, h, B, dh_scratch, Bp, parts, st);
+  if (rc != RB_OK) return rc;
+  if (parts & RB_HEAD_BWD_LAYER1) {   // hidden <= 1024 (k_head_bwd1_dx's EoAll holds 2H factors): head_shape_check
+    const float* dhT = dh_scratch + (size_t)B * 2 * d.H;
+    const size_t smem_w = (size_t)BL_STAGES * BLW_STAGE * sizeof(float);
+    const size_t smem_x = (size_t)BL_STAGES * BLX_STAGE * sizeof(float);
+    rc = rbi::ensure_dynamic_smem(k_head_bwd1_wgrad, smem_w, "rb_head_backward_large");
+    if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_head_bwd1_dx, smem_x, "rb_head_backward_large");
+    if (rc != RB_OK) return rc;
+    const int ktiles = (d.K1 + BL_NT - 1) / BL_NT;
+    {
+      rbi::ProfScope prof_(RB_K_HEAD_BWD1_WGRAD, st);
+      k_head_bwd1_wgrad<<<dim3(ktiles, 2 * d.H / BL_MT), BL_T, smem_w, st>>>(d, g, x, dhT, B, Bp);
+    }
+    rc = rbi::check_launch("rb_head_backward_large(wgrad1)");
+    if (rc != RB_OK) return rc;
+    {
+      rbi::ProfScope prof_(RB_K_HEAD_BWD1_DX, st);
+      k_head_bwd1_dx<<<dim3((B + BL_MT - 1) / BL_MT, ktiles), BL_T, smem_x, st>>>(d, x, dh_scratch, B, dx, relu_mask_x);
+    }
+  }
+  return rbi::check_launch("rb_head_backward_large(dx)");
 }
 
 int rb_bias_grad(const float* grad_out, int B, int C, int HW, float* out, rb_stream_t stream) {
