@@ -315,7 +315,10 @@ void orc_c51(const float* q_on_s, const float* q_on_ns, const float* q_tg_ns, co
       m[z] = 0.0f;
     }
     for (int z = 0; z < Z; ++z) m[l[z]] += pt[z] * ((float)u[z] - bb[z]);
-    for (int z = 0; z < Z; ++z) m[u[z]] += pt[z] * (bb[z] - (float)l[z]);
+    /* fp32 rounding can put b just past Z - 1 at Tz = Vmax (e.g. Z 62 with V +-1): u = Z, outside m.  That
+     * contribution, pt * (b - l), is within the rounding of b; it is dropped, as the kernel drops it. */
+    for (int z = 0; z < Z; ++z)
+      if (u[z] < Z) m[u[z]] += pt[z] * (bb[z] - (float)l[z]);
     float ce = 0.0f, msum = 0.0f;
     for (int z = 0; z < Z; ++z) {
       ce += m[z] * logp[z];

@@ -133,9 +133,14 @@ def q_values(z, A, Z, support):
     (L_z = their scale).  A term of the warp's sums passes at most 9 roundings (4 per lane for Z <= 128, 5 shuffle
     levels) and expf is within 2 ulp, so the worst case of those errors is about 11.5 u sum_z p (|s| + |ev|) = 5.75 u of
     this scale (u = 2^-24), below TAU = 8.4 u."""
-    q, L = _dueling(z, A, Z)
-    pz = torch.softmax(q, dim=2)
-    s = _d(support).view(1, 1, Z)
+    return expectation(*_dueling(z, A, Z), support)
+
+
+def expectation(q, L, support):
+    """Expected value over the support of softmax_z(q) [M][A] of logits q [M][A][Z] known to u L, and its scale (see
+    q_values)."""
+    pz = torch.softmax(_d(q), dim=2)
+    s = _d(support).view(1, 1, -1)
     ev = (pz * s).sum(2)
     evx = ev.unsqueeze(2)
     scale = 2 * (pz * (s.abs() + evx.abs())).sum(2) + (pz * (s - evx).abs() * L).sum(2)
