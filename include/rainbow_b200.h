@@ -73,7 +73,7 @@ enum {
   RB_K_TREE_UPDATE = 0, RB_K_TREE_FIND, RB_K_TREE_SAMPLE, RB_K_GATHER, RB_K_ITER_STATES, RB_K_APPEND, RB_K_C51,
   RB_K_NOISY_RESAMPLE, RB_K_NOISY_COMPOSE, RB_K_SQNORM, RB_K_CLIP_ADAM, RB_K_HEAD_FC1, RB_K_HEAD_FC2, RB_K_HEAD_LOGITS,
   RB_K_HEAD_WGRAD2, RB_K_HEAD_DH, RB_K_HEAD_BWD1, RB_K_NOISE_FACTORS, RB_K_C51_DUELING, RB_K_BIAS_GRAD, RB_K_Q_VALUES,
-  RB_K_HEAD_REDUCE1, RB_K_CONV_WGRAD, RB_K_HEAD_BWD1_WGRAD, RB_K_HEAD_BWD1_DX, RB_KERNEL_COUNT
+  RB_K_HEAD_REDUCE1, RB_K_CONV_WGRAD, RB_K_HEAD_BWD1_WGRAD, RB_K_HEAD_BWD1_DX, RB_K_LEARN_STATS, RB_KERNEL_COUNT
 };
 
 int rb_abi_version(void);
@@ -332,6 +332,47 @@ int rb_peer_clip_adam(const float* const* peer_grad, float* const* peer_param, u
                       double* const* peer_norms, int world, int rank, int64_t P, float* gred, float* exp_avg,
                       float* exp_avg_sq, float grad_scale, float max_norm, float lr, float beta1, float beta2, float eps,
                       int64_t* step_count, uint64_t* epoch, void* scratch, float* norm_out, rb_stream_t stream);
+
+/* Learner statistics of one update (agent.py:66-98 computes most of them and discards them), recorded on the device.
+ * One record, 48 bytes; i runs over the B samples of the batch:
+ *   update       running index of the record (the value of *counter when it was written)
+ *   loss_mean    mean_i loss_i, loss_i = -sum_z m_iz log p_iz (agent.py:94; the TD priority before ^omega)
+ *   loss_max     max_i loss_i
+ *   objective    mean_i w_i loss_i (agent.py:96)
+ *   q_mean       mean_i sum_z softmax(q(s_i, a_i))_z support_z, the online logits of the taken action
+ *   target_mean  mean_i sum_z m_iz support_z
+ *   edge_mass    mean_i (m_i,0 + m_i,Z-1), the projected mass the clamp to [Vmin, Vmax] piles onto the end atoms
+ *   weight_min   min_i w_i
+ *   grad_norm    *grad_norm (the pre-clip norm written by rb_clip_adam / rb_peer_adam_gather as norm_out)
+ *   clip_coef    min(1, max_norm / (grad_norm + 1e-6)), the factor rb_clip_adam scaled the gradient by
+ *   applied      1 if the optimiser stepped, 0 if *gate == 0 made it skip the step */
+typedef struct rb_learn_stats_record {
+  int64_t update;
+  float loss_mean, loss_max, objective, q_mean, target_mean, edge_mass, weight_min, grad_norm, clip_coef, applied;
+} rb_learn_stats_record;
+
+/* The record of one update, in two parts so that only a one-thread launch has to follow the optimiser step:
+ *   rb_learn_stats_batch   (as soon as the loss kernel has run; the learner puts it on a side stream beside the backward)
+ *     computes the batch fields from loss[B], weights[B], actions[B] (int64), m[B][Z] (the m_out of rb_c51_loss_grad /
+ *     rb_c51_dueling_loss_grad), support[Z] and the online logits of the s rows in exactly one of two layouts: z = the
+ *     fused head's (z_value | z_advantage) [>= B rows][Z + A Z] (dueling combination model.py:75 applied here), or
+ *     q = [B][A][Z]; the other pointer is NULL.  The results stay in `scratch`.
+ *   rb_learn_stats_write   (after the optimiser step) writes them with *grad_norm (device float), the clip coefficient and
+ *     the gate (optional device int32; NULL = the step was applied) into ring[*counter % capacity] and advances *counter
+ *     (device int64), so each replay of a captured graph writes a fresh slot.
+ * rb_learn_stats = both, in that order on one stream.  scratch: double[rb_learn_stats_scratch_elems()], ZERO-INITIALISED
+ * once by the caller (its last element is a self-resetting completion ticket); one scratch per stream of records.  Sums
+ * over the batch run in float64 in a fixed order (an eager launch and a graph replay agree bitwise).  RB_ERR_INVAL: a NULL
+ * pointer, or both / neither of z and q; RB_ERR_RANGE: Z > RB_MAX_ATOMS or capacity <= 0.  A refused call writes nothing. */
+int rb_learn_stats_scratch_elems(void);
+int rb_learn_stats_batch(const float* loss, const float* weights, const int64_t* actions, const float* m, const float* support,
+                         const float* z, const float* q, int B, int A, int Z, double* scratch, rb_stream_t stream);
+int rb_learn_stats_write(const double* scratch, const float* grad_norm, const int32_t* gate, float max_norm,
+                         rb_learn_stats_record* ring, int capacity, int64_t* counter, rb_stream_t stream);
+int rb_learn_stats(const float* loss, const float* weights, const int64_t* actions, const float* m, const float* support,
+                   const float* z, const float* q, int B, int A, int Z, const float* grad_norm, const int32_t* gate,
+                   float max_norm, double* scratch, rb_learn_stats_record* ring, int capacity, int64_t* counter,
+                   rb_stream_t stream);
 
 #ifdef __cplusplus
 }

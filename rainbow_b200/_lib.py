@@ -69,7 +69,18 @@ SIGNATURES = {
     "rb_clip_adam_scratch_elems": (C.c_int, []),
     "rb_clip_adam": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
     "rb_q_values": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "rb_learn_stats_scratch_elems": (C.c_int, []),
+    "rb_learn_stats_batch": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "rb_learn_stats_write": (C.c_int, [_vp, _vp, _vp, _f32, _vp, _i32, _vp, _vp]),
+    "rb_learn_stats": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _vp, _i32, _vp,
+                                 _vp]),
 }
+
+# rb_learn_stats_record of include/rainbow_b200.h (48 bytes): field name -> numpy dtype, in memory order
+LEARN_STATS_FIELDS = [("update", "<i8")] + [(n, "<f4") for n in (
+    "loss_mean", "loss_max", "objective", "q_mean", "target_mean", "edge_mass", "weight_min", "grad_norm", "clip_coef",
+    "applied")]
+LEARN_STATS_RECORD_BYTES = 48
 
 
 class RainbowB200Error(RuntimeError):
@@ -122,7 +133,7 @@ def stream():
 KERNEL_IDS = ["tree_update", "tree_find", "tree_sample", "gather", "iter_states", "append", "c51", "noisy_resample",
               "noisy_compose", "sqnorm", "clip_adam", "head_fc1", "head_fc2", "head_logits", "head_wgrad2", "head_dh",
               "head_bwd1", "noise_factors", "c51_dueling", "bias_grad", "q_values", "head_reduce1", "conv_wgrad",
-              "head_bwd1_wgrad", "head_bwd1_dx"]  # order of the enum in include/rainbow_b200.h
+              "head_bwd1_wgrad", "head_bwd1_dx", "learn_stats"]  # order of the enum in include/rainbow_b200.h
 
 
 class KernelTimer:

@@ -11,6 +11,8 @@ One `learn(mem)` (agent.py:61-100) is:
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
     K4 rb_tree_update                         (agent.py:100 -> memory.py:157-159)
+    [args.learn_stats = R > 0: rb_learn_stats_batch on a side stream after K3, rb_learn_stats_write after K7 -- one record
+     per update into a device ring, read with Agent.learn_stats()]
 
 Nothing in that chain synchronises with the host, so the whole update is captured into one CUDA graph
 (`cuda_graph=True`, the default) and replayed: the update is launch-latency bound otherwise
@@ -222,6 +224,10 @@ class Agent:
         self._rejected_seen = 0
         self._q_graphs = {}       # training-mode flag -> captured one-state act / evaluate_q graph
         self.last_loss = None  # per-sample losses of the most recent update (device tensor)
+        self._warm = 0
+        self._stats = None        # learn-statistics ring (set_learn_stats)
+        self.learn_stats_capacity = 0
+        self.set_learn_stats(int(getattr(args, "learn_stats", 0) or 0))
 
     # ---- acting / evaluation (agent.py:49-59,110-118) ---------------------------------------------
     def reset_noise(self):
@@ -415,8 +421,11 @@ class Agent:
                 z_on, h_on, p_on = on.head().forward(xs_d, x_ns)              # rows [0,B) = s, [B,2B) = s'
                 main.wait_event(done_tg)
         with torch.no_grad():
+            m = torch.empty((B, self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
             loss, dz = c51_dueling_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals, weights,
-                                             self.support, self.Vmin, self.Vmax, self.delta_z, self.discount ** self.n)
+                                             self.support, self.Vmin, self.Vmax, self.delta_z, self.discount ** self.n,
+                                             m_out=m)
+            stats_done = self._stats_batch(batch, loss, m, z=z_on) if m is not None else None
             wb_done = None
             if after_loss is not None:
                 # the priority write-back (agent.py:100) needs nothing but the per-sample losses: it runs on a side
@@ -472,6 +481,8 @@ class Agent:
             x_s.backward(dx)
             self.sync.all_reduce_(self.optimiser.flat_grad)
         self.optimiser.step(grad_scale=1.0 / self.sync.world_size, gate=self._step_gate)
+        if stats_done is not None:
+            self._stats_write(stats_done)
         if wb_done is not None:
             main.wait_event(wb_done)
         return loss
@@ -492,12 +503,16 @@ class Agent:
             else:
                 self.target_net.reset_noise(*target_noise)
             q_t = self.target_net.logits(next_states)
+            m = torch.empty((q_s.shape[0], self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
             loss, grad = c51_loss_grad(q_s.detach(), q_ns, q_t, actions, returns, nonterminals, weights, self.support,
-                                       self.Vmin, self.Vmax, self.delta_z, self.discount ** self.n)
+                                       self.Vmin, self.Vmax, self.delta_z, self.discount ** self.n, m_out=m)
+            stats_done = self._stats_batch(batch, loss, m, q=q_s.detach()) if m is not None else None
         self.optimiser.zero_grad()
         q_s.backward(grad)
         self.sync.all_reduce_(self.optimiser.flat_grad)
         self.optimiser.step(grad_scale=1.0 / self.sync.world_size, gate=self._step_gate)
+        if stats_done is not None:
+            self._stats_write(stats_done)
         if after_loss is not None:
             after_loss(loss)
         return loss
@@ -575,3 +590,71 @@ class Agent:
                 warnings.warn(f"rainbow_b200: {rejected - self._rejected_seen} sampled batches were rejected "
                               f"{mem.max_attempts} times in a row and skipped (no update, no priority write-back)")
             self._rejected_seen = rejected
+
+    # ---- learner statistics (agent.py:66-98 computes most of them and discards them) ----------------
+    def set_learn_stats(self, capacity):
+        """Record one rb_learn_stats_record per update (include/rainbow_b200.h) into a device ring of `capacity` records;
+        0 turns the recording off (no extra launch, no m output of the loss kernel, the update graph of today).  The ring
+        is allocated here, outside any capture.  A change drops the captured update graphs: they are recaptured after
+        fresh warm-up updates."""
+        capacity = int(capacity)
+        if capacity < 0:
+            raise ValueError(f"learn_stats capacity must be >= 0, got {capacity}")
+        if capacity == self.learn_stats_capacity:
+            return
+        self._stats = None
+        if capacity:
+            # record 0 is a header whose first 8 bytes hold the device counter; the ring follows: both come back in one copy
+            words = (capacity + 1) * _lib.LEARN_STATS_RECORD_BYTES // 4
+            buf = torch.zeros(words, dtype=torch.int32, device=self.device)
+            scratch = torch.zeros(_lib.load().rb_learn_stats_scratch_elems(), dtype=torch.float64, device=self.device)
+            self._stats = dict(buf=buf, host=torch.zeros(words, dtype=torch.int32).pin_memory(), read=0, scratch=scratch,
+                               last=None)
+        self.learn_stats_capacity = capacity
+        self._graphs, self._warm = {}, 0
+
+    def learn_stats(self):
+        """The records written since the previous call, oldest first: {field: numpy array} for the fields of
+        rb_learn_stats_record, plus "dropped", the number of records the ring overwrote before they were read.
+        One stream synchronisation and one device-to-host copy."""
+        st = self._stats
+        if st is None:
+            raise _lib.RainbowB200Error("learn statistics are off: set args.learn_stats (or call set_learn_stats) to a ring "
+                                        "capacity > 0")
+        R = self.learn_stats_capacity
+        st["host"].copy_(st["buf"], non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        rec = st["host"].numpy().view(np.dtype(_lib.LEARN_STATS_FIELDS))   # [R + 1] records, [0] = header
+        count = int(rec["update"][0])
+        first = max(st["read"], count - R)
+        rows = rec[1 + np.arange(first, count) % R]
+        out = {name: np.ascontiguousarray(rows[name]) for name, _ in _lib.LEARN_STATS_FIELDS}
+        out["dropped"] = first - st["read"]
+        st["read"] = count
+        return out
+
+    def _stats_batch(self, batch, loss, m, z=None, q=None):
+        """rb_learn_stats_batch on a side stream as soon as the losses exist: it runs beside the backward.  Returns the
+        event _stats_write waits for.  The inputs of the latest record stay reachable in self._stats["last"]."""
+        main = torch.cuda.current_stream(self.device)
+        side = self._side_streams()[0]
+        ready = torch.cuda.Event()
+        ready.record(main)
+        with torch.cuda.stream(side):
+            side.wait_event(ready)
+            _lib.check(_lib.load().rb_learn_stats_batch(
+                _lib.ptr(loss), _lib.ptr(batch[6]), _lib.ptr(batch[2]), _lib.ptr(m), _lib.ptr(self.support), _lib.ptr(z),
+                _lib.ptr(q), loss.shape[0], self.action_space, self.atoms, _lib.ptr(self._stats["scratch"]), _lib.stream()))
+            done = torch.cuda.Event()
+            done.record(side)
+        self._stats["last"] = dict(m=m, z=z, q=q)
+        return done
+
+    def _stats_write(self, done):
+        """rb_learn_stats_write after the optimiser step (its norm and gate are final): one thread on the caller's stream."""
+        torch.cuda.current_stream(self.device).wait_event(done)
+        buf = self._stats["buf"]
+        _lib.check(_lib.load().rb_learn_stats_write(
+            _lib.ptr(self._stats["scratch"]), _lib.ptr(self.optimiser.grad_norm), _lib.ptr(self._step_gate),
+            self.optimiser.max_norm, buf.data_ptr() + _lib.LEARN_STATS_RECORD_BYTES, self.learn_stats_capacity,
+            buf.data_ptr(), _lib.stream()))

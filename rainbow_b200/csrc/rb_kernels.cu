@@ -1131,6 +1131,175 @@ k_q_select(const float* __restrict__ z, int M, int A, int Z, const float* __rest
 }
 
 // ================================================================================================
+// Learner statistics (agent.py:66-98 computes most of them and discards them): one record per update into a device ring.
+// ================================================================================================
+// Two launches, so that only a one-thread kernel has to wait for the optimiser step:
+//   k_learn_stats_batch   everything that needs only the loss kernel's outputs.  Warp g of the grid takes the samples g,
+//                         g + warps, ... (lane owns atoms lane + 32 r): q(s, a) of the taken action with the arithmetic of
+//                         c51_expected_value, sum m * support as a warp sum, the end-atom mass, the loss / weight terms.
+//                         Sums are float64: each warp in sample order, each CTA over its warps in order into its partial
+//                         slot of the scratch; the last CTA to finish (self-resetting ticket) reduces the partials in CTA
+//                         order (fixed xor butterflies, then the warps in order) and leaves the seven finished fields in
+//                         the scratch.  Which CTA is last does not change the order: eager launches and graph replays agree
+//                         bitwise.
+//   k_learn_stats_record  after the optimiser step: those fields, the norm, clip coefficient and gate into slot
+//                         *counter % capacity; advances *counter.
+// Scratch (double, zero-initialised once): [0, 7) the finished fields, [8, 8 + 8 * STATS_MAX_CTAS) the per-CTA partials,
+// then the ticket word.
+constexpr int STATS_THREADS = 256;
+constexpr int STATS_WARPS = STATS_THREADS / 32;
+constexpr int STATS_MAX_CTAS = 256;                 // = STATS_THREADS: the last CTA reduces one partial per thread
+constexpr int STATS_PART = 8;
+constexpr int STATS_SCRATCH = STATS_PART + STATS_PART * STATS_MAX_CTAS + 1;
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__device__ __forceinline__ double warp_max_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+__device__ __forceinline__ double warp_min_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// per-warp values of the 7 accumulators -> s_part[k][warp] (lane 0); k: loss, w * loss, q(s, a), sum m * support, edge
+// mass (sums), loss max, weight min
+__device__ __forceinline__ void stats_store(double (&s_part)[7][STATS_WARPS], const double (&v)[7], int warp, int lane) {
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < 7; ++k) s_part[k][warp] = v[k];
+  }
+}
+
+__device__ __forceinline__ void stats_combine(const double (&s_part)[7][STATS_WARPS], double (&t)[7]) {
+  t[0] = t[1] = t[2] = t[3] = t[4] = 0.0;
+  t[5] = -CUDART_INF;
+  t[6] = CUDART_INF;
+  for (int w = 0; w < STATS_WARPS; ++w) {
+#pragma unroll
+    for (int k = 0; k < 5; ++k) t[k] += s_part[k][w];
+    t[5] = fmax(t[5], s_part[5][w]);
+    t[6] = fmin(t[6], s_part[6][w]);
+  }
+}
+
+__global__ void __launch_bounds__(STATS_THREADS)
+k_learn_stats_batch(const float* __restrict__ loss, const float* __restrict__ weights, const int64_t* __restrict__ actions,
+                    const float* __restrict__ m, const float* __restrict__ support, const float* __restrict__ z,
+                    const float* __restrict__ q, int B, int A, int Z, double* __restrict__ scratch) {
+  __shared__ double s_part[7][STATS_WARPS];
+  __shared__ bool s_last;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  constexpr int R = RB_MAX_ATOMS / 32;
+  float sup[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  double v[7] = {0.0, 0.0, 0.0, 0.0, 0.0, -CUDART_INF, CUDART_INF};
+  const int warps = gridDim.x * STATS_WARPS;
+  for (int i = blockIdx.x * STATS_WARPS + warp; i < B; i += warps) {
+    const int act = (int)actions[i];
+    const float* mr = m + (size_t)i * Z;
+    const float l = __ldg(loss + i), w = __ldg(weights + i);
+    float tv = 0.0f;
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+      if (lane + 32 * r < Z) tv = __fadd_rn(tv, __fmul_rn(__ldg(mr + lane + 32 * r), sup[r]));
+    const float edge = __fadd_rn(__ldg(mr), __ldg(mr + Z - 1));
+    float x[R];
+    if (z) {   // dueling combination of the taken action, as k_c51_dueling forms it
+      const float* zr = z + (size_t)i * (Z + A * Z);
+#pragma unroll
+      for (int r = 0; r < R; ++r) {
+        const int c = lane + 32 * r;
+        x[r] = -CUDART_INF_F;
+        if (c < Z) {
+          float mean = 0.0f;
+          for (int a = 0; a < A; ++a) mean += __ldg(zr + Z + a * Z + c);
+          x[r] = __ldg(zr + c) + __ldg(zr + Z + act * Z + c) - mean / (float)A;
+        }
+      }
+    } else {
+      const float* qr = q + ((size_t)i * A + act) * Z;
+#pragma unroll
+      for (int r = 0; r < R; ++r) x[r] = (lane + 32 * r < Z) ? __ldg(qr + lane + 32 * r) : -CUDART_INF_F;
+    }
+    const float ev = c51_expected_value<R>(x, sup, Z, lane);
+    tv = warp_sum(tv);   // the butterflies leave the same value in every lane
+    v[0] += (double)l;
+    v[1] += (double)w * (double)l;   // exact product
+    v[2] += (double)ev;
+    v[3] += (double)tv;
+    v[4] += (double)edge;
+    v[5] = fmax(v[5], (double)l);
+    v[6] = fmin(v[6], (double)w);
+  }
+  stats_store(s_part, v, warp, lane);
+  __syncthreads();
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(scratch + STATS_SCRATCH - 1);
+  if (tid == 0) {
+    double t[7];
+    stats_combine(s_part, t);
+    double* part = scratch + STATS_PART + STATS_PART * blockIdx.x;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) part[k] = t[k];
+    __threadfence();
+    s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  double p[7] = {0.0, 0.0, 0.0, 0.0, 0.0, -CUDART_INF, CUDART_INF};
+  if (tid < (int)gridDim.x) {
+    const double* part = scratch + STATS_PART + STATS_PART * tid;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) p[k] = __ldcg(part + k);
+  }
+#pragma unroll
+  for (int k = 0; k < 5; ++k) p[k] = warp_sum_f64(p[k]);
+  p[5] = warp_max_f64(p[5]);
+  p[6] = warp_min_f64(p[6]);
+  stats_store(s_part, p, warp, lane);
+  __syncthreads();
+  if (tid == 0) {
+    double t[7];
+    stats_combine(s_part, t);
+#pragma unroll
+    for (int k = 0; k < 5; ++k) scratch[k] = (double)(float)(t[k] / B);   // loss_mean, objective, q_mean, target_mean, edge_mass
+    scratch[5] = t[5];                                                    // loss_max
+    scratch[6] = t[6];                                                    // weight_min
+    *ticket = 0u;
+  }
+}
+
+__global__ void k_learn_stats_record(const double* __restrict__ scratch, const float* __restrict__ grad_norm,
+                                     const int32_t* __restrict__ gate, float max_norm, rb_learn_stats_record* __restrict__ ring,
+                                     int capacity, int64_t* __restrict__ counter) {
+  const float norm = *grad_norm;
+  rb_learn_stats_record rec;
+  rec.update = *counter;
+  rec.loss_mean = (float)scratch[0];
+  rec.loss_max = (float)scratch[5];
+  rec.objective = (float)scratch[1];
+  rec.q_mean = (float)scratch[2];
+  rec.target_mean = (float)scratch[3];
+  rec.edge_mass = (float)scratch[4];
+  rec.weight_min = (float)scratch[6];
+  rec.grad_norm = norm;
+  rec.clip_coef = fminf(max_norm / (norm + 1e-6f), 1.0f);   // as k_clip_adam / k_peer_adam
+  rec.applied = (gate && *gate == 0) ? 0.0f : 1.0f;
+  ring[rec.update % capacity] = rec;
+  *counter = rec.update + 1;
+}
+
+// ================================================================================================
 // K6  noisy_resample : factorised Gaussian noise for every NoisyLinear of one net, one launch.
 // ================================================================================================
 struct NoisyPlan {
@@ -1638,6 +1807,57 @@ int rb_q_values(const float* z, int M, int actions, int atoms, const float* supp
   { ProfScope prof_(RB_K_Q_VALUES, (cudaStream_t)stream);
     k_q_select<<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, support, q, best_action, best_q); }
   return check_launch("rb_q_values");
+}
+
+static int stats_batch_check(const float* loss, const float* weights, const int64_t* actions, const float* m,
+                             const float* support, const float* z, const float* q, int B, int A, int Z, const double* scratch) {
+  if (!loss || !weights || !actions || !m || !support || !scratch) return fail(RB_ERR_INVAL, "rb_learn_stats: null pointer");
+  if ((z == nullptr) == (q == nullptr)) return fail(RB_ERR_INVAL, "rb_learn_stats: give exactly one of z and q");
+  if (B <= 0 || A <= 0 || Z <= 1) return fail(RB_ERR_INVAL, "rb_learn_stats: B, A > 0 and Z > 1 are required");
+  if (Z > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_learn_stats: Z exceeds RB_MAX_ATOMS");
+  return RB_OK;
+}
+
+static int stats_record_check(const double* scratch, const float* grad_norm, const rb_learn_stats_record* ring, int capacity,
+                              const int64_t* counter) {
+  if (!scratch || !grad_norm || !ring || !counter) return fail(RB_ERR_INVAL, "rb_learn_stats: null pointer");
+  if (capacity <= 0) return fail(RB_ERR_RANGE, "rb_learn_stats: the ring needs a positive capacity");
+  return RB_OK;
+}
+
+int rb_learn_stats_scratch_elems(void) { return STATS_SCRATCH; }
+
+int rb_learn_stats_batch(const float* loss, const float* weights, const int64_t* actions, const float* m, const float* support,
+                         const float* z, const float* q, int B, int A, int Z, double* scratch, rb_stream_t stream) {
+  int rc = stats_batch_check(loss, weights, actions, m, support, z, q, B, A, Z, scratch);
+  if (rc != RB_OK) return rc;
+  int ctas = (B + STATS_WARPS - 1) / STATS_WARPS;
+  if (ctas > STATS_MAX_CTAS) ctas = STATS_MAX_CTAS;
+  { ProfScope prof_(RB_K_LEARN_STATS, (cudaStream_t)stream);
+    k_learn_stats_batch<<<ctas, STATS_THREADS, 0, (cudaStream_t)stream>>>(loss, weights, actions, m, support, z, q, B, A, Z,
+                                                                          scratch); }
+  return check_launch("rb_learn_stats_batch");
+}
+
+int rb_learn_stats_write(const double* scratch, const float* grad_norm, const int32_t* gate, float max_norm,
+                         rb_learn_stats_record* ring, int capacity, int64_t* counter, rb_stream_t stream) {
+  int rc = stats_record_check(scratch, grad_norm, ring, capacity, counter);
+  if (rc != RB_OK) return rc;
+  { ProfScope prof_(RB_K_LEARN_STATS, (cudaStream_t)stream);
+    k_learn_stats_record<<<1, 1, 0, (cudaStream_t)stream>>>(scratch, grad_norm, gate, max_norm, ring, capacity, counter); }
+  return check_launch("rb_learn_stats_write");
+}
+
+int rb_learn_stats(const float* loss, const float* weights, const int64_t* actions, const float* m, const float* support,
+                   const float* z, const float* q, int B, int A, int Z, const float* grad_norm, const int32_t* gate,
+                   float max_norm, double* scratch, rb_learn_stats_record* ring, int capacity, int64_t* counter,
+                   rb_stream_t stream) {
+  int rc = stats_batch_check(loss, weights, actions, m, support, z, q, B, A, Z, scratch);
+  if (rc == RB_OK) rc = stats_record_check(scratch, grad_norm, ring, capacity, counter);
+  if (rc != RB_OK) return rc;
+  rc = rb_learn_stats_batch(loss, weights, actions, m, support, z, q, B, A, Z, scratch, stream);
+  if (rc != RB_OK) return rc;
+  return rb_learn_stats_write(scratch, grad_norm, gate, max_norm, ring, capacity, counter, stream);
 }
 
 int rb_noisy_compose(const float* mu, const float* sigma, const float* eps, int64_t count, float* out, rb_stream_t stream) {
