@@ -127,9 +127,20 @@ class FusedClipAdam:
             self.numel, float(grad_scale), self.max_norm, self.lr, self.betas[0], self.betas[1], self.eps,
             _lib.ptr(self.step_count), _lib.ptr(self._partial), _lib.ptr(self.grad_norm), _lib.ptr(gate), _lib.stream()))
 
-    def state_dict(self):
-        return dict(step=int(self.step_count.item()), exp_avg=self.exp_avg.clone(), exp_avg_sq=self.exp_avg_sq.clone(),
-                    lr=self.lr, eps=self.eps, betas=self.betas, max_norm=self.max_norm)
+    def state_dict(self, clone=True):
+        """`clone=False` returns the live moment tensors (a checkpoint streams them to disk and restores into them in
+        place).  `layout` says what the moments cover: every element ("replicated", also under NCCL data parallelism) or,
+        with the peer optimiser, this rank's shard of each segment."""
+        own = (lambda t: t.clone()) if clone else (lambda t: t)
+        return dict(step=int(self.step_count.item()), exp_avg=own(self.exp_avg), exp_avg_sq=own(self.exp_avg_sq),
+                    lr=self.lr, eps=self.eps, betas=self.betas, max_norm=self.max_norm, layout=self.layout())
+
+    def layout(self):
+        if self.peer is None:
+            return dict(kind="replicated", numel=self.numel)
+        p = self.peer
+        return dict(kind="peer", numel=self.numel, world=p.world, rank=p.rank, segments=[list(s) for s in p.segments],
+                    parts=list(p.parts))
 
     def load_state_dict(self, sd):
         self.step_count.fill_(int(sd["step"]))
@@ -333,6 +344,23 @@ class Agent:
 
     def save(self, path, name="model.pth"):
         torch.save(self.online_net.state_dict(), os.path.join(path, name))
+
+    # ---- exact resume (rainbow_b200/checkpoint.py) -----------------------------------------------------
+    def save_checkpoint(self, path, mem=None):
+        """Synchronise the device and write everything that decides the next update -- parameters, target net, Adam
+        state, both nets' noise streams, the statistics ring, and the replay `mem` if given -- to `path/rank{r}/`,
+        atomically.  Hyper-parameters are recorded but come from the live `args` on load.  The caller's host generators
+        (numpy / torch global RNGs: act_e_greedy, rng="numpy" sampling) are not part of the checkpoint.  Under data
+        parallelism every rank calls it (the ranks share one save id)."""
+        from . import checkpoint
+        checkpoint.save(self, path, mem)
+
+    def load_checkpoint(self, path, mem=None):
+        """Restore a save_checkpoint() into this agent (built as usual with the same structure) and into `mem`, in place:
+        captured update and act graphs stay valid.  Everything is validated first; a refusal raises RainbowB200Error and
+        changes nothing (under data parallelism every rank raises)."""
+        from . import checkpoint
+        checkpoint.load(self, path, mem)
 
     # ---- the update ------------------------------------------------------------------------------
     def _fused_path(self, B):

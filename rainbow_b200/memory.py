@@ -33,6 +33,19 @@ Transition_dtype = np.dtype([("timestep", np.int32), ("state", np.uint8, (84, 84
                              ("reward", np.float32), ("nonterminal", np.bool_)])
 
 
+# The replay's persistent fields, one list for pickling (ReplayMemory.__getstate__ / __setstate__) and for
+# rainbow_b200.checkpoint: host attributes of the ReplayMemory with their role on a checkpoint restore -- "structure" must
+# match the live object, "setting" keeps the live object's value, "state" is restored -- and the device arrays of its
+# SegmentTree as (pickle key, SegmentTree attribute).  Both formats add the ring's host mirrors (index, full) and device
+# scalars (running max, sampling counter) in their own form.
+PERSISTENT_ROLES = (("capacity", "structure"), ("history", "structure"), ("discount", "setting"), ("n", "setting"),
+                    ("priority_weight", "state"), ("priority_exponent", "setting"), ("t", "state"), ("rng", "setting"),
+                    ("seed", "state"), ("max_attempts", "setting"), ("strict", "setting"))
+PERSISTENT_HOST = tuple(name for name, _ in PERSISTENT_ROLES)
+PERSISTENT_ARRAYS = (("sum_tree", "tree"), ("frames", "frames"), ("timestep", "timestep"), ("action", "action"),
+                     ("reward", "reward"), ("nonterminal", "nonterminal"))
+
+
 def _require_cuda(device):
     device = torch.device(device)
     if device.type != "cuda":
@@ -462,14 +475,12 @@ class ReplayMemory:
         save_reference_pickle()."""
         self.flush_appends()
         tr = self.transitions
-        return dict(
-            version=1, capacity=self.capacity, history=self.history, discount=self.discount, n=self.n,
-            priority_weight=self.priority_weight, priority_exponent=self.priority_exponent, t=self.t, rng=self.rng,
-            seed=self.seed, max_attempts=self.max_attempts, strict=self.strict, device=str(self.device),
-            rng_counter=int(self._rng_counter.item()), index=tr.index, full=tr.full, max=tr.max,
-            sum_tree=tr.sum_tree, frames=tr.frames.cpu().numpy(), timestep=tr.timestep.cpu().numpy(),
-            action=tr.action.cpu().numpy(), reward=tr.reward.cpu().numpy(),
-            nonterminal=tr.nonterminal.cpu().numpy())
+        state = dict(version=1)
+        state.update((k, getattr(self, k)) for k in PERSISTENT_HOST)
+        state.update(device=str(self.device), rng_counter=int(self._rng_counter.item()), index=tr.index, full=tr.full,
+                     max=tr.max)
+        state.update((key, getattr(tr, attr).cpu().numpy()) for key, attr in PERSISTENT_ARRAYS)
+        return state
 
     def _init_runtime(self, rng_counter=0):
         self.n_step_scaling = torch.tensor([self.discount ** i for i in range(self.n)], dtype=torch.float32,
@@ -486,12 +497,11 @@ class ReplayMemory:
         if "version" not in s and "transitions" in s:
             return self._setstate_reference(s)
         self.device = _require_cuda(s["device"])
-        self.capacity, self.history, self.discount, self.n = s["capacity"], s["history"], s["discount"], s["n"]
-        self.priority_weight, self.priority_exponent, self.t = s["priority_weight"], s["priority_exponent"], s["t"]
-        self.rng, self.seed, self.max_attempts, self.strict = s["rng"], s["seed"], s["max_attempts"], s["strict"]
+        for k in PERSISTENT_HOST:
+            setattr(self, k, s[k])
         self.transitions = SegmentTree(self.capacity, self.device)
-        self.transitions.load_arrays(s["sum_tree"], s["frames"], s["timestep"], s["action"], s["reward"],
-                                     s["nonterminal"], s["index"], s["full"], s["t"], s["max"])
+        self.transitions.load_arrays(**{key: s[key] for key, _ in PERSISTENT_ARRAYS}, index=s["index"], full=s["full"],
+                                     t_episode=s["t"], max_value=s["max"])
         self._init_runtime(s["rng_counter"])
 
     def _setstate_reference(self, s):

@@ -206,6 +206,7 @@ class DQN(nn.Module):
         self.hidden_size = args.hidden_size
         if args.architecture not in _ARCH:
             raise ValueError(f"unknown architecture '{args.architecture}'")
+        self.architecture = args.architecture
         specs, self.conv_output_size = _ARCH[args.architecture]
         mods, c_in = [], args.history_length
         for c_out, k, s in specs:
