@@ -58,6 +58,7 @@ extern "C" {
 #define RB_MAX_NOISY_LAYERS 8
 #define RB_MAX_PEERS 8           /* ranks of one NVLink domain handled by rb_peer_clip_adam */
 #define RB_APPEND_BATCH 8        /* transitions per rb_append_batch launch */
+#define RB_MAX_SHIFT_PAD 16      /* largest pad of rb_gather_shift */
 
 /* status words written by rb_tree_sample (int32[4]): status[0] = 1 if the batch now in the output buffers passed the
  * whole-batch validity test (memory.py:131), 0 otherwise; status[1] = draws used; status[2] = number of device-RNG
@@ -73,7 +74,8 @@ enum {
   RB_K_TREE_UPDATE = 0, RB_K_TREE_FIND, RB_K_TREE_SAMPLE, RB_K_GATHER, RB_K_ITER_STATES, RB_K_APPEND, RB_K_C51,
   RB_K_NOISY_RESAMPLE, RB_K_NOISY_COMPOSE, RB_K_SQNORM, RB_K_CLIP_ADAM, RB_K_HEAD_FC1, RB_K_HEAD_FC2, RB_K_HEAD_LOGITS,
   RB_K_HEAD_WGRAD2, RB_K_HEAD_DH, RB_K_HEAD_BWD1, RB_K_NOISE_FACTORS, RB_K_C51_DUELING, RB_K_BIAS_GRAD, RB_K_Q_VALUES,
-  RB_K_HEAD_REDUCE1, RB_K_CONV_WGRAD, RB_K_HEAD_BWD1_WGRAD, RB_K_HEAD_BWD1_DX, RB_K_LEARN_STATS, RB_KERNEL_COUNT
+  RB_K_HEAD_REDUCE1, RB_K_CONV_WGRAD, RB_K_HEAD_BWD1_WGRAD, RB_K_HEAD_BWD1_DX, RB_K_LEARN_STATS, RB_K_GATHER_SHIFT,
+  RB_KERNEL_COUNT
 };
 
 int rb_abi_version(void);
@@ -122,6 +124,23 @@ int rb_gather(const uint8_t* frames, const int32_t* timestep, const int32_t* act
               const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n,
               const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
               float* nonterminals, rb_stream_t stream);
+
+/* rb_gather with random-shift augmentation of the observations (DrQ, Kostrikov et al. 2020; no reference counterpart):
+ * every observation -- each sample's state and its next state -- is edge-padded by `pad` pixels and cropped back to
+ * 84 x 84 at its own integer offset (oy, ox), each uniform in [0, 2 pad], the same for all of its history frames:
+ *   out[c][y][x] = in[c][clamp(y + oy - pad, 0, 83)][clamp(x + ox - pad, 0, 83)]
+ * where `in` is what rb_gather writes (blanking included).  actions, returns and nonterminals are rb_gather's, bitwise.
+ * Offsets: one Philox4x32-10 call per sample b with key `seed` and counter (c_lo, c_hi, b, 0x53484654), c = *rng_counter
+ * as the kernel reads it (rb_tree_sample has just advanced it, so each batch and each graph replay draws afresh; this call
+ * does not advance it); words x, y give the state's (oy, ox), z, w the next state's; offset = (word * (2 pad + 1)) >> 32.
+ * shifts (required): int32[2][B][2] (side: 0 = state, 1 = next state; sample; (oy, ox)) receives the offsets used.
+ * RB_ERR_RANGE: pad outside [1, RB_MAX_SHIFT_PAD], plus every check of rb_gather; RB_ERR_INVAL: a NULL pointer.  A refused
+ * call launches nothing. */
+int rb_gather_shift(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                    const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n,
+                    const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
+                    float* nonterminals, int pad, uint64_t seed, const uint64_t* rng_counter, int32_t* shifts,
+                    rb_stream_t stream);
 
 /* memory.py:166-178 ReplayMemory.__next__, batched: states for current_idx = first .. first+count-1,
  * backward-only blanking, negative indices wrap.  out is float32[count][history][84*84]. */

@@ -37,6 +37,8 @@ SIGNATURES = {
     "rb_tree_sample": (C.c_int, [_vp, _i64, _i64, _vp, _i32, _i32, _vp, _i32, _u64, _vp, _i32, _f32, _vp, _i32,
                                  _vp, _vp, _vp, _vp, _vp, _vp]),
     "rb_gather": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rb_gather_shift": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32,
+                                  _u64, _vp, _vp, _vp]),
     "rb_iter_states": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _i32, _vp, _vp]),
     "rb_append": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int32, _f32, _i32, _vp]),
     "rb_append_batch": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
@@ -133,7 +135,7 @@ def stream():
 KERNEL_IDS = ["tree_update", "tree_find", "tree_sample", "gather", "iter_states", "append", "c51", "noisy_resample",
               "noisy_compose", "sqnorm", "clip_adam", "head_fc1", "head_fc2", "head_logits", "head_wgrad2", "head_dh",
               "head_bwd1", "noise_factors", "c51_dueling", "bias_grad", "q_values", "head_reduce1", "conv_wgrad",
-              "head_bwd1_wgrad", "head_bwd1_dx", "learn_stats"]  # order of the enum in include/rainbow_b200.h
+              "head_bwd1_wgrad", "head_bwd1_dx", "learn_stats", "gather_shift"]  # order of the enum in include/rainbow_b200.h
 
 
 class KernelTimer:

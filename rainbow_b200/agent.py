@@ -3,6 +3,8 @@
 One `learn(mem)` (agent.py:61-100) is:
 
     K1 rb_tree_sample + K2 rb_gather          (mem.sample, memory.py:148-155)
+                                              [args.augment_shift = p > 0: rb_gather_shift instead -- random-shift
+                                               augmentation of s and s' (DrQ), offsets drawn on the device]
     3 x conv body (torch: cuDNN)              (agent.py:66,71,75 -> model.py:70-71)
     K6 rb_noisy_resample (target net)         (agent.py:74)
     fused noisy dueling heads (rb_head_forward) on the conv features -- online net on [s; s'], target on s'
@@ -171,6 +173,10 @@ class Agent:
         self.n = args.multi_step
         self.discount = args.discount
         self.norm_clip = args.norm_clip
+        # random-shift augmentation of the sampled states (DrQ): pad in pixels, 0 = off.  Acting and evaluation stay unaugmented.
+        self.augment_shift = int(getattr(args, "augment_shift", 0) or 0)
+        if not 0 <= self.augment_shift <= ReplayMemory.MAX_SHIFT_PAD:
+            raise ValueError(f"augment_shift must be in [0, {ReplayMemory.MAX_SHIFT_PAD}], got {self.augment_shift}")
 
         self.online_net = DQN(args, self.action_space).to(device=self.device)
         model_path = getattr(args, "model", None)
@@ -546,11 +552,12 @@ class Agent:
         return loss
 
     def _learn_eager(self, mem):
-        batch = mem.sample(self.batch_size)
         if isinstance(mem, ReplayMemory):
+            batch = mem.sample(self.batch_size, shift_pad=self.augment_shift)
             gate = mem.sample_gate()
             return self._update_from_batch(batch, after_loss=lambda loss: mem.update_priorities(batch[0], loss, gate=gate),
                                            gate=gate)
+        batch = mem.sample(self.batch_size)
         loss = self._update_from_batch(batch)
         mem.update_priorities(batch[0], loss.detach().cpu().numpy())  # a foreign (reference-style, host) memory: agent.py:100
         return loss
@@ -564,7 +571,7 @@ class Agent:
         torch.cuda.synchronize(self.device)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            batch = mem.sample_into(ws)
+            batch = mem.sample_into(ws, shift_pad=self.augment_shift)
             loss = self._update_from_batch(batch, after_loss=lambda l: mem.update_priorities(batch[0], l, gate=ws.status),
                                            gate=ws.status)
         return graph, ws, loss
@@ -580,6 +587,9 @@ class Agent:
         """agent.py:61-100.  Exactly one update per call: the first GRAPH_WARMUP calls run eagerly on a side
         stream (torch's documented warm-up recipe for whole-step capture), the next call captures the graph and
         every call from then on is one graph launch."""
+        if self.augment_shift and not isinstance(mem, ReplayMemory):
+            raise _lib.RainbowB200Error("args.augment_shift needs a rainbow_b200 ReplayMemory: the shifts are drawn and "
+                                        "applied on the device by its gather")
         # the captured graph bakes in: this memory's buffers, the batch size and training-mode (noisy) weights
         graphable = (self.use_cuda_graph and isinstance(mem, ReplayMemory) and mem.rng == "philox" and
                      self.online_net.training)

@@ -351,6 +351,8 @@ def _meta(agent, mem):
     hyper = dict(learning_rate=opt.lr, adam_eps=opt.eps, betas=list(opt.betas), norm_clip=agent.norm_clip,
                  discount=agent.discount, multi_step=agent.n, batch_size=agent.batch_size, V_min=agent.Vmin,
                  V_max=agent.Vmax)
+    if agent.augment_shift:   # only when on: manifests of runs without augmentation stay as they were
+        hyper["augment_shift"] = agent.augment_shift
     meta = dict(world_size=agent.sync.world_size, rank=agent.sync.rank, optimiser=sd["layout"],
                 structure=_structure(agent, mem), hyper_parameters=hyper, learner=learner, replay=None)
     if mem is not None:

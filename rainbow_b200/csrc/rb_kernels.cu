@@ -446,6 +446,25 @@ __device__ __forceinline__ float4 u8x4_to_unit(uint32_t w) {
                      __fdiv_rn((float)((w >> 16) & 0xffu), 255.0f), __fdiv_rn((float)(w >> 24), 255.0f));
 }
 
+// per-sample scalars, once per sample (memory.py:140-145)
+__device__ __forceinline__ void gather_scalars(uint64_t first, const int32_t* __restrict__ action, const float* __restrict__ reward,
+                                               const uint8_t* __restrict__ nonterminal, int64_t size, int64_t idx, int b,
+                                               int history, int n, const float* __restrict__ gamma_pow,
+                                               int64_t* __restrict__ actions, float* __restrict__ returns,
+                                               float* __restrict__ nonterminals) {
+  const int sa = history - 1;
+  actions[b] = (int64_t)__ldg(action + pymod(idx, size));  // slot H-1 is never blanked
+  float acc = 0.0f;
+  for (int k = 0; k < n; ++k) {
+    int sk = sa + k;
+    float r = slot_blank(first, sk, history) ? 0.0f : __ldg(reward + pymod(idx + k, size));
+    acc = __fadd_rn(acc, __fmul_rn(r, __ldg(gamma_pow + k)));
+  }
+  returns[b] = acc;
+  const int sl = history + n - 1;
+  nonterminals[b] = slot_blank(first, sl, history) ? 0.0f : (__ldg(nonterminal + pymod(idx + n, size)) ? 1.0f : 0.0f);
+}
+
 __global__ void __launch_bounds__(GATHER_THREADS)
 k_gather(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
          const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
@@ -488,19 +507,96 @@ k_gather(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timeste
       __stcs(dst_n + 4 * v + 0, a); __stcs(dst_n + 4 * v + 1, bq); __stcs(dst_n + 4 * v + 2, c); __stcs(dst_n + 4 * v + 3, d);
     }
   }
-  // per-sample scalars, once per sample (memory.py:140-145)
+  if (blockIdx.x == 0 && threadIdx.x == 0)
+    gather_scalars(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns, nonterminals);
+}
+
+// ================================================================================================
+// K2s gather_shift : k_gather + random-shift augmentation (DrQ): every observation is edge-padded by `pad` pixels and
+// cropped back to 84 x 84 at its own offset (oy, ox) in [0, 2 pad]:  out[y][x] = in[clamp(y+oy-pad)][clamp(x+ox-pad)].
+// ================================================================================================
+// Same grid and CTA-per-stored-frame mapping as k_gather, but the split is by output rows (at split 2 part 0 writes rows
+// [0, 42), part 1 rows [42, 84)).  The input rows those outputs can reach under any offset -- the CTA's rows and `pad` more
+// on either side -- are staged once in shared memory with 16-byte loads; then each appearance of the frame (state and/or
+// next state) is written from there with its own observation's offset.  An output row is 21 float4, so each streaming
+// float4 store lies inside one row.
+// Offsets: one Philox4x32-10 call per sample b, counter (c_lo, c_hi, b, SHIFT_STREAM) with c = *rng_counter (advanced by
+// rb_tree_sample just before), key = seed; words x, y -> the state's (oy, ox), z, w -> the next state's;
+// offset = (word * (2 pad + 1)) >> 32.
+constexpr int FRAME_SIDE = 84;
+constexpr int ROW_VEC = FRAME_SIDE / 4;              // float4 per output row
+constexpr uint32_t SHIFT_STREAM = 0x53484654u;       // "SHFT": apart from sampling (0x5A4D504C) and noise (0x4E4F4953 + i)
+
+__device__ __forceinline__ int clamp_px(int v) { return min(max(v, 0), FRAME_SIDE - 1); }
+
+__device__ __forceinline__ int shift_offset(uint32_t word, int pad) {
+  return (int)(((uint64_t)word * (uint64_t)(2 * pad + 1)) >> 32);
+}
+
+// four output pixels (y, x .. x+3) of a frame staged in shared memory, shifted by (dy, dx)
+__device__ __forceinline__ float4 shifted4(const uint8_t* s_frame, int y, int x, int dy, int dx) {
+  const uint8_t* row = s_frame + clamp_px(y + dy) * FRAME_SIDE;
+  return make_float4(__fdiv_rn((float)row[clamp_px(x + dx)], 255.0f), __fdiv_rn((float)row[clamp_px(x + 1 + dx)], 255.0f),
+                     __fdiv_rn((float)row[clamp_px(x + 2 + dx)], 255.0f), __fdiv_rn((float)row[clamp_px(x + 3 + dx)], 255.0f));
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_shift(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+               const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+               const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+               float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+               float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
+               const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
+  __shared__ uint64_t s_first;
+  __shared__ __align__(16) uint8_t s_frame[RB_FRAME_BYTES];
+  const int b = blockIdx.y;
+  const int W = history + n;
+  const int used = blockIdx.x / split, part = blockIdx.x % split;
+  const int s = (n >= history && used >= history) ? n + (used - history) : used;
+  const int64_t idx = data_idx[b];
+  const int64_t pos = pymod(idx - (history - 1) + s, size);
+  const int rows = (FRAME_SIDE + split - 1) / split;
+  const int r0 = part * rows, r1 = min(FRAME_SIDE, r0 + rows);
+  // the 16-byte vectors covering input rows [r0 - pad, r1 + pad) (a frame starts on a 16-byte boundary: 7056 = 441 x 16)
+  const int v0 = max(r0 - pad, 0) * FRAME_SIDE / 16;
+  const int v1 = min(FRAME_VEC, (min(r1 + pad, FRAME_SIDE) * FRAME_SIDE + 15) / 16);
+  const uint4* src = reinterpret_cast<const uint4*>(frames + (size_t)pos * RB_FRAME_BYTES);
+  uint4 pre = make_uint4(0, 0, 0, 0);
+  if (v0 + (int)threadIdx.x < v1) pre = __ldg(src + v0 + threadIdx.x);
+  const unsigned long long c = *rng_counter;
+  if (threadIdx.x < 32) {
+    uint64_t f = window_first_bits(timestep, size, idx, history, W);
+    if (threadIdx.x == 0) s_first = f;
+  }
+  const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)b, SHIFT_STREAM),
+                                make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+  const int oy_s = shift_offset(r.x, pad), ox_s = shift_offset(r.y, pad);
+  const int oy_n = shift_offset(r.z, pad), ox_n = shift_offset(r.w, pad);
+  __syncthreads();
+  const uint64_t first = s_first;
+  const bool blank = slot_blank(first, s, history);
+  if (!blank) {
+    uint4* dst = reinterpret_cast<uint4*>(s_frame);
+    for (int v = v0 + threadIdx.x; v < v1; v += GATHER_THREADS) dst[v] = (v == v0 + (int)threadIdx.x) ? pre : __ldg(src + v);
+  }
+  __syncthreads();
+
+  float4* dst_s = (s < history) ? reinterpret_cast<float4*>(states + ((size_t)b * history + s) * RB_FRAME_BYTES) : nullptr;
+  float4* dst_n = (s >= n && s < n + history)
+                      ? reinterpret_cast<float4*>(next_states + ((size_t)b * history + (s - n)) * RB_FRAME_BYTES)
+                      : nullptr;
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = r0 * ROW_VEC + threadIdx.x; i < r1 * ROW_VEC; i += GATHER_THREADS) {
+    const int y = i / ROW_VEC, x = (i - y * ROW_VEC) * 4;
+    if (dst_s) __stcs(dst_s + i, blank ? zero : shifted4(s_frame, y, x, oy_s - pad, ox_s - pad));
+    if (dst_n) __stcs(dst_n + i, blank ? zero : shifted4(s_frame, y, x, oy_n - pad, ox_n - pad));
+  }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    const int sa = history - 1;
-    actions[b] = (int64_t)__ldg(action + pymod(idx, size));  // slot H-1 is never blanked
-    float acc = 0.0f;
-    for (int k = 0; k < n; ++k) {
-      int sk = sa + k;
-      float r = slot_blank(first, sk, history) ? 0.0f : __ldg(reward + pymod(idx + k, size));
-      acc = __fadd_rn(acc, __fmul_rn(r, __ldg(gamma_pow + k)));
-    }
-    returns[b] = acc;
-    const int sl = W - 1;
-    nonterminals[b] = slot_blank(first, sl, history) ? 0.0f : (__ldg(nonterminal + pymod(idx + n, size)) ? 1.0f : 0.0f);
+    gather_scalars(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns, nonterminals);
+    int32_t* sh_s = shifts + 2 * (size_t)b;          // int32 [2][B][2]: (side, sample, (oy, ox))
+    int32_t* sh_n = shifts + 2 * ((size_t)B + b);
+    sh_s[0] = oy_s; sh_s[1] = ox_s;
+    sh_n[0] = oy_n; sh_n[1] = ox_n;
   }
 }
 
@@ -1617,16 +1713,39 @@ static int gather_split(int ctas_without_split) {
   return split;
 }
 
+// the argument checks of rb_gather, shared with rb_gather_shift
+static int gather_check(const char* who, const uint8_t* frames, const int32_t* timestep, const int32_t* action,
+                        const float* reward, const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B,
+                        int history, int n, const float* gamma_pow, const float* states, const float* next_states,
+                        const int64_t* actions, const float* returns, const float* nonterminals) {
+  char what[96];
+  if (!frames || !timestep || !action || !reward || !nonterminal || !data_idx || !gamma_pow || !states || !next_states ||
+      !actions || !returns || !nonterminals) {
+    snprintf(what, sizeof what, "%s: null pointer", who);
+    return fail(RB_ERR_INVAL, what);
+  }
+  if (B <= 0 || history <= 0 || n <= 0 || size <= 0) {
+    snprintf(what, sizeof what, "%s: sizes must be positive", who);
+    return fail(RB_ERR_INVAL, what);
+  }
+  if (history + n > RB_MAX_WINDOW) {
+    snprintf(what, sizeof what, "%s: history + n exceeds RB_MAX_WINDOW", who);
+    return fail(RB_ERR_RANGE, what);
+  }
+  if (B > 65535) {
+    snprintf(what, sizeof what, "%s: B exceeds 65535", who);
+    return fail(RB_ERR_RANGE, what);
+  }
+  return RB_OK;
+}
+
 int rb_gather(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
               const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n,
               const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
               float* nonterminals, rb_stream_t stream) {
-  if (!frames || !timestep || !action || !reward || !nonterminal || !data_idx || !gamma_pow || !states || !next_states ||
-      !actions || !returns || !nonterminals)
-    return fail(RB_ERR_INVAL, "rb_gather: null pointer");
-  if (B <= 0 || history <= 0 || n <= 0 || size <= 0) return fail(RB_ERR_INVAL, "rb_gather: sizes must be positive");
-  if (history + n > RB_MAX_WINDOW) return fail(RB_ERR_RANGE, "rb_gather: history + n exceeds RB_MAX_WINDOW");
-  if (B > 65535) return fail(RB_ERR_RANGE, "rb_gather: B exceeds 65535");
+  const int rc = gather_check("rb_gather", frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n,
+                              gamma_pow, states, next_states, actions, returns, nonterminals);
+  if (rc != RB_OK) return rc;
   const int used = (history + n < 2 * history) ? history + n : 2 * history;
   const int split = gather_split(used * B);
   dim3 grid(used * split, B);
@@ -1635,6 +1754,26 @@ int rb_gather(const uint8_t* frames, const int32_t* timestep, const int32_t* act
                                                               B, history, n, gamma_pow, states, next_states, actions,
                                                               returns, nonterminals, split); }
   return check_launch("rb_gather");
+}
+
+int rb_gather_shift(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                    const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n,
+                    const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
+                    float* nonterminals, int pad, uint64_t seed, const uint64_t* rng_counter, int32_t* shifts,
+                    rb_stream_t stream) {
+  const int rc = gather_check("rb_gather_shift", frames, timestep, action, reward, nonterminal, size, data_idx, B, history,
+                              n, gamma_pow, states, next_states, actions, returns, nonterminals);
+  if (rc != RB_OK) return rc;
+  if (!rng_counter || !shifts) return fail(RB_ERR_INVAL, "rb_gather_shift: null pointer");
+  if (pad < 1 || pad > RB_MAX_SHIFT_PAD) return fail(RB_ERR_RANGE, "rb_gather_shift: pad outside [1, RB_MAX_SHIFT_PAD]");
+  const int used = (history + n < 2 * history) ? history + n : 2 * history;
+  const int split = gather_split(used * B);
+  dim3 grid(used * split, B);
+  { ProfScope prof_(RB_K_GATHER_SHIFT, (cudaStream_t)stream);
+    k_gather_shift<<<grid, GATHER_THREADS, 0, (cudaStream_t)stream>>>(
+      frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states, next_states, actions,
+      returns, nonterminals, split, pad, seed, (const unsigned long long*)rng_counter, shifts); }
+  return check_launch("rb_gather_shift");
 }
 
 int rb_iter_states(const uint8_t* frames, const int32_t* timestep, int64_t size, int64_t first, int count, int history,

@@ -8,6 +8,8 @@ called through the C ABI in include/rainbow_b200.h:
     append             -> rb_append        (K5)   memory.py:105-108, 56-61
     sample             -> rb_tree_sample   (K1)   memory.py:124-132, 148-154
                           rb_gather        (K2)   memory.py:111-121, 134-146
+                          (rb_gather_shift with shift_pad > 0: the same plus random-shift augmentation, no reference
+                          counterpart)
     update_priorities  -> rb_tree_update   (K4)   memory.py:157-159, 23-48
     __next__           -> rb_iter_states          memory.py:166-178
 
@@ -222,6 +224,7 @@ class _SampleWorkspace:
         self.returns = torch.empty(B, dtype=f32, device=device)
         self.nonterminals = torch.empty((B, 1), dtype=f32, device=device)
         self.status = torch.zeros(4, dtype=torch.int32, device=device)   # ok flag, draws used, rejected batches so far, -
+        self.shifts = None   # int32 [2][B][2] offsets of the last augmented gather (allocated by the first one)
 
     def as_tuple(self):
         return (self.tree_idx, self.states, self.actions, self.returns, self.next_states, self.nonterminals,
@@ -236,6 +239,7 @@ class ReplayMemory:
     max_attempts times -- costs a device synchronisation)."""
 
     APPEND_BATCH = 8  # RB_APPEND_BATCH
+    MAX_SHIFT_PAD = 16  # RB_MAX_SHIFT_PAD
 
     def __init__(self, args, capacity, rng="philox", seed=None, max_attempts=64, strict=False, defer_appends=False):
         self.device = _require_cuda(args.device)
@@ -370,25 +374,46 @@ class ReplayMemory:
             _lib.ptr(self._beta_dev), self.max_attempts, _lib.ptr(ws.probs), _lib.ptr(ws.data_idx), _lib.ptr(ws.tree_idx),
             _lib.ptr(ws.weights), _lib.ptr(ws.status), _lib.stream()))
 
-    def _launch_gather(self, ws):
-        tr = self.transitions
-        _lib.check(self._lib.rb_gather(
-            _lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action), _lib.ptr(tr.reward),
-            _lib.ptr(tr.nonterminal), tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, self.n,
-            _lib.ptr(self.n_step_scaling), _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions),
-            _lib.ptr(ws.returns), _lib.ptr(ws.nonterminals), _lib.stream()))
+    def _check_shift_pad(self, shift_pad):
+        shift_pad = int(shift_pad)
+        if not 0 <= shift_pad <= self.MAX_SHIFT_PAD:
+            raise ValueError(f"shift_pad must be in [0, {self.MAX_SHIFT_PAD}], got {shift_pad}")
+        if shift_pad and self.rng == "numpy":
+            raise ValueError("shift_pad > 0 needs rng='philox': the offsets are drawn from the device stream (the reference "
+                             "has no augmentation, so there is no numpy stream to reproduce)")
+        return shift_pad
 
-    def sample_into(self, ws):
+    def _launch_gather(self, ws, shift_pad=0):
+        tr = self.transitions
+        common = (_lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action), _lib.ptr(tr.reward),
+                  _lib.ptr(tr.nonterminal), tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, self.n,
+                  _lib.ptr(self.n_step_scaling), _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions),
+                  _lib.ptr(ws.returns), _lib.ptr(ws.nonterminals))
+        if not shift_pad:
+            _lib.check(self._lib.rb_gather(*common, _lib.stream()))
+            return
+        if ws.shifts is None:
+            ws.shifts = torch.empty((2, ws.B, 2), dtype=torch.int32, device=self.device)
+        _lib.check(self._lib.rb_gather_shift(*common, shift_pad, self.seed, _lib.ptr(self._rng_counter), _lib.ptr(ws.shifts),
+                                             _lib.stream()))
+
+    def sample_into(self, ws, shift_pad=0):
         """Device-RNG sample into caller-owned buffers: two launches, no synchronisation (graph capturable).
-        The caller is responsible for push_beta() and flush_appends() (outside any graph capture)."""
+        The caller is responsible for push_beta() and flush_appends() (outside any graph capture).
+        shift_pad = p > 0 (at most MAX_SHIFT_PAD) augments the states and next states by random shifts (DrQ): each
+        observation edge-padded by p pixels and cropped back to 84 x 84 at its own offset drawn on the device
+        (rb_gather_shift); `ws.shifts` receives the offsets.  0 gathers exactly as the reference does."""
+        shift_pad = self._check_shift_pad(shift_pad)
         self._launch_sample(ws)
-        self._launch_gather(ws)
+        self._launch_gather(ws, shift_pad)
         self._last = ws
         return ws.as_tuple()
 
-    def sample(self, batch_size):
+    def sample(self, batch_size, shift_pad=0):
         """memory.py:148-155.  Returns (tree_idxs, states, actions, returns, next_states, nonterminals, weights),
-        all device tensors (the reference returns tree_idxs as numpy; update_priorities takes either)."""
+        all device tensors (the reference returns tree_idxs as numpy; update_priorities takes either).
+        shift_pad: random-shift augmentation as in sample_into(); needs rng="philox" (ValueError otherwise)."""
+        shift_pad = self._check_shift_pad(shift_pad)
         ws = _SampleWorkspace(int(batch_size), self.history, self.device)
         self.flush_appends()
         self.push_beta()
@@ -404,7 +429,7 @@ class ReplayMemory:
             self._launch_gather(ws)
             self._last = ws
             return ws.as_tuple()
-        out = self.sample_into(ws)
+        out = self.sample_into(ws, shift_pad)
         if self.strict:
             self.check_last_sample()
         return out
