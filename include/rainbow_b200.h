@@ -31,7 +31,7 @@
  *   reward       float32[size]
  *   nonterminal  uint8[size]
  *   ring_state   int64[5]  {head (next write slot), full (0/1), t_episode, appended_total, launch ticket of
- *                          rb_append_batch (zero between launches)}
+ *                          rb_append / rb_append_batch (zero between launches)}
  *   running_max  float32[1] largest exponentiated priority seen (memory.py:20,48)
  *   rng_counter  uint64[1]  Philox draw counter, advanced by the kernels themselves
  *                           (so a replayed CUDA graph draws fresh numbers)
@@ -45,7 +45,7 @@
 extern "C" {
 #endif
 
-#define RB_ABI_VERSION 2
+#define RB_ABI_VERSION 3
 
 #define RB_OK 0
 #define RB_ERR_INVAL (-22)       /* bad argument (EINVAL) */
@@ -151,7 +151,7 @@ int rb_iter_states(const uint8_t* frames, const int32_t* timestep, int64_t size,
  * quantise the newest frame (f32*255, truncating cast), store the record at ring_state.head with
  * timestep = ring_state.t_episode, set its leaf to *running_max and walk to the root, advance the
  * head, set full on wrap, t_episode = terminal ? 0 : t_episode+1.
- * state_last_frame: float32[84*84] device pointer (state[-1]). */
+ * state_last_frame: float32[84*84] device pointer (state[-1]).  The same launch as rb_append_batch with k = 1. */
 int rb_append(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
               float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max,
               const float* state_last_frame, int32_t action_value, float reward_value, int terminal,
@@ -226,12 +226,13 @@ typedef struct rb_head_grads {   /* gradients are OVERWRITTEN (not accumulated) 
 int rb_head_splits(int conv_features, int hidden, int* s1, int* s2);
 int rb_head_ticket_count(void);
 /* Whether the fused head takes this shape, without touching the device: RB_OK, or the code rb_head_forward over `rows`
- * rows (rows > 0) and rb_head_backward over `backward_batch` rows (backward_batch > 0) would return for it with valid
- * pointers.  rows == 0 / backward_batch == 0 leave that call out.  Both calls check these limits before they launch
+ * rows (rows > 0) and rb_head_backward over `backward_batch` rows (backward_batch > 0, up to 512) would return for it with
+ * valid pointers.  rows == 0 / backward_batch == 0 leave that call out.  Both calls check these limits before they launch
  * anything: a refused backward writes nothing. */
 int rb_head_supported(int conv_features, int hidden, int atoms, int actions, int rows, int backward_batch);
 /* probes / tests only: bit 0 skips the layer-1 launch of rb_head_forward, bit 1 the layer-2 launch, bit 2 forces the FFMA
- * layer-1 kernel instead of the tensor-core one, bit 3 the split-K layer-2 kernel instead of the single-pass one (0 = normal) */
+ * layer-1 kernel instead of the tensor-core one, bit 3 the split-K layer-2 kernel instead of the single-pass one, bit 4
+ * makes rb_head_backward run its large-batch layer-1 kernels at every B (0 = normal) */
 int rb_head_debug(int flags);
 
 /* Forward over M = m_lo + m_hi rows (x_lo: [m_lo][conv_features], x_hi: [m_hi][conv_features] or NULL).
@@ -246,10 +247,14 @@ int rb_head_forward(const rb_head_params* p, const float* x_lo, int m_lo, const 
 /* q[M][actions][atoms] = zv + za - mean_a(za) (model.py:75) from z. */
 int rb_head_logits(const float* z, int M, int actions, int atoms, float* q, rb_stream_t stream);
 
-/* Backward for B <= 32 rows, hidden <= 1024 and actions * atoms small enough for the dh kernel's shared memory (about
- * 1060; rb_head_supported says which shapes): given dz[B][atoms*(1+actions)] (value block first), x[B][conv_features] and h[B][2*hidden]
- * writes all 16 parameter gradients through `g` and dx[B][conv_features].  dh_scratch: float32[(B + 32) * 2*hidden]
- * (dh [B][2*hidden], then its transpose [2*hidden][32] for the layer-1 kernel).
+/* Backward for 1 <= B <= 512 rows, hidden <= 1024 and actions * atoms small enough for the dh kernel's shared memory
+ * (about 1060; rb_head_supported says which shapes): given dz[B][atoms*(1+actions)] (value block first),
+ * x[B][conv_features] and h[B][2*hidden] writes all 16 parameter gradients through `g` and dx[B][conv_features].
+ * dh_scratch: float32[(B + Bp) * 2*hidden], Bp = B rounded up to a multiple of 32 (dh [B][2*hidden], then its transpose
+ * [2*hidden][Bp] with the columns past B zero, for the layer-1 kernels).
+ * Layer 1 has two implementations with the same outputs, and the call picks by B: up to 32 rows one pass over W1 makes
+ * the weight gradients and dx together (k_head_bwd1); above that they run as two GEMM-shaped tensor-core launches,
+ * weight gradients reduced over the batch, then dx reduced over both streams' rows (k_head_bwd1_wgrad, k_head_bwd1_dx).
  * relu_mask_x != 0 additionally zeroes dx where x <= 0, i.e. folds in the backward of the ReLU that produced the conv
  * features (model.py:59), so dx is the gradient w.r.t. the last conv layer's pre-activation.
  * `parts` selects which of the three launches to enqueue (so a caller can put the independent layer-2 weight
@@ -261,18 +266,6 @@ int rb_head_logits(const float* z, int M, int actions, int atoms, float* q, rb_s
 #define RB_HEAD_BWD_ALL 7
 int rb_head_backward(const rb_head_params* p, const rb_head_grads* g, const float* x, const float* h, const float* dz, int B,
                      float* dh_scratch, float* dx, int relu_mask_x, int parts, rb_stream_t stream);
-
-/* What rb_head_backward_large returns for this shape with valid pointers, without touching the device: RB_OK for
- * 1 <= B <= 512, hidden <= 1024 and the dh kernel's actions * atoms limit (the same as rb_head_backward's). */
-int rb_head_large_supported(int conv_features, int hidden, int atoms, int actions, int B);
-/* The same backward as rb_head_backward (same outputs, `parts` bits and relu_mask_x) for 1 <= B <= 512 rows: layer 1 runs
- * as two GEMM-shaped tensor-core launches (weight gradients reduced over the batch, dx reduced over both streams' rows)
- * instead of k_head_bwd1's single pass.  dh_scratch: float32[(B + Bp) * 2*hidden], Bp = B rounded up to a multiple of 32
- * (dh [B][2*hidden], then its transpose [2*hidden][Bp] with the columns past B zero); at B <= 32 the layout of
- * rb_head_backward.  It runs its own layer-1 kernels at every B.  The shape check runs before any launch: a refused call
- * writes nothing. */
-int rb_head_backward_large(const rb_head_params* p, const rb_head_grads* g, const float* x, const float* h, const float* dz,
-                           int B, float* dh_scratch, float* dx, int relu_mask_x, int parts, rb_stream_t stream);
 
 /* agent.py:53-55 Agent.act / :110-112 evaluate_q after the network body, for M states at once: from the head output
  * z[M][atoms*(1+actions)] computes q[m][a] = sum_z support_z * softmax_z(zv + za[a] - mean_a za) (model.py:75-79) and its

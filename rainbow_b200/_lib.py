@@ -54,8 +54,6 @@ SIGNATURES = {
     "rb_head_forward": (C.c_int, [_hp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rb_head_logits": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp]),
     "rb_head_backward": (C.c_int, [_hp, _hg, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _vp]),
-    "rb_head_large_supported": (C.c_int, [_i32, _i32, _i32, _i32, _i32]),
-    "rb_head_backward_large": (C.c_int, [_hp, _hg, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _vp]),
     "rb_bias_grad": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp]),
     "rb_conv_wgrad_scratch_elems": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _i32]),
     "rb_conv_wgrad": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
@@ -105,7 +103,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError if the .so does not export a declared symbol
         fn.restype = res
         fn.argtypes = args
-    if lib.rb_abi_version() != 2:
+    if lib.rb_abi_version() != 3:
         raise RainbowB200Error("librainbow_b200.so ABI version mismatch")
     _lib = lib
     return lib

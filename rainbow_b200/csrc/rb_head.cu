@@ -622,6 +622,7 @@ k_head_dh(const __grid_constant__ HeadDesc d, const float* __restrict__ dz, cons
 constexpr int B1_K = 32;   // k columns per CTA
 constexpr int B1_O = 32;   // rows of W1 per chunk
 constexpr int B1_T = 256;  // threads
+constexpr int B1_MAX_B = 32;   // batch rows (one 32-row tile); rb_head_backward runs the large-batch kernels above it
 
 constexpr int B1_STAGES = 3;                 // cp.async ring: two chunks in flight ahead of the one being consumed (3 CTAs per SM: one wave)
 // Row strides (floats) chosen for the mma.m16n8k8 fragment loads: "A" tiles (rows indexed by lane / 4, columns by lane % 4)
@@ -820,10 +821,10 @@ k_head_bwd1(const __grid_constant__ HeadDesc d, const __grid_constant__ HeadGrad
 }
 
 // ------------------------------------------------------------------------------------------------
-// Layer-1 backward for 1 <= B <= 512 rows (rb_head_backward_large).  At these batch sizes the two products are real GEMMs
-// (3.3 GFLOP each at conv_features 3136, hidden 512, B 512), and the dh chunk alone would need 128 KB per ring stage in
-// k_head_bwd1's one-pass structure, so they run as two launches, both as error-compensated TF32 on mma.sync (the same
-// arithmetic as k_head_bwd1) with fp32 accumulation:
+// Layer-1 backward for 1 <= B <= 512 rows (rb_head_backward runs it above 32 rows).  At these batch sizes the two
+// products are real GEMMs (3.3 GFLOP each at conv_features 3136, hidden 512, B 512), and the dh chunk alone would need
+// 128 KB per ring stage in k_head_bwd1's one-pass structure, so they run as two launches, both as error-compensated TF32
+// on mma.sync (the same arithmetic as k_head_bwd1) with fp32 accumulation:
 //   k_head_bwd1_wgrad: g[o][k] = sum_m dhT[o][m] * x[m][k] per stream, g_sigma = g * eps_out[o] eps_in[k]; CTA tile
 //                      64 o x 64 k; the batch is reduced in 32-row steps through a 3-stage cp.async ring, inside the CTA in
 //                      a fixed order (no atomics, no split across CTAs).  The k-tile-0 CTAs also write the bias gradients.
@@ -1246,10 +1247,10 @@ k_conv_wgrad_reduce(const float* __restrict__ part, int n_part, int n_w, int n_b
   }
 }
 
-// Every shape limit of rb_head_forward (rows > 0) and rb_head_backward (backward: over bwd_batch rows; large: the limits
-// of rb_head_backward_large instead), checked before anything is launched; rb_head_supported / rb_head_large_supported
-// export it so callers can pick another path instead of meeting the error mid-update.
-int head_shape_check(int K1, int H, int Z, int A, int rows, int bwd_batch, bool backward, bool large = false) {
+// Every shape limit of rb_head_forward (rows > 0) and rb_head_backward (backward: over bwd_batch rows), checked before
+// anything is launched; rb_head_supported exports it so callers can pick another path instead of meeting the error
+// mid-update.  Both layer-1 implementations of the backward share these limits.
+int head_shape_check(int K1, int H, int Z, int A, int rows, int bwd_batch, bool backward) {
   if (K1 <= 0 || H <= 0 || Z <= 1 || A <= 0 || rows < 0) return rbi::fail(RB_ERR_INVAL, "rb_head: bad size");
   if (K1 % 32 || H % 64) return rbi::fail(RB_ERR_RANGE, "rb_head: conv_features % 32 == 0 and hidden % 64 == 0 required");
   if (rows > 0) {
@@ -1259,10 +1260,7 @@ int head_shape_check(int K1, int H, int Z, int A, int rows, int bwd_batch, bool 
     if (mt > 65535 || mt * tiles1 > 2048 || mt * tiles2 > 2048) return rbi::fail(RB_ERR_RANGE, "rb_head_forward: too many rows");
   }
   if (backward) {
-    if (large && (bwd_batch <= 0 || bwd_batch > BL_MAX_B))
-      return rbi::fail(RB_ERR_RANGE, "rb_head_backward_large: 1 <= B <= 512 required");
-    if (!large && (bwd_batch <= 0 || bwd_batch > 32))
-      return rbi::fail(RB_ERR_RANGE, "rb_head_backward: 1 <= B <= 32 required (rb_head_backward_large takes up to 512)");
+    if (bwd_batch <= 0 || bwd_batch > BL_MAX_B) return rbi::fail(RB_ERR_RANGE, "rb_head_backward: 1 <= B <= 512 required");
     const long long ns_max = (long long)A * Z > Z ? (long long)A * Z : Z;
     const long long ld_dz = ns_max | 1;
     const long long smem = (32 * ld_dz + 2 * ((ns_max + 3) & ~3ll) * DH_KB) * (long long)sizeof(float);
@@ -1293,15 +1291,14 @@ int head_check(const rb_head_params* p, const char* who) {
   return RB_OK;
 }
 
-// The checks and gradient pointers both backward entry points share; the shape check runs before anything is launched.
+// The argument checks and gradient pointers of rb_head_backward; the shape check runs before anything is launched.
 int head_bwd_prepare(const rb_head_params* p, const rb_head_grads* gr, const float* x, const float* h, const float* dz, int B,
-                     const float* dh_scratch, const float* dx, int parts, bool large, HeadGrads* g) {
-  const char* who = large ? "rb_head_backward_large: null pointer or bad size" : "rb_head_backward: null pointer or bad size";
-  int rc = head_check(p, who);
+                     const float* dh_scratch, const float* dx, int parts, HeadGrads* g) {
+  int rc = head_check(p, "rb_head_backward: null pointer or bad size");
   if ((parts & 7) == 0) return rbi::fail(RB_ERR_INVAL, "rb_head_backward: parts must select at least one of RB_HEAD_BWD_*");
   if (rc != RB_OK) return rc;
   if (!gr || !x || !h || !dz || !dh_scratch || !dx) return rbi::fail(RB_ERR_INVAL, "rb_head_backward: null pointer");
-  rc = head_shape_check(p->conv_features, p->hidden, p->atoms, p->actions, 0, B, true, large);   // all limits, whatever `parts` selects
+  rc = head_shape_check(p->conv_features, p->hidden, p->atoms, p->actions, 0, B, true);   // all limits, whatever `parts` selects
   if (rc != RB_OK) return rc;
   for (int s = 0; s < 2; ++s) {
     if (!gr->w1_mu[s] || !gr->w1_sigma[s] || !gr->b1_mu[s] || !gr->b1_sigma[s] || !gr->w2_mu[s] || !gr->w2_sigma[s] ||
@@ -1313,7 +1310,7 @@ int head_bwd_prepare(const rb_head_params* p, const rb_head_grads* gr, const flo
   return RB_OK;
 }
 
-// Layer-2 launches of both backward entry points: k_head_wgrad2 (any B) and k_head_dh over ceil(B / 32) batch tiles,
+// Layer-2 launches of rb_head_backward: k_head_wgrad2 (any B) and k_head_dh over ceil(B / 32) batch tiles,
 // writing dh [B][2H] and dhT [2H][ldT] to dh_scratch.
 int head_bwd_layer2(const HeadDesc& d, const HeadGrads& g, const float* dz, const float* h, int B, float* dh_scratch, int ldT,
                     int parts, cudaStream_t st) {
@@ -1376,7 +1373,9 @@ int rb_head_supported(int conv_features, int hidden, int atoms, int actions, int
   return head_shape_check(conv_features, hidden, atoms, actions, rows, backward_batch, backward_batch != 0);
 }
 
-static int g_head_debug = 0;   // bit 0: skip the layer-1 launch, bit 1: skip the layer-2 launch (timing probes only); bit 2: FFMA layer 1; bit 3: split-K layer 2
+// bit 0: skip the layer-1 launch, bit 1: skip the layer-2 launch (timing probes only); bit 2: FFMA layer 1; bit 3: split-K
+// layer 2; bit 4: large-batch layer-1 backward at every B
+static int g_head_debug = 0;
 int rb_head_debug(int flags) {
   g_head_debug = flags;
   return RB_OK;
@@ -1447,57 +1446,41 @@ int rb_head_logits(const float* z, int M, int actions, int atoms, float* q, rb_s
 int rb_head_backward(const rb_head_params* p, const rb_head_grads* gr, const float* x, const float* h, const float* dz, int B,
                      float* dh_scratch, float* dx, int relu_mask_x, int parts, rb_stream_t stream) {
   HeadGrads g;
-  int rc = head_bwd_prepare(p, gr, x, h, dz, B, dh_scratch, dx, parts, false, &g);
+  int rc = head_bwd_prepare(p, gr, x, h, dz, B, dh_scratch, dx, parts, &g);
   if (rc != RB_OK) return rc;
   const HeadDesc d = to_desc(p);
   cudaStream_t st = (cudaStream_t)stream;
-  rc = head_bwd_layer2(d, g, dz, h, B, dh_scratch, 32, parts, st);
-  if (rc != RB_OK) return rc;
-  if (parts & RB_HEAD_BWD_LAYER1) {   // hidden <= 1024 (EoAll holds H / 2 factors): head_shape_check
+  const int Bp = (B + BL_R - 1) / BL_R * BL_R;   // columns of dhT: 32 = B1_MAX_B whenever k_head_bwd1 runs
+  rc = head_bwd_layer2(d, g, dz, h, B, dh_scratch, Bp, parts, st);
+  if (rc != RB_OK || !(parts & RB_HEAD_BWD_LAYER1)) return rc;
+  const float* dhT = dh_scratch + (size_t)B * 2 * d.H;
+  // hidden <= 1024 (k_head_bwd1's EoAll holds H / 2 factors, k_head_bwd1_dx's 2H): head_shape_check
+  if (B <= B1_MAX_B && !(g_head_debug & 16)) {
     dim3 grid(d.K1 / B1_K, 4);
     rbi::ProfScope prof_(RB_K_HEAD_BWD1, st);
     const size_t smem_b1 = (size_t)B1_STAGES * B1_STAGE * sizeof(float);
     rc = rbi::ensure_dynamic_smem(k_head_bwd1, smem_b1, "rb_head_backward");
     if (rc != RB_OK) return rc;
-    k_head_bwd1<<<grid, B1_T, smem_b1, st>>>(d, g, x, dh_scratch, dh_scratch + (size_t)B * 2 * d.H, B, dx, relu_mask_x);
+    k_head_bwd1<<<grid, B1_T, smem_b1, st>>>(d, g, x, dh_scratch, dhT, B, dx, relu_mask_x);
+    return rbi::check_launch("rb_head_backward(bwd1)");
   }
-  return rbi::check_launch("rb_head_backward(bwd1)");
-}
-
-int rb_head_large_supported(int conv_features, int hidden, int atoms, int actions, int B) {
-  return head_shape_check(conv_features, hidden, atoms, actions, 0, B, true, true);
-}
-
-int rb_head_backward_large(const rb_head_params* p, const rb_head_grads* gr, const float* x, const float* h, const float* dz,
-                           int B, float* dh_scratch, float* dx, int relu_mask_x, int parts, rb_stream_t stream) {
-  HeadGrads g;
-  int rc = head_bwd_prepare(p, gr, x, h, dz, B, dh_scratch, dx, parts, true, &g);
+  const size_t smem_w = (size_t)BL_STAGES * BLW_STAGE * sizeof(float);
+  const size_t smem_x = (size_t)BL_STAGES * BLX_STAGE * sizeof(float);
+  rc = rbi::ensure_dynamic_smem(k_head_bwd1_wgrad, smem_w, "rb_head_backward");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_head_bwd1_dx, smem_x, "rb_head_backward");
   if (rc != RB_OK) return rc;
-  const HeadDesc d = to_desc(p);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int Bp = (B + BL_R - 1) / BL_R * BL_R;
-  rc = head_bwd_layer2(d, g, dz, h, B, dh_scratch, Bp, parts, st);
-  if (rc != RB_OK) return rc;
-  if (parts & RB_HEAD_BWD_LAYER1) {   // hidden <= 1024 (k_head_bwd1_dx's EoAll holds 2H factors): head_shape_check
-    const float* dhT = dh_scratch + (size_t)B * 2 * d.H;
-    const size_t smem_w = (size_t)BL_STAGES * BLW_STAGE * sizeof(float);
-    const size_t smem_x = (size_t)BL_STAGES * BLX_STAGE * sizeof(float);
-    rc = rbi::ensure_dynamic_smem(k_head_bwd1_wgrad, smem_w, "rb_head_backward_large");
-    if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_head_bwd1_dx, smem_x, "rb_head_backward_large");
-    if (rc != RB_OK) return rc;
-    const int ktiles = (d.K1 + BL_NT - 1) / BL_NT;
-    {
-      rbi::ProfScope prof_(RB_K_HEAD_BWD1_WGRAD, st);
-      k_head_bwd1_wgrad<<<dim3(ktiles, 2 * d.H / BL_MT), BL_T, smem_w, st>>>(d, g, x, dhT, B, Bp);
-    }
-    rc = rbi::check_launch("rb_head_backward_large(wgrad1)");
-    if (rc != RB_OK) return rc;
-    {
-      rbi::ProfScope prof_(RB_K_HEAD_BWD1_DX, st);
-      k_head_bwd1_dx<<<dim3((B + BL_MT - 1) / BL_MT, ktiles), BL_T, smem_x, st>>>(d, x, dh_scratch, B, dx, relu_mask_x);
-    }
+  const int ktiles = (d.K1 + BL_NT - 1) / BL_NT;
+  {
+    rbi::ProfScope prof_(RB_K_HEAD_BWD1_WGRAD, st);
+    k_head_bwd1_wgrad<<<dim3(ktiles, 2 * d.H / BL_MT), BL_T, smem_w, st>>>(d, g, x, dhT, B, Bp);
   }
-  return rbi::check_launch("rb_head_backward_large(dx)");
+  rc = rbi::check_launch("rb_head_backward(wgrad1)");
+  if (rc != RB_OK) return rc;
+  {
+    rbi::ProfScope prof_(RB_K_HEAD_BWD1_DX, st);
+    k_head_bwd1_dx<<<dim3((B + BL_MT - 1) / BL_MT, ktiles), BL_T, smem_x, st>>>(d, x, dh_scratch, B, dx, relu_mask_x);
+  }
+  return rbi::check_launch("rb_head_backward(dx)");
 }
 
 int rb_bias_grad(const float* grad_out, int B, int C, int HW, float* out, rb_stream_t stream) {

@@ -626,84 +626,12 @@ k_iter_states(const uint8_t* __restrict__ frames, const int32_t* __restrict__ ti
 }
 
 // ================================================================================================
-// K5  append : quantise + store one transition, set its leaf to the running max, walk to the root.
+// K5  append : up to RB_APPEND_BATCH transitions in ONE launch (rb_append: one; rb_append_batch: the actor's queue,
+// SURVEY 8(f).2).  Each is quantised and stored, its leaf set to the running max, and the tree walked to the root.
 // ================================================================================================
 constexpr int APPEND_THREADS = 256;
 
-__global__ void __launch_bounds__(APPEND_THREADS)
-k_append(float* tree, int64_t tree_start, int64_t size, uint8_t* __restrict__ frames, int32_t* timestep,
-         int32_t* action, float* reward, uint8_t* nonterminal, int64_t* ring_state, const float* running_max,
-         const float* __restrict__ state_last, int32_t action_value, float reward_value, int terminal) {
-  const int64_t head = ring_state[0];
-  const int64_t t_ep = ring_state[2];
-  const int tid = threadIdx.x;
-  // frame: f32 * 255 then truncating cast (memory.py:106); 4 pixels per thread-iteration
-  uint32_t* dst = reinterpret_cast<uint32_t*>(frames + (size_t)head * RB_FRAME_BYTES);
-  const float4* src = reinterpret_cast<const float4*>(state_last);
-  {  // all of a thread's loads in flight at once: the frame may sit in pinned host memory (a PCIe round trip per load)
-    constexpr int PER = (RB_FRAME_BYTES / 4 + APPEND_THREADS - 1) / APPEND_THREADS;   // 7
-    float4 x[PER];
-#pragma unroll
-    for (int u = 0; u < PER; ++u) {
-      const int v = tid + u * APPEND_THREADS;
-      x[u] = (v < RB_FRAME_BYTES / 4) ? src[v] : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-#pragma unroll
-    for (int u = 0; u < PER; ++u) {
-      const int v = tid + u * APPEND_THREADS;
-      if (v < RB_FRAME_BYTES / 4) {
-        uint32_t a = (uint32_t)(uint8_t)(int)__fmul_rn(x[u].x, 255.0f);
-        uint32_t b = (uint32_t)(uint8_t)(int)__fmul_rn(x[u].y, 255.0f);
-        uint32_t c = (uint32_t)(uint8_t)(int)__fmul_rn(x[u].z, 255.0f);
-        uint32_t d = (uint32_t)(uint8_t)(int)__fmul_rn(x[u].w, 255.0f);
-        dst[v] = a | (b << 8) | (c << 16) | (d << 24);
-      }
-    }
-  }
-  if (tid < 32) {
-    // warp 0: the walk.  All siblings along the path are independent of the new value, so lane j
-    // fetches the sibling at level j (one round trip), then lane 0 chains the float32 additions
-    // child + sibling (commutative, so left/right order does not matter bit-wise).
-    const int L = tree_depth(tree_start);
-    const float value = *running_max;  // memory.py:107: new transitions get the max priority
-    const int64_t leaf = head + tree_start;
-    float sib = 0.0f;
-    if (tid < L) {
-      int64_t node = leaf;
-      for (int j = 0; j < tid; ++j) node = (node - 1) >> 1;
-      int64_t sibling = (node & 1) ? node + 1 : node - 1;  // odd = left child
-      sib = __ldcg(tree + sibling);
-    }
-    float acc = value;
-    int64_t node = leaf;
-    if (tid == 0) __stcg(tree + node, acc);
-    for (int j = 0; j < L; ++j) {
-      float sj = __shfl_sync(0xffffffffu, sib, j);
-      acc = __fadd_rn(acc, sj);
-      node = (node - 1) >> 1;
-      if (tid == 0) __stcg(tree + node, acc);
-    }
-    if (tid == 0) {
-      timestep[head] = (int32_t)t_ep;
-      action[head] = action_value;
-      reward[head] = reward_value;
-      nonterminal[head] = terminal ? 0 : 1;
-    }
-  }
-  __syncthreads();
-  if (tid == 0) {
-    int64_t nh = head + 1 == size ? 0 : head + 1;
-    ring_state[0] = nh;
-    if (nh == 0) ring_state[1] = 1;
-    ring_state[2] = terminal ? 0 : t_ep + 1;
-    ring_state[3] = ring_state[3] + 1;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// K5b  append_batch : up to RB_APPEND_BATCH queued transitions in ONE launch (actor side, SURVEY 8(f).2).
-// ------------------------------------------------------------------------------------------------
-// Equivalent to calling k_append k times in order: the records go to slots head, head+1, ... (mod size), the
+// Equivalent to k single appends in order: the records go to slots head, head+1, ... (mod size), the
 // in-episode counter follows the terminals, every new leaf gets the running max (which appends never change) and,
 // because every internal node is recomputed from its children, the tree after k sequential walks equals the tree
 // after ONE level-synchronous batched walk over the k leaves (same argument as for rb_tree_update).  The frame
@@ -1629,6 +1557,16 @@ int adam_ctas(int64_t P) {
   return (int)want;
 }
 
+// The launch of rb_append and rb_append_batch, after each has checked its own arguments.
+int append_launch(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
+                  float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max, const AppendBatch& ab,
+                  rb_stream_t stream, const char* who) {
+  { ProfScope prof_(RB_K_APPEND, (cudaStream_t)stream);
+    k_append_batch<<<ab.k, APPEND_THREADS, 0, (cudaStream_t)stream>>>(tree, tree_start, size, frames, timestep, action,
+                                                                      reward, nonterminal, ring_state, running_max, ab); }
+  return check_launch(who);
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1793,13 +1731,18 @@ int rb_append(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, in
   if (!tree || !frames || !timestep || !action || !reward || !nonterminal || !ring_state || !running_max || !state_last_frame)
     return fail(RB_ERR_INVAL, "rb_append: null pointer");
   if (size <= 0 || (size & 1)) return fail(RB_ERR_INVAL, "rb_append: an even size is required");
-  if (tree_depth(tree_start) > 32) return fail(RB_ERR_RANGE, "rb_append: tree deeper than 32 levels");  // one lane per level
+  // k_append_batch's limit; a deeper tree holds more than 2^30 transitions (7.6 TB of frames), which no replay reaches
+  if (tree_depth(tree_start) > 30) return fail(RB_ERR_RANGE, "rb_append: tree deeper than 30 levels");
   if (((uintptr_t)state_last_frame & 15) != 0) return fail(RB_ERR_INVAL, "rb_append: state_last_frame must be 16-byte aligned");
-  { ProfScope prof_(RB_K_APPEND, (cudaStream_t)stream);
-    k_append<<<1, APPEND_THREADS, 0, (cudaStream_t)stream>>>(tree, tree_start, size, frames, timestep, action, reward,
-                                                           nonterminal, ring_state, running_max, state_last_frame,
-                                                           action_value, reward_value, terminal); }
-  return check_launch("rb_append");
+  AppendBatch ab;
+  memset(&ab, 0, sizeof(ab));
+  ab.k = 1;
+  ab.frame[0] = state_last_frame;
+  ab.action[0] = action_value;
+  ab.reward[0] = reward_value;
+  ab.terminal[0] = terminal ? 1 : 0;
+  return append_launch(tree, tree_start, size, frames, timestep, action, reward, nonterminal, ring_state, running_max, ab,
+                       stream, "rb_append");
 }
 
 int rb_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
@@ -1822,10 +1765,8 @@ int rb_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* fram
     ab.reward[j] = rewards[j];
     ab.terminal[j] = terminals[j] ? 1 : 0;
   }
-  { ProfScope prof_(RB_K_APPEND, (cudaStream_t)stream);
-    k_append_batch<<<k, APPEND_THREADS, 0, (cudaStream_t)stream>>>(tree, tree_start, size, frames, timestep, action, reward,
-                                                                   nonterminal, ring_state, running_max, ab); }
-  return check_launch("rb_append_batch");
+  return append_launch(tree, tree_start, size, frames, timestep, action, reward, nonterminal, ring_state, running_max, ab,
+                       stream, "rb_append_batch");
 }
 
 int rb_c51_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,

@@ -93,9 +93,6 @@ def resample_noise(layers, seed, rng_counter, x_in=None, x_out=None):
 
 @functools.lru_cache(maxsize=None)
 def _head_shape_rc(conv_features, hidden, atoms, actions, rows, backward_batch):
-    if backward_batch > FusedHead.SMALL_BATCH:   # forward limits from rb_head_supported, backward from rb_head_large_supported
-        return (_lib.load().rb_head_supported(conv_features, hidden, atoms, actions, rows, 0) or
-                _lib.load().rb_head_large_supported(conv_features, hidden, atoms, actions, backward_batch))
     return _lib.load().rb_head_supported(conv_features, hidden, atoms, actions, rows, backward_batch)
 
 
@@ -103,7 +100,6 @@ class FusedHead:
     """Launcher of the fused noisy dueling head kernels for one DQN (csrc/rb_head.cu)."""
 
     MAX_ROWS = 4096
-    SMALL_BATCH = 32   # backward batches up to this size run rb_head_backward (k_head_bwd1), larger ones rb_head_backward_large
 
     def __init__(self, net):
         self.net = net
@@ -118,8 +114,7 @@ class FusedHead:
     @staticmethod
     def supported(net, rows=1, backward_batch=0):
         """Whether the fused kernels take this net's head over `rows` forward rows and, if backward_batch > 0, a backward
-        over that many rows (rb_head_supported; above SMALL_BATCH rows the backward's limits are rb_head_large_supported's);
-        atoms <= 128 is what rb_q_values and the fused C51 loss take."""
+        over that many rows, up to 512 (rb_head_supported); atoms <= 128 is what rb_q_values and the fused C51 loss take."""
         return (net.atoms <= 128 and next(net.parameters()).is_cuda and
                 _head_shape_rc(net.conv_output_size, net.hidden_size, net.atoms, net.action_space, rows, backward_batch) == 0)
 
@@ -190,11 +185,11 @@ class FusedHead:
         return B + -(-B // 32) * 32
 
     def backward(self, p, x, h, dz, dh_scratch, dx, relu_mask_x=False, parts=7):
+        """rb_head_backward over the B = x.shape[0] rows; the library picks the layer-1 kernels for B."""
         g = self.grads()
-        B = x.shape[0]
-        fn = self.lib.rb_head_backward if B <= self.SMALL_BATCH else self.lib.rb_head_backward_large
-        _lib.check(fn(C.byref(p), C.byref(g), _lib.ptr(x), _lib.ptr(h), _lib.ptr(dz), B, _lib.ptr(dh_scratch), _lib.ptr(dx),
-                      1 if relu_mask_x else 0, parts, _lib.stream()))
+        _lib.check(self.lib.rb_head_backward(C.byref(p), C.byref(g), _lib.ptr(x), _lib.ptr(h), _lib.ptr(dz), x.shape[0],
+                                             _lib.ptr(dh_scratch), _lib.ptr(dx), 1 if relu_mask_x else 0, parts,
+                                             _lib.stream()))
         return dx
 
 

@@ -33,7 +33,7 @@ def test_abi_exports_every_declared_symbol():
     assert declared == set(_lib.SIGNATURES), "python binding table and header disagree"
     for name in declared:
         assert hasattr(lib, name), f"librainbow_b200.so does not export {name}"
-    assert lib.rb_abi_version() == 2
+    assert lib.rb_abi_version() == 3
     assert lib.rb_clip_adam_scratch_elems() > 0
 
 
@@ -93,7 +93,9 @@ def test_head_supported_without_gpu():
     assert lib.rb_head_supported(576, 2048, 51, 6, 64, 0) == 0
     assert lib.rb_head_supported(576, 1024, 51, 6, 4096, 0) == 0          # 64 row tiles x 32 layer-1 tiles = 2048 tickets
     assert lib.rb_head_supported(576, 2048, 51, 6, 4096, 0) == -34        # 64 x 64 > 2048
-    assert lib.rb_head_supported(576, 256, 51, 6, 64, 33) == -34          # backward batch > 32
+    assert lib.rb_head_supported(576, 256, 51, 6, 64, 33) == 0            # the backward's batch: 1 to 512
+    assert lib.rb_head_supported(576, 256, 51, 6, 64, 512) == 0
+    assert lib.rb_head_supported(576, 256, 51, 6, 64, 513) == -34
     assert lib.rb_head_supported(576, 96, 51, 6, 64, 0) == -34            # hidden % 64
     assert lib.rb_head_supported(48, 256, 51, 6, 64, 0) == -34            # conv_features % 32
     assert lib.rb_head_supported(576, 256, 1, 6, 64, 0) == -22            # atoms > 1

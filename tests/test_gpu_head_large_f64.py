@@ -1,14 +1,16 @@
-"""The large-batch backward of the fused noisy dueling head (rb_head_backward_large: k_head_wgrad2, k_head_dh over 32-row
-batch tiles, k_head_bwd1_wgrad, k_head_bwd1_dx) through its C ABI against the float64 reference of tests/head_ref.py, per
-element (|err| <= tau * scale), in the harness style of tests/test_gpu_head_f64.py:
+"""The large-batch backward of the fused noisy dueling head (rb_head_backward with the layer-1 kernels it runs above 32
+rows: k_head_wgrad2, k_head_dh over 32-row batch tiles, k_head_bwd1_wgrad, k_head_bwd1_dx; rb_head_debug bit 4 makes it
+run them at every B) through its C ABI against the float64 reference of tests/head_ref.py, per element
+(|err| <= tau * scale), in the harness style of tests/test_gpu_head_f64.py:
 
  * B in {1, 31, 32, 33, 64, 100, 255, 256, 511, 512} x hidden {64, 512, 1024}, conv_features cycling {576, 3136, 64},
    (actions, atoms) cycling BWD_AZ (actions * atoms up to 1062: the dh kernel's eps_out fallback), all ReLU-mask / eval
    combinations, and C4's learner shape (3136 / 512 / 6 / 51 / B 512);
  * NaN-prefilled outputs, guard rows past B, the dhT layout [2H][round_up(B, 32)] with its zero columns, a second launch
    and a CUDA-graph replay bitwise identical to an eager launch, the kernels read from the graph's kernel nodes;
- * at B <= 32 against rb_head_backward: dh and dhT bitwise equal, the other outputs within tau;
- * rb_head_large_supported agrees with the call, and a refused call writes nothing;
+ * without the debug bit the call runs these kernels above 32 rows, with the same outputs bitwise, and k_head_bwd1 at
+   B <= 32: dh and dhT bitwise equal, the other outputs within tau;
+ * rb_head_supported agrees with the call up to and past B 512, and a refused call writes nothing;
  * the learner at batch 512 against the unmodified reference (tests/golden/update_c4.npz, oracle/gen_update_c4.py),
    graph replay == eager at batch 64 and 512, and the shapes whose fused backward is refused updating on the library path.
 The tensor-core bounds are TAU_LARGE_WGRAD / TAU_LARGE_DX of tests/test_large_batch_tf32_numerics.py.  Observed largest
@@ -45,16 +47,20 @@ def large_kernels_of(dot):
 
 
 def backward(hd, x, h, dz, B, relu, large=True, parts=7):
-    """One rb_head_backward(_large) launch into NaN-filled outputs; returns (rc, grads, dh scratch, dx)."""
+    """One rb_head_backward launch into NaN-filled outputs; returns (rc, grads, dh scratch, dx).  large=True sets
+    rb_head_debug bit 4 for the call (the large-batch layer-1 kernels at every B); large=False lets the call choose."""
     H, K1 = hd.H, hd.K1
-    rows = B + (bp(B) if large else 32)
     grads = {f"{k}.{s}": torch.full_like(hd.p[k][s], NAN) for k in R.PARAMS for s in range(2)}
-    dh_s = torch.full((rows * 2 * H + GUARD,), NAN, device=DEV)        # dh [B][2H], dhT [2H][Bp], guard
+    dh_s = torch.full(((B + bp(B)) * 2 * H + GUARD,), NAN, device=DEV)   # dh [B][2H], dhT [2H][Bp], guard
     dx = torch.full((B + GUARD, K1), NAN, device=DEV)
     L = lib()
-    fn = L.rb_head_backward_large if large else L.rb_head_backward
-    rc = fn(C.byref(hd.ps), C.byref(grads_struct(grads)), x.data_ptr(), h.data_ptr(), dz.data_ptr(), B, dh_s.data_ptr(),
-            dx.data_ptr(), 1 if relu else 0, parts, stream())
+    if large:
+        L.rb_head_debug(16)
+    try:
+        rc = L.rb_head_backward(C.byref(hd.ps), C.byref(grads_struct(grads)), x.data_ptr(), h.data_ptr(), dz.data_ptr(), B,
+                                dh_s.data_ptr(), dx.data_ptr(), 1 if relu else 0, parts, stream())
+    finally:
+        L.rb_head_debug(0)
     return rc, grads, dh_s, dx
 
 
@@ -129,31 +135,41 @@ def test_head_backward_large_f64(case, tmp_path):
     for k in grads:
         assert torch.equal(grads_g[k], grads[k]), f"{k}: graph replay == eager launch"
 
-    if B <= 32:   # the two implementations: same layer-2 kernels, different layer-1 kernels
-        rc_s, grads_s, dh_ss, dx_s = backward(hd, x, h, dz, B, relu, large=False)
-        assert rc_s == 0
-        assert torch.equal(dh_ss[:n], dh_s[:n]), "dh and dhT bitwise equal to rb_head_backward's"
+    # without the debug bit: the large-batch kernels above 32 rows, k_head_bwd1 at B <= 32 (same layer-2 kernels)
+    _, (rc_d, grads_d, dh_d, dx_d), dot = graph_kernels(lambda: backward(hd, x, h, dz, B, relu, large=False),
+                                                        tmp_path / "bwd_default.dot")
+    assert rc_d == 0
+    ran = large_kernels_of(dot)
+    assert torch.equal(dh_d[:n], dh_s[:n]), "dh and dhT bitwise equal to the large-batch kernels' run"
+    if B > 32:
+        assert ran == dict(wgrad2=True, dh=True, wgrad1=True, dx=True, small_bwd1=False), ran
+        assert torch.equal(dx_d[:B], dx[:B]), "the default call runs the same kernels"
+        for k in grads:
+            assert torch.equal(grads_d[k], grads[k]), f"{k}: the default call runs the same kernels"
+    else:
+        assert ran == dict(wgrad2=True, dh=True, wgrad1=False, dx=False, small_bwd1=True), ran
         refs = dict(list(ref2.items()) + list(ref1.items()))
         for k in grads:
-            R.assert_within(f"{k} vs rb_head_backward", grads[k], R._d(grads_s[k]), refs[k][1], tau_of(k))
-        R.assert_within("dx vs rb_head_backward", dx[:B], R._d(dx_s[:B]), refs["dx"][1], tau_of("dx"))
+            R.assert_within(f"{k} vs k_head_bwd1", grads[k], R._d(grads_d[k]), refs[k][1], tau_of(k))
+        R.assert_within("dx vs k_head_bwd1", dx[:B], R._d(dx_d[:B]), refs["dx"][1], tau_of("dx"))
 
 
 @pytest.mark.parametrize("H", [64, 1024, 1088, 2048])
 def test_head_large_supported_agrees_with_the_call(H):
-    """rb_head_large_supported(conv_features, hidden, atoms, actions, B) returns what rb_head_backward_large returns with
-    valid pointers, for every `parts`; a refused call leaves its NaN-filled outputs untouched."""
+    """rb_head_supported(conv_features, hidden, atoms, actions, 0, B) returns what rb_head_backward returns with valid
+    pointers at batch sizes past k_head_bwd1's 32 rows, for every `parts`; a refused call leaves its NaN-filled outputs
+    untouched."""
     L = lib()
     K1 = 32
     for A, Z in ((18, 59), (18, 60), (11, 101), (6, 51)):
         hd = Head(K1, H, Z, A, True, 5)
         for B in (33, 512, 513):
-            want = L.rb_head_large_supported(K1, H, Z, A, B)
+            want = L.rb_head_supported(K1, H, Z, A, 0, B)
             x = R.make_features(B, K1, 7, DEV)
             h = torch.rand(B, 2 * H, device=DEV)
             dz = torch.randn(B, hd.ncols, device=DEV)
             for parts in (1, 2, 4, 7):
-                got, grads, dh_s, dx = backward(hd, x, h, dz, B, True, parts=parts)
+                got, grads, dh_s, dx = backward(hd, x, h, dz, B, True, large=False, parts=parts)
                 assert got == want, (A, Z, B, parts, got, want)
                 if want != 0:
                     torch.cuda.synchronize()
@@ -319,7 +335,7 @@ def test_large_batch_update_graph_has_the_new_kernels(B, tmp_path):
 @pytest.mark.parametrize("B", [64, 512])
 def test_large_batch_graph_replay_equals_eager_bitwise(B):
     """2 eager warm-up updates + capture + replays leave parameters, Adam moments, priorities and losses bit-identical to
-    the same number of eager updates, at batch sizes that run rb_head_backward_large (cuDNN deterministic)."""
+    the same number of eager updates, at batch sizes that run the large-batch layer-1 kernels (cuDNN deterministic)."""
     def trajectory(use_graph, steps=6):
         ag = _agent(B, cuda_graph=use_graph)
         mem, _ = synthetic_ring(16384, seed=3, args=dict(batch_size=B))
@@ -349,7 +365,7 @@ def test_large_batch_graph_replay_equals_eager_bitwise(B):
 @pytest.mark.parametrize("B,hidden,A,Z", [(513, 512, 6, 51), (64, 2048, 6, 51), (64, 64, 18, 101)],
                          ids=["B513", "hidden2048", "A18-Z101"])
 def test_large_batch_library_path_where_the_fused_backward_refuses(B, hidden, A, Z):
-    """Batch 513, hidden 2048 and (A 18, Z 101) are outside rb_head_backward_large: the learner updates them on the library
+    """Batch 513, hidden 2048 and (A 18, Z 101) are outside rb_head_backward: the learner updates them on the library
     path, with the same result as fused_head=False, without raising."""
     from rainbow_b200.agent import Agent
 

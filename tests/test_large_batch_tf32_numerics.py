@@ -1,5 +1,5 @@
-"""Bounds of the tensor-core products of the large-batch layer-1 backward (rb_head_backward_large: k_head_bwd1_wgrad,
-k_head_bwd1_dx), derived in the IEEE model of tests/test_split_tf32_numerics.py at each product's own reduction shape:
+"""Bounds of the tensor-core products of the large-batch layer-1 backward (k_head_bwd1_wgrad, k_head_bwd1_dx, which
+rb_head_backward runs above 32 rows), derived in the IEEE model of tests/test_split_tf32_numerics.py at each product's own reduction shape:
 
  * the weight gradient g[o][k] = sum_m dh[m][o] x[m][k] is reduced over the whole batch inside one CTA: 64 and 512 batch
    rows;
@@ -10,7 +10,7 @@ Each bound must sit at least 5x above the largest per-element |err| / scale the 
 least 5x below the median of every cheaper variant (a correction term dropped, plain TF32).  tests/test_gpu_head_large_f64.py
 holds the kernels to these bounds against the float64 reference of tests/head_ref.py.
 
-Also the shape limits of rb_head_large_supported, which are host arithmetic."""
+Also the backward's shape limits in rb_head_supported, which are host arithmetic."""
 import numpy as np
 import pytest
 
@@ -57,22 +57,33 @@ def test_large_batch_tau_separates_3xtf32_from_degraded_variants(case):
 
 
 def test_head_large_supported_without_gpu():
-    """rb_head_large_supported is host arithmetic: 1 <= B <= 512, hidden <= 1024, the dh kernel's actions * atoms limit and
-    the forward's generic shape rules; rb_head_supported's own batch rule (B <= 32) is unchanged."""
+    """rb_head_supported(..., rows 0, B) is host arithmetic: 1 <= B <= 512, hidden <= 1024, the dh kernel's actions * atoms
+    limit and the forward's generic shape rules, the same at every batch size on both sides of k_head_bwd1's 32 rows."""
+    import ctypes as C
+
     from rainbow_b200 import _lib
     lib = _lib.load()
     for B in (1, 31, 32, 33, 64, 100, 256, 511, 512):
-        assert lib.rb_head_large_supported(3136, 512, 51, 6, B) == 0, B          # C4's learner at every batch size
-    assert lib.rb_head_large_supported(3136, 512, 51, 6, 513) == -34
-    assert lib.rb_head_large_supported(3136, 512, 51, 6, 0) == -34
-    assert lib.rb_head_large_supported(3136, 512, 51, 6, -1) == -34
-    assert lib.rb_head_large_supported(576, 1024, 51, 6, 512) == 0
-    assert lib.rb_head_large_supported(576, 1088, 51, 6, 512) == -34             # hidden <= 1024
-    assert lib.rb_head_large_supported(576, 2048, 51, 6, 64) == -34
-    assert lib.rb_head_large_supported(576, 64, 59, 18, 512) == 0                # dh kernel: 204 160 B of shared memory
-    assert lib.rb_head_large_supported(576, 64, 60, 18, 512) == -34              # 207 488 B
-    assert lib.rb_head_large_supported(576, 64, 101, 18, 64) == -34
-    assert lib.rb_head_large_supported(576, 96, 51, 6, 64) == -34                # hidden % 64
-    assert lib.rb_head_large_supported(48, 256, 51, 6, 64) == -34                # conv_features % 32
-    assert lib.rb_head_large_supported(576, 256, 1, 6, 64) == -22                # atoms > 1
-    assert lib.rb_head_supported(576, 256, 51, 6, 64, 33) == -34                 # the small backward still stops at 32
+        assert lib.rb_head_supported(3136, 512, 51, 6, 0, B) == 0, B            # C4's learner at every batch size
+    assert lib.rb_head_supported(3136, 512, 51, 6, 0, 513) == -34
+    assert lib.rb_head_supported(3136, 512, 51, 6, 0, -1) == -34
+    assert lib.rb_head_supported(576, 1024, 51, 6, 0, 512) == 0
+    assert lib.rb_head_supported(576, 1088, 51, 6, 0, 512) == -34               # hidden <= 1024
+    assert lib.rb_head_supported(576, 2048, 51, 6, 0, 64) == -34
+    assert lib.rb_head_supported(576, 64, 59, 18, 0, 512) == 0                  # dh kernel: 204 160 B of shared memory
+    assert lib.rb_head_supported(576, 64, 60, 18, 0, 512) == -34                # 207 488 B
+    assert lib.rb_head_supported(576, 64, 101, 18, 0, 64) == -34
+    assert lib.rb_head_supported(576, 96, 51, 6, 0, 64) == -34                  # hidden % 64
+    assert lib.rb_head_supported(48, 256, 51, 6, 0, 64) == -34                  # conv_features % 32
+    assert lib.rb_head_supported(576, 256, 1, 6, 0, 64) == -22                  # atoms > 1
+    assert lib.rb_head_supported(576, 256, 51, 6, 64, 33) == 0                  # past k_head_bwd1's 32 rows
+    # backward_batch 0 leaves the backward out of rb_head_supported; the call itself refuses 0 rows before any launch
+    assert lib.rb_head_supported(3136, 512, 51, 6, 0, 0) == 0
+    fake = 256                                                                   # never dereferenced: validation fails first
+    p, g = _lib.HeadParams(), _lib.HeadGrads()
+    for name, _ in _lib.HeadParams._fields_[:8]:
+        getattr(p, name)[:] = [fake, fake]
+    for name, _ in _lib.HeadGrads._fields_:
+        getattr(g, name)[:] = [fake, fake]
+    p.conv_features, p.hidden, p.atoms, p.actions = 3136, 512, 51, 6
+    assert lib.rb_head_backward(C.byref(p), C.byref(g), fake, fake, fake, 0, fake, fake, 1, 7, None) == -34

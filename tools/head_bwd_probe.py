@@ -1,12 +1,13 @@
 """Times the noisy head's backward at the canonical learner shape (conv_features 3136, hidden 512, 6 actions, 51 atoms)
 by batch size, with CUDA events after warm-up, on one GPU:
 
- * rb_head_backward (k_head_wgrad2, k_head_dh, k_head_bwd1) at B <= 32;
- * rb_head_backward_large (k_head_wgrad2, k_head_dh, k_head_bwd1_wgrad, k_head_bwd1_dx) at B in {8, 32, 64, 128, 256, 512};
+ * rb_head_backward with k_head_bwd1 as layer 1 (k_head_wgrad2, k_head_dh, k_head_bwd1) at B <= 32;
+ * rb_head_backward with the large-batch layer 1 (k_head_wgrad2, k_head_dh, k_head_bwd1_wgrad, k_head_bwd1_dx) at B in
+   {8, 32, 64, 128, 256, 512}, with rb_head_debug bit 4 forcing it at B <= 32;
  * the library head backward the learner runs when the fused head is off: autograd through W = mu + sigma * eps (fp32 GEMMs)
    back to the 16 parameters and the conv features.
 
-All three compute the same gradients.  The learner picks rb_head_backward up to 32 rows and rb_head_backward_large above;
+All three compute the same gradients.  rb_head_backward runs k_head_bwd1 up to 32 rows and the large-batch kernels above;
 this is the evidence for that threshold.  Prints the card's name and power limit with the numbers and writes them to
 tool_out/head_bwd_probe.json.
 
@@ -55,7 +56,7 @@ def time_us(fn, iters, warmup=20):
     return e0.elapsed_time(e1) * 1e3 / iters
 
 
-def fused(p, B, large):
+def fused(p, B):
     """A closure running one fused backward over B rows (all three parts, one stream)."""
     L = _lib.load()
     ps = _lib.HeadParams()
@@ -73,12 +74,21 @@ def fused(p, B, large):
     dz = torch.randn(B, Z * (1 + A), device=DEV) * 0.1
     dh = torch.empty((B + -(-B // 32) * 32) * 2 * H, device=DEV)
     dx = torch.empty(B, K1, device=DEV)
-    fn = L.rb_head_backward_large if large else L.rb_head_backward
     st = torch.cuda.current_stream().cuda_stream
 
     def run():
-        _lib.check(fn(C.byref(ps), C.byref(gs), x.data_ptr(), h.data_ptr(), dz.data_ptr(), B, dh.data_ptr(), dx.data_ptr(), 1, 7, st))
+        _lib.check(L.rb_head_backward(C.byref(ps), C.byref(gs), x.data_ptr(), h.data_ptr(), dz.data_ptr(), B, dh.data_ptr(), dx.data_ptr(), 1, 7, st))
     return run
+
+
+def time_fused_us(p, B, large, iters):
+    """time_us of the fused backward; large=True sets rb_head_debug bit 4 (the large-batch layer-1 kernels at every B)."""
+    L = _lib.load()
+    L.rb_head_debug(16 if large else 0)
+    try:
+        return time_us(fused(p, B), iters)
+    finally:
+        L.rb_head_debug(0)
 
 
 def library(p, B):
@@ -111,11 +121,11 @@ def main():
     p = R.make_head(K1, H, Z, A, True, 3, DEV)
     rows = []
     for B in (8, 32, 64, 128, 256, 512):
-        row = dict(B=B, large_us=time_us(fused(p, B, True), opts.iters), library_us=time_us(library(p, B), opts.iters))
+        row = dict(B=B, large_us=time_fused_us(p, B, True, opts.iters), library_us=time_us(library(p, B), opts.iters))
         if B <= 32:
-            row["small_us"] = time_us(fused(p, B, False), opts.iters)
+            row["small_us"] = time_fused_us(p, B, False, opts.iters)
         rows.append(row)
-        print(f"B {B:4d}: rb_head_backward {row.get('small_us', float('nan')):8.1f} us   rb_head_backward_large "
+        print(f"B {B:4d}: k_head_bwd1 layer 1 {row.get('small_us', float('nan')):8.1f} us   large-batch layer 1 "
               f"{row['large_us']:8.1f} us   library autograd {row['library_us']:8.1f} us", flush=True)
     os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
     with open(os.path.join(ROOT, "tool_out", "head_bwd_probe.json"), "w") as f:
