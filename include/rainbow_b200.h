@@ -59,6 +59,7 @@ extern "C" {
 #define RB_MAX_PEERS 8           /* ranks of one NVLink domain handled by rb_peer_clip_adam */
 #define RB_APPEND_BATCH 8        /* transitions per rb_append_batch launch */
 #define RB_MAX_SHIFT_PAD 16      /* largest pad of rb_gather_shift */
+#define RB_MAX_AUG_COPIES 8      /* most copies of a state (M) or next state (K) in rb_gather_aug */
 
 /* status words written by rb_tree_sample (int32[4]): status[0] = 1 if the batch now in the output buffers passed the
  * whole-batch validity test (memory.py:131), 0 otherwise; status[1] = draws used; status[2] = number of device-RNG
@@ -75,7 +76,7 @@ enum {
   RB_K_NOISY_RESAMPLE, RB_K_NOISY_COMPOSE, RB_K_SQNORM, RB_K_CLIP_ADAM, RB_K_HEAD_FC1, RB_K_HEAD_FC2, RB_K_HEAD_LOGITS,
   RB_K_HEAD_WGRAD2, RB_K_HEAD_DH, RB_K_HEAD_BWD1, RB_K_NOISE_FACTORS, RB_K_C51_DUELING, RB_K_BIAS_GRAD, RB_K_Q_VALUES,
   RB_K_HEAD_REDUCE1, RB_K_CONV_WGRAD, RB_K_HEAD_BWD1_WGRAD, RB_K_HEAD_BWD1_DX, RB_K_LEARN_STATS, RB_K_GATHER_SHIFT,
-  RB_KERNEL_COUNT
+  RB_K_GATHER_AUG, RB_K_C51_DUELING_AVG, RB_KERNEL_COUNT
 };
 
 int rb_abi_version(void);
@@ -141,6 +142,31 @@ int rb_gather_shift(const uint8_t* frames, const int32_t* timestep, const int32_
                     const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
                     float* nonterminals, int pad, uint64_t seed, const uint64_t* rng_counter, int32_t* shifts,
                     rb_stream_t stream);
+
+/* rb_gather_shift generalised to DrQ's K / M copies (Kostrikov et al. 2020, Algorithm 1) and SPR's intensity augmentation
+ * (Schwarzer et al. 2021); no reference counterpart.  Every sample's state is written m_copies = M times and its next state
+ * k_copies = K times, copy-major: states float32[M*B][history][84][84] (rows [jB, (j+1)B) hold copy j), next_states
+ * float32[K*B][...] the same way.  Each copy of each observation has its own shift offset (as rb_gather_shift; none when
+ * pad == 0) and its own intensity multiplier, the same for all of its history frames:
+ *   out[c][y][x] = fl32(in[c][clamp(y + oy - pad, 0, 83)][clamp(x + ox - pad, 0, 83)] * mult)
+ *   mult = fmaf(intensity, clamp(N(0, 1), -2, 2), 1)     (intensity == 0: mult = 1 and no multiply is done)
+ * where `in` is what rb_gather writes.  actions, returns and nonterminals are rb_gather's, bitwise.
+ * Draws, key `seed`, c = *rng_counter as the kernel reads it (not advanced by this call), for sample b and copy j:
+ *   offsets    Philox4x32-10 counter (c_lo, c_hi, b, 0x53484654 + j): x, y -> the state's (oy, ox), z, w -> the next
+ *              state's, offset = (word * (2 pad + 1)) >> 32 -- copy 0's are rb_gather_shift's;
+ *   multiplier Philox4x32-10 counter (c_lo, c_hi, b, 0x494E5453 + j) through Box-Muller: the first normal of (x, y) is the
+ *              state's, the first of (z, w) the next state's.
+ * shifts int32[2][copies][B][2] and scales float32[2][copies][B] (side: 0 = state, 1 = next state; copy; sample), copies =
+ * max(M, K), receive the draws (offsets 0 when pad == 0, multipliers 1 when intensity == 0); side 0 copies >= M and side 1
+ * copies >= K are drawn but not applied.
+ * RB_ERR_RANGE: pad outside [0, RB_MAX_SHIFT_PAD], intensity outside [0, 0.5] or not finite, m_copies or k_copies outside
+ * [1, RB_MAX_AUG_COPIES], plus every check of rb_gather; RB_ERR_INVAL: a NULL pointer, or pad 0 with intensity 0 and
+ * M = K = 1 (that is rb_gather).  A refused call launches nothing. */
+int rb_gather_aug(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                  const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n,
+                  const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
+                  float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
+                  const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream);
 
 /* memory.py:166-178 ReplayMemory.__next__, batched: states for current_idx = first .. first+count-1,
  * backward-only blanking, negative indices wrap.  out is float32[count][history][84*84]. */
@@ -294,6 +320,19 @@ int rb_c51_dueling_loss_grad(const float* z_online, const float* z_target, int a
                              const float* returns, const float* nonterminals, const float* weights, const float* support,
                              float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss, float* dz, float* m_out,
                              int64_t* astar_out, rb_stream_t stream);
+
+/* rb_c51_dueling_loss_grad with DrQ's averaging over K target copies and M online copies (Kostrikov et al. 2020,
+ * Algorithm 1).  z_online has (M + K) B rows: copy j of s at row jB + i, then copy k of s' at row (M + k) B + i; z_target
+ * K B rows, copy k of s' at row kB + i.  For sample i: a*_k is the double-DQN arg-max on online(s'_k) (first maximum wins)
+ * and m_k the projection of target(s'_k) at a*_k; m = (sum_k m_k, fp32 in k order) / K; loss_j = -sum m log p_j(a) for
+ * online(s_j); loss[i] = (sum_j loss_j) / M.  dz[M B][atoms*(1+actions)]: row jB + i is the gradient of online(s_j) with
+ * weight / (M B) in place of weight / B.  m_out [B][atoms] (optional) receives m, astar_out [K][B] (optional) a*_k.
+ * At M = K = 1 every output equals rb_c51_dueling_loss_grad's, bitwise.  RB_ERR_RANGE: M or K outside
+ * [1, RB_MAX_AUG_COPIES], plus rb_c51_dueling_loss_grad's limits with M + 2K staged rows.  A refused call writes nothing. */
+int rb_c51_dueling_avg_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                 const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                                 const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int M,
+                                 int K, float* loss, float* dz, float* m_out, int64_t* astar_out, rb_stream_t stream);
 
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */

@@ -4,11 +4,15 @@ One `learn(mem)` (agent.py:61-100) is:
 
     K1 rb_tree_sample + K2 rb_gather          (mem.sample, memory.py:148-155)
                                               [args.augment_shift = p > 0: rb_gather_shift instead -- random-shift
-                                               augmentation of s and s' (DrQ), offsets drawn on the device]
+                                               augmentation of s and s' (DrQ), offsets drawn on the device;
+                                               args.augment_intensity > 0 or augment_m / augment_k > 1: rb_gather_aug --
+                                               shift + intensity augmentation of M copies of s and K copies of s']
     3 x conv body (torch: cuDNN)              (agent.py:66,71,75 -> model.py:70-71)
     K6 rb_noisy_resample (target net)         (agent.py:74)
     fused noisy dueling heads (rb_head_forward) on the conv features -- online net on [s; s'], target on s'
     K3 rb_c51_dueling_loss_grad               (agent.py:67,72-73,76-96 + softmax halves of model.py:76-79 + model.py:75)
+                                              [M or K > 1: rb_c51_dueling_avg_loss_grad -- DrQ's target averaged over
+                                               the K copies of s', loss over the M copies of s]
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
@@ -60,6 +64,21 @@ def c51_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns
         _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
         float(gamma_n), B, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), _lib.stream()))
+    return loss, dz
+
+
+def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin,
+                              vmax, delta_z, gamma_n, M, K, m_out=None, astar_out=None):
+    """DrQ's K / M averaging (rb_c51_dueling_avg_loss_grad): z_online [(M + K) B, Z(1+A)] (M copies of s, then K copies of
+    s', copy-major), z_target [K B, Z(1+A)]; returns (loss[B], dz[M B, Z(1+A)]): the loss averaged over the M online
+    copies against the target averaged over the K target copies, and its gradient for every online copy of s."""
+    B = actions.shape[0]
+    loss = torch.empty(B, dtype=torch.float32, device=actions.device)
+    dz = torch.empty((M * B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
+    _lib.check(_lib.load().rb_c51_dueling_avg_loss_grad(
+        _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+        _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
+        float(gamma_n), B, M, K, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), _lib.stream()))
     return loss, dz
 
 
@@ -177,6 +196,15 @@ class Agent:
         self.augment_shift = int(getattr(args, "augment_shift", 0) or 0)
         if not 0 <= self.augment_shift <= ReplayMemory.MAX_SHIFT_PAD:
             raise ValueError(f"augment_shift must be in [0, {ReplayMemory.MAX_SHIFT_PAD}], got {self.augment_shift}")
+        # intensity augmentation (SPR: 1 + s * clip(N(0, 1), -2, 2) per observation, s = 0.05; 0 = off) and DrQ's K / M
+        # averaging: the target over K augmented copies of s', the loss over M copies of s (1 / 1 = one copy, as today)
+        self.augment_intensity = float(getattr(args, "augment_intensity", 0.0) or 0.0)
+        if not 0.0 <= self.augment_intensity <= ReplayMemory.MAX_INTENSITY:
+            raise ValueError(f"augment_intensity must be in [0, {ReplayMemory.MAX_INTENSITY}], got {self.augment_intensity}")
+        self.augment_copies = (int(getattr(args, "augment_m", 1)), int(getattr(args, "augment_k", 1)))
+        if not all(1 <= c <= ReplayMemory.MAX_AUG_COPIES for c in self.augment_copies):
+            raise ValueError(f"augment_m and augment_k must be in [1, {ReplayMemory.MAX_AUG_COPIES}], got "
+                             f"{self.augment_copies}")
 
         self.online_net = DQN(args, self.action_space).to(device=self.device)
         model_path = getattr(args, "model", None)
@@ -370,19 +398,22 @@ class Agent:
 
     # ---- the update ------------------------------------------------------------------------------
     def _fused_path(self, B):
+        """Whether an update over B samples runs on the fused head: (M + K) B online rows forward, M B backward, with the
+        agent's augment_m / augment_k copies (1 / 1: [s; s'] and s)."""
         on = self.online_net
-        return (self.use_fused_head and on.training and on.fused_ok(2 * B, backward_batch=B) and
-                self.target_net.fused_ok(B))
+        M, K = self.augment_copies
+        return (self.use_fused_head and on.training and on.fused_ok((M + K) * B, backward_batch=M * B) and
+                self.target_net.fused_ok(K * B))
 
     @staticmethod
     def _adjacent(states, next_states):
-        """The [2B, ...] tensor whose halves are `states` and `next_states`, if they are laid out that way."""
-        if (states.is_contiguous() and next_states.is_contiguous() and states.shape == next_states.shape and
+        """The tensor whose two parts are `states` and `next_states`, in that order, if they are laid out that way."""
+        if (states.is_contiguous() and next_states.is_contiguous() and states.shape[1:] == next_states.shape[1:] and
                 next_states.data_ptr() == states.data_ptr() + states.numel() * states.element_size() and
                 states._base is not None and states._base is next_states._base):
             base = states._base
-            if base.data_ptr() == states.data_ptr() and base.numel() == 2 * states.numel():
-                return base.view((2 * states.shape[0],) + tuple(states.shape[1:]))
+            if base.data_ptr() == states.data_ptr() and base.numel() == states.numel() + next_states.numel():
+                return base.view((states.shape[0] + next_states.shape[0],) + tuple(states.shape[1:]))
         return None
 
     def _side_streams(self):
@@ -395,10 +426,15 @@ class Agent:
         The three network passes are independent until the loss, and every conv kernel of this size leaves most of the
         132 SMs of an H100 idle, so they run as three concurrent branches (fork/join with events; inside the captured CUDA graph
         they become parallel branches): online(s) with autograd on the caller's stream, online(s') and the whole
-        target pass (noise draw, convs, head) on two side streams."""
+        target pass (noise draw, convs, head) on two side streams.
+        DrQ's K / M: `states` may hold M copies of the B sampled states and `next_states` K copies of the next states
+        (copy-major); the online pass then runs over all (M + K) B rows, the target pass over K B rows, and the backward
+        over the M B rows of s."""
         idxs, states, actions, returns, next_states, nonterminals, weights = batch
         on, tg = self.online_net, self.target_net
-        B = states.shape[0]
+        B = actions.shape[0]
+        Bs = states.shape[0]                 # M B rows of s
+        M, K = Bs // B, next_states.shape[0] // B
         main = torch.cuda.current_stream(self.device)
         s_ns, s_tg = self._side_streams()
         fork = torch.cuda.Event()
@@ -427,9 +463,9 @@ class Agent:
         if both is not None:
             with torch.no_grad():
                 acts2 = on.conv_forward_saving(both)
-                acts = [a[:B] for a in acts2]              # the s half (batch-major: contiguous slices) feeds the backward
-                x_both = acts2[-1].view(2 * B, -1)
-                x_s, xs_d = x_both[:B], x_both[:B]
+                acts = [a[:Bs] for a in acts2]             # the s rows (batch-major: contiguous slices) feed the backward
+                x_both = acts2[-1].view(Bs + next_states.shape[0], -1)
+                x_s, xs_d = x_both[:Bs], x_both[:Bs]
                 if noise_done is not None:
                     main.wait_event(noise_done)
                 z_on, h_on, p_on = on.head().forward(x_both)              # rows [0,B) = s, [B,2B) = s'
@@ -443,7 +479,7 @@ class Agent:
             if manual:
                 with torch.no_grad():
                     acts = on.conv_forward_saving(states)  # library kernels, backward scheduled by hand below
-                x_s = acts[-1].view(B, -1)
+                x_s = acts[-1].view(Bs, -1)
             else:
                 x_s = on.features(states)                  # autograd graph: convs only
             with torch.no_grad():
@@ -456,9 +492,14 @@ class Agent:
                 main.wait_event(done_tg)
         with torch.no_grad():
             m = torch.empty((B, self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
-            loss, dz = c51_dueling_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals, weights,
-                                             self.support, self.Vmin, self.Vmax, self.delta_z, self.discount ** self.n,
-                                             m_out=m)
+            if (M, K) == (1, 1):
+                loss, dz = c51_dueling_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
+                                                 weights, self.support, self.Vmin, self.Vmax, self.delta_z,
+                                                 self.discount ** self.n, m_out=m)
+            else:
+                loss, dz = c51_dueling_avg_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
+                                                     weights, self.support, self.Vmin, self.Vmax, self.delta_z,
+                                                     self.discount ** self.n, M, K, m_out=m)
             stats_done = self._stats_batch(batch, loss, m, z=z_on) if m is not None else None
             wb_done = None
             if after_loss is not None:
@@ -471,7 +512,7 @@ class Agent:
                     after_loss(loss)
                     wb_done = torch.cuda.Event()
                     wb_done.record(s_ns)
-            dh = torch.empty((FusedHead.dh_rows(B), 2 * on.hidden_size), dtype=torch.float32, device=self.device)   # dh, then its transpose
+            dh = torch.empty((FusedHead.dh_rows(Bs), 2 * on.hidden_size), dtype=torch.float32, device=self.device)   # dh, then its transpose
             dx = torch.empty_like(xs_d)
             if manual:
                 # dx comes back already masked by the last conv layer's ReLU; conv gradients are overwritten.
@@ -481,10 +522,10 @@ class Agent:
                 dz_ready.record(main)
                 with torch.cuda.stream(s_tg):
                     s_tg.wait_event(dz_ready)
-                    hd.backward(p_on, xs_d, h_on[:B], dz, dh, dx, parts=hd.BWD_WGRAD2)
+                    hd.backward(p_on, xs_d, h_on[:Bs], dz, dh, dx, parts=hd.BWD_WGRAD2)
                     w2_done = torch.cuda.Event()
                     w2_done.record(s_tg)
-                hd.backward(p_on, xs_d, h_on[:B], dz, dh, dx, relu_mask_x=True, parts=hd.BWD_DH | hd.BWD_LAYER1)
+                hd.backward(p_on, xs_d, h_on[:Bs], dz, dh, dx, relu_mask_x=True, parts=hd.BWD_DH | hd.BWD_LAYER1)
                 main.wait_event(w2_done)
                 head_ready = None
                 if self.sync.enabled:
@@ -510,7 +551,7 @@ class Agent:
                     main.wait_event(head_reduced)
             else:
                 self.optimiser.zero_conv_grad()
-                on.head().backward(p_on, xs_d, h_on[:B], dz, dh, dx)       # writes the 16 head gradients + dx
+                on.head().backward(p_on, xs_d, h_on[:Bs], dz, dh, dx)      # writes the 16 head gradients + dx
         if not manual:
             x_s.backward(dx)
             self.sync.all_reduce_(self.optimiser.flat_grad)
@@ -526,8 +567,12 @@ class Agent:
         given, is called as soon as the losses exist (the fused path runs it on a side stream).  `gate`: the sample's
         status words; a rejected batch leaves the parameters untouched (world 1)."""
         self._step_gate = gate if self.sync.world_size == 1 else None
-        if self._fused_path(batch[1].shape[0]):
+        B = batch[2].shape[0]
+        copies = (batch[1].shape[0] // B, batch[4].shape[0] // B)
+        if self._fused_path(B):
             return self._update_fused(batch, target_noise, after_loss)
+        if copies != (1, 1):
+            raise self._copies_error(copies)
         idxs, states, actions, returns, next_states, nonterminals, weights = batch
         q_s = self.online_net.logits(states)
         with torch.no_grad():
@@ -551,9 +596,17 @@ class Agent:
             after_loss(loss)
         return loss
 
+    @staticmethod
+    def _copies_error(copies):
+        return _lib.RainbowB200Error(
+            f"augment_m / augment_k = {copies} needs the fused head's update (args.fused_head = True, training mode, "
+            f"augment_m * batch_size <= 512 and a shape the fused head takes); the library head trains on one copy of s and "
+            f"s' only")
+
     def _learn_eager(self, mem):
         if isinstance(mem, ReplayMemory):
-            batch = mem.sample(self.batch_size, shift_pad=self.augment_shift)
+            batch = mem.sample(self.batch_size, shift_pad=self.augment_shift, intensity=self.augment_intensity,
+                               copies=self.augment_copies)
             gate = mem.sample_gate()
             return self._update_from_batch(batch, after_loss=lambda loss: mem.update_priorities(batch[0], loss, gate=gate),
                                            gate=gate)
@@ -565,13 +618,14 @@ class Agent:
     def _capture(self, mem):
         """Record one whole update (sample -> ... -> priority write-back) into a CUDA graph.  Capturing does
         not execute; the caller replays."""
-        ws = _SampleWorkspace(self.batch_size, mem.history, self.device)
+        ws = _SampleWorkspace(self.batch_size, mem.history, self.device, self.augment_copies)
         mem.flush_appends()
         mem.push_beta()  # outside the capture: a captured fill_ would freeze beta at today's value
         torch.cuda.synchronize(self.device)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            batch = mem.sample_into(ws, shift_pad=self.augment_shift)
+            batch = mem.sample_into(ws, shift_pad=self.augment_shift, intensity=self.augment_intensity,
+                                    copies=self.augment_copies)
             loss = self._update_from_batch(batch, after_loss=lambda l: mem.update_priorities(batch[0], l, gate=ws.status),
                                            gate=ws.status)
         return graph, ws, loss
@@ -590,6 +644,11 @@ class Agent:
         if self.augment_shift and not isinstance(mem, ReplayMemory):
             raise _lib.RainbowB200Error("args.augment_shift needs a rainbow_b200 ReplayMemory: the shifts are drawn and "
                                         "applied on the device by its gather")
+        if (self.augment_intensity or self.augment_copies != (1, 1)) and not isinstance(mem, ReplayMemory):
+            raise _lib.RainbowB200Error("args.augment_intensity / augment_m / augment_k need a rainbow_b200 ReplayMemory: "
+                                        "the augmented copies are drawn and written on the device by its gather")
+        if self.augment_copies != (1, 1) and not self._fused_path(self.batch_size):
+            raise self._copies_error(self.augment_copies)   # before sampling: a refused learn() leaves the replay as it was
         # the captured graph bakes in: this memory's buffers, the batch size and training-mode (noisy) weights
         graphable = (self.use_cuda_graph and isinstance(mem, ReplayMemory) and mem.rng == "philox" and
                      self.online_net.training)

@@ -353,6 +353,10 @@ def _meta(agent, mem):
                  V_max=agent.Vmax)
     if agent.augment_shift:   # only when on: manifests of runs without augmentation stay as they were
         hyper["augment_shift"] = agent.augment_shift
+    if agent.augment_intensity:
+        hyper["augment_intensity"] = agent.augment_intensity
+    if agent.augment_copies != (1, 1):
+        hyper["augment_m"], hyper["augment_k"] = agent.augment_copies
     meta = dict(world_size=agent.sync.world_size, rank=agent.sync.rank, optimiser=sd["layout"],
                 structure=_structure(agent, mem), hyper_parameters=hyper, learner=learner, replay=None)
     if mem is not None:

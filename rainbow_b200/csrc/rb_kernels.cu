@@ -600,6 +600,123 @@ k_gather_shift(const uint8_t* __restrict__ frames, const int32_t* __restrict__ t
   }
 }
 
+// ================================================================================================
+// K2a gather_aug : k_gather_shift generalised to M copies of every state and K copies of every next state (DrQ's K / M),
+// each copy with its own shift offset and its own intensity multiplier (SPR's intensity augmentation):
+//   out = fl32(fl32(in / 255) * mult),  mult = fma(s, clamp(N(0, 1), -2, 2), 1)   (no multiply at all when s == 0)
+// ================================================================================================
+// Same grid, CTA-per-stored-frame mapping and row split as k_gather_shift: the reachable input rows are staged once, then
+// every copy of each appearance of the frame is written from shared memory (copy j of the state to rows [jB, (j+1)B) of
+// `states`, copy k of the next state to rows [kB, (k+1)B) of `next_states`).
+// Draws, counter word 3 = the stream; c = *rng_counter as rb_tree_sample left it, key = seed:
+//   copy j offsets     (c_lo, c_hi, b, SHIFT_STREAM + j): x, y -> the state's (oy, ox), z, w -> the next state's (copy 0's
+//                      are k_gather_shift's);
+//   copy j multiplier  (c_lo, c_hi, b, INTS_STREAM + j): box_muller(x, y).x -> the state's, box_muller(z, w).x -> the next
+//                      state's.
+// The streams in use: sampling 0x5A4D504C, noise 0x4E4F4953 + i (i < RB_MAX_NOISY_LAYERS), shift 0x53484654 + j and
+// intensity 0x494E5453 + j (j < RB_MAX_AUG_COPIES): the four ranges [0x494E5453, 0x494E545A], [0x4E4F4953, 0x4E4F495A],
+// [0x53484654, 0x5348465B] and {0x5A4D504C} are disjoint.
+constexpr uint32_t INTS_STREAM = 0x494E5453u;        // "INTS"
+
+__device__ __forceinline__ float4 aug4(const uint8_t* s_frame, int y, int x, int dy, int dx, bool scaled, float mult) {
+  float4 v = shifted4(s_frame, y, x, dy, dx);
+  if (scaled) v = make_float4(__fmul_rn(v.x, mult), __fmul_rn(v.y, mult), __fmul_rn(v.z, mult), __fmul_rn(v.w, mult));
+  return v;
+}
+
+__device__ __forceinline__ float intensity_mult(float s, float normal) {
+  return __fmaf_rn(s, fminf(fmaxf(normal, -2.0f), 2.0f), 1.0f);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_aug(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+             const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+             const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+             float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+             float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, float intensity, int m_copies,
+             int k_copies, uint64_t seed, const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts,
+             float* __restrict__ scales) {
+  __shared__ uint64_t s_first;
+  __shared__ int s_off[2][RB_MAX_AUG_COPIES][2];   // (side, copy, (dy, dx)) = offset - pad
+  __shared__ float s_mult[2][RB_MAX_AUG_COPIES];
+  __shared__ __align__(16) uint8_t s_frame[RB_FRAME_BYTES];
+  const int b = blockIdx.y;
+  const int W = history + n;
+  const int copies = max(m_copies, k_copies);
+  const int used = blockIdx.x / split, part = blockIdx.x % split;
+  const int s = (n >= history && used >= history) ? n + (used - history) : used;
+  const int64_t idx = data_idx[b];
+  const int64_t pos = pymod(idx - (history - 1) + s, size);
+  const int rows = (FRAME_SIDE + split - 1) / split;
+  const int r0 = part * rows, r1 = min(FRAME_SIDE, r0 + rows);
+  const int v0 = max(r0 - pad, 0) * FRAME_SIDE / 16;
+  const int v1 = min(FRAME_VEC, (min(r1 + pad, FRAME_SIDE) * FRAME_SIDE + 15) / 16);
+  const uint4* src = reinterpret_cast<const uint4*>(frames + (size_t)pos * RB_FRAME_BYTES);
+  uint4 pre = make_uint4(0, 0, 0, 0);
+  if (v0 + (int)threadIdx.x < v1) pre = __ldg(src + v0 + threadIdx.x);
+  if (threadIdx.x < 32) {
+    uint64_t f = window_first_bits(timestep, size, idx, history, W);
+    if (threadIdx.x == 0) s_first = f;
+  }
+  const bool scaled = intensity > 0.0f;
+  if (threadIdx.x >= 32 && threadIdx.x < 32 + copies) {   // one thread per copy draws its offsets and multipliers
+    const int j = threadIdx.x - 32;
+    const unsigned long long c = *rng_counter;
+    const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+    int oy_s = 0, ox_s = 0, oy_n = 0, ox_n = 0;
+    if (pad > 0) {
+      const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)b, SHIFT_STREAM + (uint32_t)j), key);
+      oy_s = shift_offset(r.x, pad); ox_s = shift_offset(r.y, pad);
+      oy_n = shift_offset(r.z, pad); ox_n = shift_offset(r.w, pad);
+    }
+    float m_s = 1.0f, m_n = 1.0f;
+    if (scaled) {
+      const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)b, INTS_STREAM + (uint32_t)j), key);
+      m_s = intensity_mult(intensity, box_muller(r.x, r.y).x);
+      m_n = intensity_mult(intensity, box_muller(r.z, r.w).x);
+    }
+    s_off[0][j][0] = oy_s - pad; s_off[0][j][1] = ox_s - pad;
+    s_off[1][j][0] = oy_n - pad; s_off[1][j][1] = ox_n - pad;
+    s_mult[0][j] = m_s; s_mult[1][j] = m_n;
+    if (blockIdx.x == 0) {   // int32 [2][copies][B][2] and float32 [2][copies][B]: (side, copy, sample)
+      int32_t* sh_s = shifts + 2 * ((size_t)j * B + b);
+      int32_t* sh_n = shifts + 2 * ((size_t)(copies + j) * B + b);
+      sh_s[0] = oy_s; sh_s[1] = ox_s;
+      sh_n[0] = oy_n; sh_n[1] = ox_n;
+      scales[(size_t)j * B + b] = m_s;
+      scales[(size_t)(copies + j) * B + b] = m_n;
+    }
+  }
+  __syncthreads();
+  const uint64_t first = s_first;
+  const bool blank = slot_blank(first, s, history);
+  if (!blank) {
+    uint4* dst = reinterpret_cast<uint4*>(s_frame);
+    for (int v = v0 + threadIdx.x; v < v1; v += GATHER_THREADS) dst[v] = (v == v0 + (int)threadIdx.x) ? pre : __ldg(src + v);
+  }
+  __syncthreads();
+
+  const bool app_s = s < history, app_n = s >= n && s < n + history;
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int j = 0; j < copies; ++j) {
+    float4* dst_s = (app_s && j < m_copies)
+                        ? reinterpret_cast<float4*>(states + (((size_t)j * B + b) * history + s) * RB_FRAME_BYTES)
+                        : nullptr;
+    float4* dst_n = (app_n && j < k_copies)
+                        ? reinterpret_cast<float4*>(next_states + (((size_t)j * B + b) * history + (s - n)) * RB_FRAME_BYTES)
+                        : nullptr;
+    const int dy_s = s_off[0][j][0], dx_s = s_off[0][j][1], dy_n = s_off[1][j][0], dx_n = s_off[1][j][1];
+    const float m_s = s_mult[0][j], m_n = s_mult[1][j];
+    for (int i = r0 * ROW_VEC + threadIdx.x; i < r1 * ROW_VEC; i += GATHER_THREADS) {
+      const int y = i / ROW_VEC, x = (i - y * ROW_VEC) * 4;
+      if (dst_s) __stcs(dst_s + i, blank ? zero : aug4(s_frame, y, x, dy_s, dx_s, scaled, m_s));
+      if (dst_n) __stcs(dst_n + i, blank ? zero : aug4(s_frame, y, x, dy_n, dx_n, scaled, m_n));
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0)
+    gather_scalars(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns, nonterminals);
+}
+
 // memory.py:166-178 validation iterator, batched: grid = (history, count)
 __global__ void __launch_bounds__(GATHER_THREADS)
 k_iter_states(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, int64_t size, int64_t first_idx,
@@ -1086,6 +1203,188 @@ k_c51_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, co
       } else {
         const int a = (idx - Z) / Z, c = (idx - Z) - a * Z;
         dzi[idx] = s_g[c] * ((a == act ? 1.0f : 0.0f) - inv_a);
+      }
+    }
+  }
+}
+
+// The loss half of c51_core against a given target distribution m (m[r] = atom lane + 32 r, 0 past Z): log p and p of the
+// online logit row q_on_s_act, loss = -sum m log p and the gradient row g = wi (p sum(m) - m), with c51_core's arithmetic.
+template <int C51_R>
+__device__ __forceinline__ float c51_loss_row(int lane, int Z, const float* q_on_s_act, const float (&m)[C51_R], float wi,
+                                              float (&g)[C51_R]) {
+  float e[C51_R], x[C51_R], mx, sum, p_on[C51_R], logp[C51_R];
+  softmax_row(q_on_s_act, Z, lane, e, x, mx, sum);
+  {
+    const float lsum = logf(sum);
+#pragma unroll
+    for (int r = 0; r < C51_R; ++r) {
+      p_on[r] = __fdiv_rn(e[r], sum);
+      logp[r] = (lane + 32 * r < Z) ? __fsub_rn(__fsub_rn(x[r], mx), lsum) : 0.0f;
+    }
+  }
+  float ce = 0.0f, msum = 0.0f;
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) {
+    ce = __fadd_rn(ce, __fmul_rn(m[r], logp[r]));
+    msum = __fadd_rn(msum, m[r]);
+  }
+  ce = warp_sum(ce);
+  msum = warp_sum(msum);
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) g[r] = __fmul_rn(wi, __fsub_rn(__fmul_rn(p_on[r], msum), m[r]));
+  return -ce;
+}
+
+// DrQ's K / M averaging (Kostrikov et al. 2020, Algorithm 1) on the fused heads' outputs: z_on has (M + K) B rows (copy j of
+// s at row jB + i, copy k of s' at row (M + k) B + i), z_tg K B rows (copy k of s' at row kB + i).  ONE CTA PER SAMPLE, as
+// k_c51_dueling, with the sample's M + 2K z rows staged in shared memory:
+//   phase 1  the expected value of every (target copy k, action a) of online(s'_k), one warp per pair;
+//   phase 2  warp k: a*_k (first maximum wins) and the projection m_k of target(s'_k) at a*_k -- c51_core itself, its
+//            loss and gradient unused;
+//   phase 3  m = (sum_k m_k in k order) / K, rounded once (m_0 exactly at K = 1);
+//   phase 4  warp j: loss_j and the gradient row of online(s_j) at the taken action against m (c51_loss_row), with
+//            wi = w / (M B);
+//   phase 5  loss = (sum_j loss_j in j order) / M; dz rows jB + i get phase 3 of k_c51_dueling.
+// At M = K = 1 every output is k_c51_dueling's, bitwise.
+template <int C51_R>
+__global__ void __launch_bounds__(C51D_T)
+k_c51_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
+                  const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                  const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax, float delta_z,
+                  float gamma_n, int B, int A, int Z, int M, int K, float* __restrict__ loss, float* __restrict__ dz,
+                  float* __restrict__ m_out, int64_t* __restrict__ astar_out) {
+  extern __shared__ __align__(16) float s_dyn[];
+  __shared__ C51Scratch s_sc[C51D_T / 32];
+  __shared__ float s_junk[C51D_T / 32];
+  constexpr int WARPS = C51D_T / 32;
+  const int N2 = Z + A * Z;
+  const int rows = M + 2 * K;
+  float* zs = s_dyn;               // [M + 2K][N2]: online(s_j), online(s'_k), target(s'_k)
+  float* q_t = zs + rows * N2;     // [K][Z] target logits of a*_k
+  float* q_s = q_t + K * Z;        // [M][Z] online logits of the taken action
+  float* s_g = q_s + M * Z;        // [M][Z] gradient rows
+  float* s_m = s_g + M * Z;        // [K][Z] projections m_k
+  float* s_mavg = s_m + K * Z;     // [Z] averaged target
+  float* s_ev = s_mavg + Z;        // [K][A] expected values
+  float* s_loss = s_ev + K * A;    // [M] loss_j
+  const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const float* on_s = zs;
+  const float* on_ns = zs + (size_t)M * N2;
+  const float* tg_ns = zs + (size_t)(M + K) * N2;
+  {
+    const int total = rows * N2;
+    for (int base = tid; base < total; base += C51D_T * 8) {
+      float v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {  // eight independent loads in flight per thread, then the stores
+        const int idx = base + u * C51D_T;
+        v[u] = 0.0f;
+        if (idx < total) {
+          const int t = idx / N2;    // staged row t: online rows 0 .. M + K - 1, then the target rows
+          const float* src = (t < M + K) ? z_on + ((size_t)t * B + i) * N2 : z_tg + ((size_t)(t - M - K) * B + i) * N2;
+          v[u] = __ldg(src + (idx - t * N2));
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int idx = base + u * C51D_T;
+        if (idx < total) zs[idx] = v[u];
+      }
+    }
+  }
+  __syncthreads();
+  const int act = (int)actions[i];
+  float sup[C51_R];
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  for (int t = warp; t < K * A; t += WARPS) {  // phase 1
+    const int k = t / A, a = t - k * A;
+    const float* r1 = on_ns + (size_t)k * N2;
+    float x[C51_R];
+#pragma unroll
+    for (int r = 0; r < C51_R; ++r) {
+      const int c = lane + 32 * r;
+      float acc = 0.0f;
+      if (c < Z)
+        for (int aa = 0; aa < A; ++aa) acc += r1[Z + aa * Z + c];
+      const float mean = acc / (float)A;
+      x[r] = (c < Z) ? r1[c] + r1[Z + a * Z + c] - mean : -CUDART_INF_F;
+    }
+    const float ev = c51_expected_value<C51_R>(x, sup, Z, lane);
+    if (lane == 0) s_ev[t] = ev;
+  }
+  __syncthreads();
+  const float ret = __ldg(returns + i), nt = __ldg(nonterminals + i), w = __ldg(weights + i);
+  for (int k = warp; k < K; k += WARPS) {  // phase 2
+    int best = 0;
+    float best_ev = -CUDART_INF_F;
+    for (int a = 0; a < A; ++a) {
+      const float ev = s_ev[k * A + a];
+      if (ev > best_ev) {  // first maximum wins, like torch.argmax
+        best_ev = ev;
+        best = a;
+      }
+    }
+    const float* r = tg_ns + (size_t)k * N2;
+    float* qt = q_t + k * Z;
+    for (int c = lane; c < Z; c += 32) {
+      float mean = 0.0f;
+      for (int a = 0; a < A; ++a) mean += r[Z + a * Z + c];
+      mean = mean / (float)A;
+      qt[c] = r[c] + r[Z + best * Z + c] - mean;
+    }
+    __syncwarp();
+    // c51_core with sample index 0 on per-copy outputs: m_k into s_m[k], a*_k into astar_out[k][i]; its loss row
+    // (fed qt again) and gradient are not used
+    float g[C51_R];
+    c51_core<C51_R>(s_sc[warp], lane, 0, B, A, Z, nullptr, qt, qt, ret, nt, w, support, vmin, vmax, delta_z, gamma_n,
+                    s_junk + warp, s_m + k * Z, astar_out ? astar_out + (size_t)k * B + i : nullptr, g, best);
+  }
+  __syncthreads();
+  for (int c = tid; c < Z; c += C51D_T) {  // phase 3
+    float acc = s_m[c];
+    for (int k = 1; k < K; ++k) acc = __fadd_rn(acc, s_m[k * Z + c]);
+    acc = __fdiv_rn(acc, (float)K);
+    s_mavg[c] = acc;
+    if (m_out) m_out[(size_t)i * Z + c] = acc;
+  }
+  __syncthreads();
+  const float wi = __fdiv_rn(w, (float)(M * B));
+  for (int j = warp; j < M; j += WARPS) {  // phase 4
+    const float* r = on_s + (size_t)j * N2;
+    float* qs = q_s + j * Z;
+    for (int c = lane; c < Z; c += 32) {
+      float mean = 0.0f;
+      for (int a = 0; a < A; ++a) mean += r[Z + a * Z + c];
+      qs[c] = r[c] + r[Z + act * Z + c] - mean / (float)A;
+    }
+    __syncwarp();
+    float m[C51_R], g[C51_R];
+#pragma unroll
+    for (int rr = 0; rr < C51_R; ++rr) m[rr] = (lane + 32 * rr < Z) ? s_mavg[lane + 32 * rr] : 0.0f;
+    const float lj = c51_loss_row<C51_R>(lane, Z, qs, m, wi, g);
+    if (lane == 0) s_loss[j] = lj;
+#pragma unroll
+    for (int rr = 0; rr < C51_R; ++rr)
+      if (lane + 32 * rr < Z) s_g[j * Z + lane + 32 * rr] = g[rr];
+  }
+  __syncthreads();
+  if (tid == 0) {  // phase 5
+    float acc = s_loss[0];
+    for (int j = 1; j < M; ++j) acc = __fadd_rn(acc, s_loss[j]);
+    loss[i] = __fdiv_rn(acc, (float)M);
+  }
+  const float inv_a = 1.0f / (float)A;
+  for (int j = 0; j < M; ++j) {
+    float* dzi = dz + ((size_t)j * B + i) * N2;
+    const float* gj = s_g + j * Z;
+    for (int idx = tid; idx < N2; idx += C51D_T) {
+      if (idx < Z) {
+        dzi[idx] = gj[idx];
+      } else {
+        const int a = (idx - Z) / Z, c = (idx - Z) - a * Z;
+        dzi[idx] = gj[c] * ((a == act ? 1.0f : 0.0f) - inv_a);
       }
     }
   }
@@ -1714,6 +2013,32 @@ int rb_gather_shift(const uint8_t* frames, const int32_t* timestep, const int32_
   return check_launch("rb_gather_shift");
 }
 
+int rb_gather_aug(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                  const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n,
+                  const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
+                  float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
+                  const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream) {
+  const int rc = gather_check("rb_gather_aug", frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n,
+                              gamma_pow, states, next_states, actions, returns, nonterminals);
+  if (rc != RB_OK) return rc;
+  if (!rng_counter || !shifts || !scales) return fail(RB_ERR_INVAL, "rb_gather_aug: null pointer");
+  if (pad < 0 || pad > RB_MAX_SHIFT_PAD) return fail(RB_ERR_RANGE, "rb_gather_aug: pad outside [0, RB_MAX_SHIFT_PAD]");
+  if (!(intensity >= 0.0f && intensity <= 0.5f)) return fail(RB_ERR_RANGE, "rb_gather_aug: intensity outside [0, 0.5]");
+  if (m_copies < 1 || m_copies > RB_MAX_AUG_COPIES || k_copies < 1 || k_copies > RB_MAX_AUG_COPIES)
+    return fail(RB_ERR_RANGE, "rb_gather_aug: copies outside [1, RB_MAX_AUG_COPIES]");
+  if (pad == 0 && intensity == 0.0f && m_copies == 1 && k_copies == 1)
+    return fail(RB_ERR_INVAL, "rb_gather_aug: no augmentation requested (that is rb_gather)");
+  const int used = (history + n < 2 * history) ? history + n : 2 * history;
+  const int split = gather_split(used * B);
+  dim3 grid(used * split, B);
+  { ProfScope prof_(RB_K_GATHER_AUG, (cudaStream_t)stream);
+    k_gather_aug<<<grid, GATHER_THREADS, 0, (cudaStream_t)stream>>>(
+      frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states, next_states, actions,
+      returns, nonterminals, split, pad, intensity, m_copies, k_copies, seed, (const unsigned long long*)rng_counter, shifts,
+      scales); }
+  return check_launch("rb_gather_aug");
+}
+
 int rb_iter_states(const uint8_t* frames, const int32_t* timestep, int64_t size, int64_t first, int count, int history,
                    float* out, rb_stream_t stream) {
   if (!frames || !timestep || !out) return fail(RB_ERR_INVAL, "rb_iter_states: null pointer");
@@ -1876,6 +2201,35 @@ int rb_c51_dueling_loss_grad(const float* z_online, const float* z_target, int a
                                                                   support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss, dz, m_out,
                                                                   astar_out); }
   return check_launch("rb_c51_dueling_loss_grad");
+}
+
+int rb_c51_dueling_avg_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                 const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                                 const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int M,
+                                 int K, float* loss, float* dz, float* m_out, int64_t* astar_out, rb_stream_t stream) {
+  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !support || !loss || !dz)
+    return fail(RB_ERR_INVAL, "rb_c51_dueling_avg_loss_grad: null pointer");
+  const int Z = atoms, A = actions_n;
+  if (B <= 0 || A <= 0 || Z <= 1)
+    return fail(RB_ERR_INVAL, "rb_c51_dueling_avg_loss_grad: B, actions > 0 and atoms > 1 are required");
+  if (Z > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_c51_dueling_avg_loss_grad: atoms exceeds RB_MAX_ATOMS");
+  if (M < 1 || M > RB_MAX_AUG_COPIES || K < 1 || K > RB_MAX_AUG_COPIES)
+    return fail(RB_ERR_RANGE, "rb_c51_dueling_avg_loss_grad: copies outside [1, RB_MAX_AUG_COPIES]");
+  const size_t smem = (size_t)((M + 2 * K) * (Z + A * Z) + (2 * M + 2 * K + 1) * Z + K * A + M) * sizeof(float);
+  if (smem > 200 * 1024) return fail(RB_ERR_RANGE, "rb_c51_dueling_avg_loss_grad: (M + 2K) * actions * atoms too large");
+  int rc_s = rbi::ensure_dynamic_smem(k_c51_dueling_avg<2>, smem, "rb_c51_dueling_avg_loss_grad");
+  if (rc_s == RB_OK) rc_s = rbi::ensure_dynamic_smem(k_c51_dueling_avg<4>, smem, "rb_c51_dueling_avg_loss_grad");
+  if (rc_s != RB_OK) return rc_s;
+  { ProfScope prof_(RB_K_C51_DUELING_AVG, (cudaStream_t)stream);
+    if (Z <= 64)
+      k_c51_dueling_avg<2><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                      weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z,
+                                                                      M, K, loss, dz, m_out, astar_out);
+    else
+      k_c51_dueling_avg<4><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                      weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z,
+                                                                      M, K, loss, dz, m_out, astar_out); }
+  return check_launch("rb_c51_dueling_avg_loss_grad");
 }
 
 int rb_q_values(const float* z, int M, int actions, int atoms, const float* support, float* q, int64_t* best_action,

@@ -9,7 +9,8 @@ called through the C ABI in include/rainbow_b200.h:
     sample             -> rb_tree_sample   (K1)   memory.py:124-132, 148-154
                           rb_gather        (K2)   memory.py:111-121, 134-146
                           (rb_gather_shift with shift_pad > 0: the same plus random-shift augmentation, no reference
-                          counterpart)
+                          counterpart; rb_gather_aug with intensity > 0 or copies != (1, 1): shift and intensity
+                          augmentation of M copies of s and K of s')
     update_priorities  -> rb_tree_update   (K4)   memory.py:157-159, 23-48
     __next__           -> rb_iter_states          memory.py:166-178
 
@@ -210,21 +211,24 @@ class SegmentTree:
 class _SampleWorkspace:
     """Output buffers of one sample() call for a given batch size."""
 
-    def __init__(self, B, history, device):
+    def __init__(self, B, history, device, copies=(1, 1)):
         f32, i64 = torch.float32, torch.int64
         self.B = B
+        self.copies = M, K = (int(copies[0]), int(copies[1]))
         self.probs = torch.empty(B, dtype=f32, device=device)
         self.data_idx = torch.empty(B, dtype=i64, device=device)
         self.tree_idx = torch.empty(B, dtype=i64, device=device)
         self.weights = torch.empty(B, dtype=f32, device=device)
-        # one allocation, s rows then s' rows: the learner can push [s; s'] through the online conv body in a single pass
-        self.both_states = torch.empty((2 * B, history, 84, 84), dtype=f32, device=device)
-        self.states, self.next_states = self.both_states[:B], self.both_states[B:]
+        # one allocation, s rows then s' rows: the learner can push [s; s'] through the online conv body in a single pass.
+        # With copies = (M, K) (rb_gather_aug) it holds M copies of s, then K copies of s', copy-major: [(M + K) B] rows.
+        self.both_states = torch.empty(((M + K) * B, history, 84, 84), dtype=f32, device=device)
+        self.states, self.next_states = self.both_states[:M * B], self.both_states[M * B:]
         self.actions = torch.empty(B, dtype=i64, device=device)
         self.returns = torch.empty(B, dtype=f32, device=device)
         self.nonterminals = torch.empty((B, 1), dtype=f32, device=device)
         self.status = torch.zeros(4, dtype=torch.int32, device=device)   # ok flag, draws used, rejected batches so far, -
-        self.shifts = None   # int32 [2][B][2] offsets of the last augmented gather (allocated by the first one)
+        self.shifts = None   # int32 [2][B][2] offsets of the last shifted gather, [2][max(M, K)][B][2] after rb_gather_aug
+        self.scales = None   # float32 [2][max(M, K)][B] intensity multipliers of the last rb_gather_aug
 
     def as_tuple(self):
         return (self.tree_idx, self.states, self.actions, self.returns, self.next_states, self.nonterminals,
@@ -240,6 +244,8 @@ class ReplayMemory:
 
     APPEND_BATCH = 8  # RB_APPEND_BATCH
     MAX_SHIFT_PAD = 16  # RB_MAX_SHIFT_PAD
+    MAX_AUG_COPIES = 8  # RB_MAX_AUG_COPIES
+    MAX_INTENSITY = 0.5
 
     def __init__(self, args, capacity, rng="philox", seed=None, max_attempts=64, strict=False, defer_appends=False):
         self.device = _require_cuda(args.device)
@@ -383,38 +389,67 @@ class ReplayMemory:
                              "has no augmentation, so there is no numpy stream to reproduce)")
         return shift_pad
 
-    def _launch_gather(self, ws, shift_pad=0):
+    def _check_augmentation(self, shift_pad, intensity, copies):
+        """Validated (shift_pad, intensity, (M, K)); ValueError outside the ranges rb_gather_aug takes."""
+        shift_pad, intensity = self._check_shift_pad(shift_pad), float(intensity)
+        M, K = (int(c) for c in copies)
+        if not 0.0 <= intensity <= self.MAX_INTENSITY:   # also refuses NaN
+            raise ValueError(f"intensity must be in [0, {self.MAX_INTENSITY}], got {intensity}")
+        if not (1 <= M <= self.MAX_AUG_COPIES and 1 <= K <= self.MAX_AUG_COPIES):
+            raise ValueError(f"copies (M, K) must each be in [1, {self.MAX_AUG_COPIES}], got {tuple(copies)}")
+        if (intensity or (M, K) != (1, 1)) and self.rng == "numpy":
+            raise ValueError("intensity > 0 or copies != (1, 1) needs rng='philox': the draws come from the device stream "
+                             "(the reference has no augmentation, so there is no numpy stream to reproduce)")
+        return shift_pad, intensity, (M, K)
+
+    def _launch_gather(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1)):
         tr = self.transitions
         common = (_lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action), _lib.ptr(tr.reward),
                   _lib.ptr(tr.nonterminal), tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, self.n,
                   _lib.ptr(self.n_step_scaling), _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions),
                   _lib.ptr(ws.returns), _lib.ptr(ws.nonterminals))
-        if not shift_pad:
+        if not shift_pad and not intensity and copies == (1, 1):
             _lib.check(self._lib.rb_gather(*common, _lib.stream()))
             return
-        if ws.shifts is None:
-            ws.shifts = torch.empty((2, ws.B, 2), dtype=torch.int32, device=self.device)
-        _lib.check(self._lib.rb_gather_shift(*common, shift_pad, self.seed, _lib.ptr(self._rng_counter), _lib.ptr(ws.shifts),
-                                             _lib.stream()))
+        if not intensity and copies == (1, 1):
+            if ws.shifts is None or ws.shifts.shape != (2, ws.B, 2):
+                ws.shifts = torch.empty((2, ws.B, 2), dtype=torch.int32, device=self.device)
+            _lib.check(self._lib.rb_gather_shift(*common, shift_pad, self.seed, _lib.ptr(self._rng_counter),
+                                                 _lib.ptr(ws.shifts), _lib.stream()))
+            return
+        c = max(copies)
+        if ws.shifts is None or ws.shifts.shape != (2, c, ws.B, 2):
+            ws.shifts = torch.empty((2, c, ws.B, 2), dtype=torch.int32, device=self.device)
+        if ws.scales is None or ws.scales.shape != (2, c, ws.B):
+            ws.scales = torch.empty((2, c, ws.B), dtype=torch.float32, device=self.device)
+        _lib.check(self._lib.rb_gather_aug(*common, shift_pad, intensity, copies[0], copies[1], self.seed,
+                                           _lib.ptr(self._rng_counter), _lib.ptr(ws.shifts), _lib.ptr(ws.scales),
+                                           _lib.stream()))
 
-    def sample_into(self, ws, shift_pad=0):
+    def sample_into(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1)):
         """Device-RNG sample into caller-owned buffers: two launches, no synchronisation (graph capturable).
         The caller is responsible for push_beta() and flush_appends() (outside any graph capture).
         shift_pad = p > 0 (at most MAX_SHIFT_PAD) augments the states and next states by random shifts (DrQ): each
         observation edge-padded by p pixels and cropped back to 84 x 84 at its own offset drawn on the device
-        (rb_gather_shift); `ws.shifts` receives the offsets.  0 gathers exactly as the reference does."""
-        shift_pad = self._check_shift_pad(shift_pad)
+        (rb_gather_shift); `ws.shifts` receives the offsets.  0 gathers exactly as the reference does.
+        intensity = s > 0 (at most MAX_INTENSITY) multiplies every observation by 1 + s * clip(N(0, 1), -2, 2) (SPR), and
+        copies = (M, K) writes M augmented copies of every state and K of every next state (DrQ's K / M): both go through
+        rb_gather_aug, whose draws land in `ws.shifts` and `ws.scales`.  `ws` must have been made for these copies."""
+        shift_pad, intensity, copies = self._check_augmentation(shift_pad, intensity, copies)
+        if ws.copies != copies:
+            raise ValueError(f"the workspace holds copies {ws.copies}, the call asks for {copies}")
         self._launch_sample(ws)
-        self._launch_gather(ws, shift_pad)
+        self._launch_gather(ws, shift_pad, intensity, copies)
         self._last = ws
         return ws.as_tuple()
 
-    def sample(self, batch_size, shift_pad=0):
+    def sample(self, batch_size, shift_pad=0, intensity=0.0, copies=(1, 1)):
         """memory.py:148-155.  Returns (tree_idxs, states, actions, returns, next_states, nonterminals, weights),
         all device tensors (the reference returns tree_idxs as numpy; update_priorities takes either).
-        shift_pad: random-shift augmentation as in sample_into(); needs rng="philox" (ValueError otherwise)."""
-        shift_pad = self._check_shift_pad(shift_pad)
-        ws = _SampleWorkspace(int(batch_size), self.history, self.device)
+        shift_pad, intensity, copies: augmentation as in sample_into(); needs rng="philox" (ValueError otherwise).  With
+        copies = (M, K) the states are [M B, ...] and the next states [K B, ...], copy-major."""
+        shift_pad, intensity, copies = self._check_augmentation(shift_pad, intensity, copies)
+        ws = _SampleWorkspace(int(batch_size), self.history, self.device, copies)
         self.flush_appends()
         self.push_beta()
         if self.rng == "numpy":
@@ -429,7 +464,7 @@ class ReplayMemory:
             self._launch_gather(ws)
             self._last = ws
             return ws.as_tuple()
-        out = self.sample_into(ws, shift_pad)
+        out = self.sample_into(ws, shift_pad, intensity, copies)
         if self.strict:
             self.check_last_sample()
         return out
