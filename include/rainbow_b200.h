@@ -60,6 +60,7 @@ extern "C" {
 #define RB_APPEND_BATCH 8        /* transitions per rb_append_batch launch */
 #define RB_MAX_SHIFT_PAD 16      /* largest pad of rb_gather_shift */
 #define RB_MAX_AUG_COPIES 8      /* most copies of a state (M) or next state (K) in rb_gather_aug */
+#define RB_MAX_RESET_SEGMENTS 32 /* most parameter tensors one rb_param_reset call covers */
 
 /* status words written by rb_tree_sample (int32[4]): status[0] = 1 if the batch now in the output buffers passed the
  * whole-batch validity test (memory.py:131), 0 otherwise; status[1] = draws used; status[2] = number of device-RNG
@@ -76,7 +77,7 @@ enum {
   RB_K_NOISY_RESAMPLE, RB_K_NOISY_COMPOSE, RB_K_SQNORM, RB_K_CLIP_ADAM, RB_K_HEAD_FC1, RB_K_HEAD_FC2, RB_K_HEAD_LOGITS,
   RB_K_HEAD_WGRAD2, RB_K_HEAD_DH, RB_K_HEAD_BWD1, RB_K_NOISE_FACTORS, RB_K_C51_DUELING, RB_K_BIAS_GRAD, RB_K_Q_VALUES,
   RB_K_HEAD_REDUCE1, RB_K_CONV_WGRAD, RB_K_HEAD_BWD1_WGRAD, RB_K_HEAD_BWD1_DX, RB_K_LEARN_STATS, RB_K_GATHER_SHIFT,
-  RB_K_GATHER_AUG, RB_K_C51_DUELING_AVG, RB_KERNEL_COUNT
+  RB_K_GATHER_AUG, RB_K_C51_DUELING_AVG, RB_K_TARGET_EMA, RB_K_PARAM_RESET, RB_KERNEL_COUNT
 };
 
 int rb_abi_version(void);
@@ -351,6 +352,33 @@ int rb_clip_adam_scratch_elems(void);
 int rb_clip_adam(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t P, float grad_scale,
                  float max_norm, float lr, float beta1, float beta2, float eps, int64_t* step_count,
                  double* partial_sums, float* norm_out, const int32_t* gate, rb_stream_t stream);
+
+/* Polyak (soft) target update over FLAT float32 buffers of n elements (no reference counterpart; the reference only copies
+ * the online net into the target, agent.py:102-103).  For every i < n:
+ *   target[i] = fmaf(tau, param[i], fl32(1 - tau) * target[i])
+ * with 1 - tau formed in fp32 and the product rounded on its own (no contraction).  tau = 1 copies param for finite target.
+ * gate (optional device int32, may be NULL): when *gate == 0 nothing is written (rejected sample batch, as rb_clip_adam).
+ * RB_ERR_INVAL: a NULL target or param, n < 0, or overlapping buffers; RB_ERR_RANGE: tau outside (0, 1] or NaN.  A refused
+ * call launches nothing; n == 0 launches nothing and returns RB_OK. */
+int rb_target_ema(float* target, const float* param, int64_t n, float tau, const int32_t* gate, rb_stream_t stream);
+
+/* Shrink-and-perturb reset (Ash & Adams 2020; the later-layer resets of Nikishin et al. 2022) of a FLAT float32 parameter
+ * buffer of n elements, over a table of segments (one per parameter tensor).  For every element j of segment s:
+ *   theta0 = fmaf(bound_s, r, constant_s),  r = 2u - 1,  u = (w >> 8) * 2^-24
+ *   param[j] = fmaf(alpha_s, param[j], fl32(1 - alpha_s) * theta0)
+ * where w is word (j & 3) of Philox4x32-10 with key `seed` and counter (k_lo, k_hi, j >> 2, 0x52534554), k = reset_index.
+ * A uniform initialisation U[-b, b) is {bound b, constant 0}, a constant c is {bound 0, constant c}.  alpha = 1 leaves a
+ * segment bitwise unchanged, alpha = 0 re-draws it.  Elements outside every segment are never written.
+ * segs: HOST array of n_segs entries, sorted by offset and non-overlapping, copied into the launch.
+ * RB_ERR_INVAL: a NULL param or segs; RB_ERR_RANGE: n_segs outside [1, RB_MAX_RESET_SEGMENTS], a segment outside [0, n),
+ * unsorted or overlapping, count <= 0, a negative or non-finite bound or constant, alpha outside [0, 1] or NaN.  A refused
+ * call launches nothing. */
+typedef struct rb_reset_segment {
+  int64_t offset, count;
+  float bound, constant, alpha;
+} rb_reset_segment;
+int rb_param_reset(float* param, int64_t n, const rb_reset_segment* segs, int n_segs, uint64_t seed, uint64_t reset_index,
+                   rb_stream_t stream);
 
 /* Multi-GPU replacement of "all-reduce the flat gradient, then rb_clip_adam on every rank" (agent.py:97-98 under data
  * parallelism; no reference counterpart): reduce-scatter by peer loads + clip + Adam on the owned 1/world parts (moments

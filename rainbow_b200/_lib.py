@@ -24,6 +24,12 @@ class HeadGrads(C.Structure):
     _fields_ = [(n, _vp * 2) for n in ("w1_mu", "w1_sigma", "b1_mu", "b1_sigma", "w2_mu", "w2_sigma", "b2_mu", "b2_sigma")]
 
 
+class ResetSegment(C.Structure):
+    """rb_reset_segment: one parameter tensor of rb_param_reset's table."""
+    _fields_ = [("offset", C.c_int64), ("count", C.c_int64), ("bound", C.c_float), ("constant", C.c_float),
+                ("alpha", C.c_float)]
+
+
 _hp, _hg = C.POINTER(HeadParams), C.POINTER(HeadGrads)
 
 # name -> (restype, argtypes); must list every symbol declared in include/rainbow_b200.h
@@ -72,6 +78,8 @@ SIGNATURES = {
                                     _vp, _vp, _vp, _vp, _vp]),
     "rb_clip_adam_scratch_elems": (C.c_int, []),
     "rb_clip_adam": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
+    "rb_target_ema": (C.c_int, [_vp, _vp, _i64, _f32, _vp, _vp]),
+    "rb_param_reset": (C.c_int, [_vp, _i64, C.POINTER(ResetSegment), _i32, _u64, _u64, _vp]),
     "rb_q_values": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "rb_learn_stats_scratch_elems": (C.c_int, []),
     "rb_learn_stats_batch": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
@@ -134,14 +142,18 @@ def stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-KERNEL_IDS = ["tree_update", "tree_find", "tree_sample", "gather", "iter_states", "append", "c51", "noisy_resample",
-              "noisy_compose", "sqnorm", "clip_adam", "head_fc1", "head_fc2", "head_logits", "head_wgrad2", "head_dh",
-              "head_bwd1", "noise_factors", "c51_dueling", "bias_grad", "q_values", "head_reduce1", "conv_wgrad",
-              "head_bwd1_wgrad", "head_bwd1_dx", "learn_stats", "gather_shift"]  # order of the enum in include/rainbow_b200.h
-# KERNEL_IDS is kept as it was (its last entry is pinned by a host test); kernels added since are appended here, in enum
-# order, and PROFILE_IDS is the one list KernelTimer reads.  A later kernel goes at the end of AUG_KERNEL_IDS.
-AUG_KERNEL_IDS = ["gather_aug", "c51_dueling_avg"]  # the enum continues after RB_K_GATHER_SHIFT with these
-PROFILE_IDS = KERNEL_IDS + AUG_KERNEL_IDS           # every kernel id, indexed by its enum value
+# Every kernel id, indexed by its value in the RB_K_* enum of include/rainbow_b200.h (RB_K_FOO -> "foo"); a host test checks
+# this list against the enum, names, order and RB_KERNEL_COUNT.  A new kernel goes at the end of this one list.
+ALL_KERNEL_IDS = ["tree_update", "tree_find", "tree_sample", "gather", "iter_states", "append", "c51", "noisy_resample",
+                  "noisy_compose", "sqnorm", "clip_adam", "head_fc1", "head_fc2", "head_logits", "head_wgrad2", "head_dh",
+                  "head_bwd1", "noise_factors", "c51_dueling", "bias_grad", "q_values", "head_reduce1", "conv_wgrad",
+                  "head_bwd1_wgrad", "head_bwd1_dx", "learn_stats", "gather_shift", "gather_aug", "c51_dueling_avg",
+                  "target_ema", "param_reset"]
+# earlier names for prefixes of it, kept for their callers: the ids up to RB_K_GATHER_SHIFT, the two augmentation kernels
+# that follow, and both together
+KERNEL_IDS = ALL_KERNEL_IDS[:ALL_KERNEL_IDS.index("gather_shift") + 1]
+AUG_KERNEL_IDS = ALL_KERNEL_IDS[len(KERNEL_IDS):ALL_KERNEL_IDS.index("c51_dueling_avg") + 1]
+PROFILE_IDS = KERNEL_IDS + AUG_KERNEL_IDS
 
 
 class KernelTimer:
@@ -155,7 +167,7 @@ class KernelTimer:
         lib = load()
         check(lib.rb_profile_enable(0))
         self.result = {}
-        for i, name in enumerate(PROFILE_IDS):
+        for i, name in enumerate(ALL_KERNEL_IDS):
             ms, n = C.c_double(0.0), C.c_int(0)
             check(lib.rb_profile_collect(i, C.byref(ms), C.byref(n)))
             if n.value:

@@ -16,6 +16,7 @@ One `learn(mem)` (agent.py:61-100) is:
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
+    [args.target_tau = tau > 0: rb_target_ema -- Polyak target update t <- tau p + (1 - tau) t, gated like K7]
     K4 rb_tree_update                         (agent.py:100 -> memory.py:157-159)
     [args.learn_stats = R > 0: rb_learn_stats_batch on a side stream after K3, rb_learn_stats_write after K7 -- one record
      per update into a device ring, read with Agent.learn_stats()]
@@ -23,18 +24,23 @@ One `learn(mem)` (agent.py:61-100) is:
 Nothing in that chain synchronises with the host, so the whole update is captured into one CUDA graph
 (`cuda_graph=True`, the default) and replayed: the update is launch-latency bound otherwise
 (the reference issues ~600 ATen ops per update, SURVEY.md 2.1).
+
+[args.reset_interval = N > 0: after every N-th learn(), one rb_param_reset launch outside the graph -- shrink-and-perturb
+ of the online parameters toward a fresh initialisation drawn on the device (Agent.reset_parameters)]
 """
+import math
 import os
 import warnings
 import weakref
 
 import numpy as np
 import torch
+from torch import nn
 
 from . import _lib
 from .dist import GradSync
 from .memory import ReplayMemory, _SampleWorkspace
-from .model import DQN, FusedHead
+from .model import DQN, FusedHead, NoisyLinear
 
 
 def c51_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax,
@@ -80,6 +86,60 @@ def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, ret
         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
         float(gamma_n), B, M, K, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), _lib.stream()))
     return loss, dz
+
+
+ENCODER, HEAD = 0, 1   # the two groups of reset_table / Agent.reset_parameters
+
+
+def reset_table(net, offsets):
+    """The initialisation of every parameter of `net` (named_parameters order, at `offsets` in the flat buffer) as
+    rb_param_reset draws it: [(offset, count, bound, constant, group)], theta0 = bound * U[-1, 1) + constant.
+      conv weight and bias   U[-b, b), b = 1 / sqrt(fan_in), fan_in = c_in k k (torch's Conv2d.reset_parameters:
+                             kaiming_uniform_(a=sqrt(5)) has exactly this bound)                          group ENCODER
+      weight_mu, bias_mu     U[-b, b), b = 1 / sqrt(in_features)          (model.py:25-30)             group HEAD
+      weight_sigma           std_init / sqrt(in_features)
+      bias_sigma             std_init / sqrt(out_features)"""
+    out = []
+    for (name, p), off in zip(net.named_parameters(), offsets):
+        owner, kind = name.rsplit(".", 1)
+        m = net.get_submodule(owner)
+        if isinstance(m, nn.Conv2d):
+            fan_in = m.in_channels // m.groups * m.kernel_size[0] * m.kernel_size[1]
+            out.append((off, p.numel(), 1.0 / math.sqrt(fan_in), 0.0, ENCODER))
+        elif isinstance(m, NoisyLinear):
+            if kind in ("weight_mu", "bias_mu"):
+                out.append((off, p.numel(), 1.0 / math.sqrt(m.in_features), 0.0, HEAD))
+            elif kind == "weight_sigma":
+                out.append((off, p.numel(), 0.0, m.std_init / math.sqrt(m.in_features), HEAD))
+            elif kind == "bias_sigma":
+                out.append((off, p.numel(), 0.0, m.std_init / math.sqrt(m.out_features), HEAD))
+            else:
+                raise _lib.RainbowB200Error(f"no reset rule for parameter {name}")
+        else:
+            raise _lib.RainbowB200Error(f"no reset rule for parameter {name}")
+    return out
+
+
+def target_reset_options(args):
+    """(target_tau, reset_interval, (reset_shrink_encoder, reset_shrink_head)) from `args`, checked: tau in [0, 1] (0 = no
+    soft target update), interval >= 0 (0 = no resets), both shrink factors in [0, 1] (defaults 1.0 and 0.0)."""
+    tau = getattr(args, "target_tau", None)
+    tau = 0.0 if tau is None else float(tau)
+    # rb_target_ema takes tau as an fp32: a tau that rounds to 0 there (below ~7e-46) would only be refused at the first update
+    if not 0.0 <= tau <= 1.0 or (tau > 0.0 and not np.float32(tau) > 0.0):
+        raise ValueError(f"target_tau must be 0 or in (0, 1] as an fp32, got {tau}")
+    interval = getattr(args, "reset_interval", None)
+    interval = 0 if interval is None else interval
+    if isinstance(interval, bool) or int(interval) != interval or interval < 0:
+        raise ValueError(f"reset_interval must be an integer >= 0, got {interval}")
+    shrink = []
+    for key, default in (("reset_shrink_encoder", 1.0), ("reset_shrink_head", 0.0)):
+        v = getattr(args, key, None)
+        v = default if v is None else float(v)
+        if not 0.0 <= v <= 1.0:
+            raise ValueError(f"{key} must be in [0, 1], got {v}")
+        shrink.append(v)
+    return tau, int(interval), tuple(shrink)
 
 
 class FusedClipAdam:
@@ -205,6 +265,9 @@ class Agent:
         if not all(1 <= c <= ReplayMemory.MAX_AUG_COPIES for c in self.augment_copies):
             raise ValueError(f"augment_m and augment_k must be in [1, {ReplayMemory.MAX_AUG_COPIES}], got "
                              f"{self.augment_copies}")
+        # Polyak target updates (tau > 0: every applied optimiser step also moves the target, DrQ(eps) / SPR / BBF) and
+        # periodic shrink-and-perturb resets of the online net (SR-SPR, BBF); both off by default
+        self.target_tau, self.reset_interval, self.reset_shrink = target_reset_options(args)
 
         self.online_net = DQN(args, self.action_space).to(device=self.device)
         model_path = getattr(args, "model", None)
@@ -253,6 +316,22 @@ class Agent:
         self.sync.broadcast_(self.optimiser.flat_param)  # identical initial parameters on every rank
         if self.peer_optimizer:
             self.sync.exchange = False   # the optimiser step does the gradient exchange itself
+        # the target's parameters as views into one flat buffer laid out exactly like flat_param (element i of one is element
+        # i of the other, padding zero in both): a soft target update is one rb_target_ema over both buffers
+        self.target_flat = torch.zeros(self.optimiser.numel, dtype=torch.float32, device=self.device)
+        with torch.no_grad():
+            for p, o in zip(self.target_net.parameters(), self.optimiser.offsets):
+                n = p.numel()
+                self.target_flat[o:o + n].copy_(p.reshape(-1))
+                p.data = self.target_flat[o:o + n].view_as(p)
+        # key of the reset draws: the same on every rank (rank 0's, broadcast like the initial parameters), so every replica
+        # draws the same theta0; the counter is the index of the reset, which the checkpoint keeps once a reset has happened
+        self.reset_seed = (int(torch.initial_seed()) * 2 + 3) & (2 ** 63 - 1)
+        if self.sync.enabled:
+            seed = torch.tensor([self.reset_seed], dtype=torch.int64, device=self.device)
+            self.reset_seed = int(self.sync.broadcast_(seed).item())
+        self.reset_count = 0
+        self._reset_base = None
         self.update_target_net()
         self.target_net.train()
         for p in self.target_net.parameters():
@@ -556,6 +635,7 @@ class Agent:
             x_s.backward(dx)
             self.sync.all_reduce_(self.optimiser.flat_grad)
         self.optimiser.step(grad_scale=1.0 / self.sync.world_size, gate=self._step_gate)
+        self._target_ema()
         if stats_done is not None:
             self._stats_write(stats_done)
         if wb_done is not None:
@@ -590,11 +670,40 @@ class Agent:
         q_s.backward(grad)
         self.sync.all_reduce_(self.optimiser.flat_grad)
         self.optimiser.step(grad_scale=1.0 / self.sync.world_size, gate=self._step_gate)
+        self._target_ema()
         if stats_done is not None:
             self._stats_write(stats_done)
         if after_loss is not None:
             after_loss(loss)
         return loss
+
+    def _target_ema(self):
+        """args.target_tau > 0: the target follows the online parameters just stepped, t <- fma(tau, p, fl32(1 - tau) t),
+        on the caller's stream and under the optimiser's gate (a rejected batch moves neither)."""
+        if self.target_tau > 0.0:
+            _lib.check(_lib.load().rb_target_ema(_lib.ptr(self.target_flat), _lib.ptr(self.optimiser.flat_param),
+                                                 self.optimiser.numel, self.target_tau, _lib.ptr(self._step_gate),
+                                                 _lib.stream()))
+
+    def reset_parameters(self, shrink_encoder=1.0, shrink_head=0.0):
+        """Shrink-and-perturb the online net toward a fresh initialisation theta0 (Ash & Adams 2020; Nikishin et al. 2022;
+        SR-SPR and BBF): theta <- fma(alpha, theta, fl32(1 - alpha) theta0), alpha = shrink_encoder for the conv layers and
+        shrink_head for the four noisy layers.  The defaults re-initialise the head and keep the encoder.  theta0 follows
+        the network's own initialisation (reset_table), drawn by rb_param_reset from the reset seed with the index of this
+        reset as counter: every rank draws the same theta0 and a resumed run repeats the draws.  One launch on the current
+        stream, in place (captured graphs stay valid); the padding of the flat buffer, the Adam moments and step count,
+        the target net, the noise and the replay are untouched (the single flat step count cannot restart Adam's bias
+        correction for a part of the buffer, so the optimiser state is kept as it is)."""
+        alphas = (float(shrink_encoder), float(shrink_head))
+        if not all(0.0 <= a <= 1.0 for a in alphas):
+            raise ValueError(f"shrink_encoder and shrink_head must be in [0, 1], got {alphas}")
+        if self._reset_base is None:
+            self._reset_base = reset_table(self.online_net, self.optimiser.offsets)
+        segs = (_lib.ResetSegment * len(self._reset_base))(
+            *[_lib.ResetSegment(off, n, b, c, alphas[g]) for off, n, b, c, g in self._reset_base])
+        _lib.check(_lib.load().rb_param_reset(_lib.ptr(self.optimiser.flat_param), self.optimiser.numel, segs, len(segs),
+                                              self.reset_seed, self.reset_count, _lib.stream()))
+        self.reset_count += 1
 
     @staticmethod
     def _copies_error(copies):
@@ -679,6 +788,8 @@ class Agent:
             self.online_net._eps_stale = self.online_net._eps_stale or pending
             self.last_loss, mem._last = loss, ws
         self._learn_calls += 1
+        if self.reset_interval and self._learn_calls % self.reset_interval == 0:
+            self.reset_parameters(*self.reset_shrink)
         if self._learn_calls % 4096 == 0 and isinstance(mem, ReplayMemory):
             # diagnostics only (the device already skipped such updates): how many batches stayed invalid after
             # max_attempts redraws -- a ring that is too empty around the write head, or zero-priority leaves

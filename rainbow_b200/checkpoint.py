@@ -3,7 +3,7 @@
 A checkpoint holds everything that decides the next update's result and nothing else (DESIGN.md §9): the online
 parameters (the whole flat buffer, padding included), the target net's parameters, the Adam moments and step count, both
 nets' noise streams (seed, Philox counter, factor vectors, epsilon buffers) and the online net's pending-draw flag, the
-learn-statistics ring, and -- when a ReplayMemory is passed -- the replay's device arrays, ring state, sampling stream and host mirrors.
+parameter-reset key and count, the learn-statistics ring, and -- when a ReplayMemory is passed -- the replay's device arrays, ring state, sampling stream and host mirrors.
 
 Layout: `path/rank{r}/` per data-parallel rank, holding `manifest.json` (format version, world size, rank, optimiser layout,
 structural config, host scalars, a save id shared by all ranks of one save, per array its dtype, shape and SHA-256, and a
@@ -357,6 +357,17 @@ def _meta(agent, mem):
         hyper["augment_intensity"] = agent.augment_intensity
     if agent.augment_copies != (1, 1):
         hyper["augment_m"], hyper["augment_k"] = agent.augment_copies
+    if agent.target_tau:
+        hyper["target_tau"] = agent.target_tau
+    if agent.reset_interval:
+        hyper["reset_interval"] = agent.reset_interval
+    if agent.reset_shrink[0] != 1.0:
+        hyper["reset_shrink_encoder"] = agent.reset_shrink[0]
+    if agent.reset_shrink[1] != 0.0:
+        hyper["reset_shrink_head"] = agent.reset_shrink[1]
+    # always: the key comes from the caller's torch seed, and a resumed process may have another one.  Manifests written
+    # before these keys existed have neither, which load() reads as no reset yet, with the live seed.
+    learner.update(reset_seed=agent.reset_seed, reset_count=agent.reset_count)
     meta = dict(world_size=agent.sync.world_size, rank=agent.sync.rank, optimiser=sd["layout"],
                 structure=_structure(agent, mem), hyper_parameters=hyper, learner=learner, replay=None)
     if mem is not None:
@@ -431,6 +442,8 @@ _SCALARS = {
     ("learner", "optimiser_step"): lambda v, m: _is_int(v, 0, _U63),
     ("learner", "learn_stats_capacity"): lambda v, m: _is_int(v, 0, 2 ** 31),
     ("learner", "learn_stats_read"): lambda v, m: _is_int(v, 0, _U63),
+    ("learner", "reset_seed"): lambda v, m: v is None or _is_int(v, 0, _U63),      # absent (both): an older manifest
+    ("learner", "reset_count"): lambda v, m: v is None or _is_int(v, 0, _U63),
     ("replay", "t"): lambda v, m: _is_int(v, 0, _U63),
     ("replay", "seed"): lambda v, m: _is_int(v, 0, _U64),
     ("replay", "priority_weight"): lambda v, m: isinstance(v, (int, float)) and not isinstance(v, bool) and math.isfinite(v),
@@ -439,6 +452,13 @@ _SCALARS = {
 }
 # a replay field that gets the "state" role in memory.PERSISTENT_ROLES must get its check here
 assert {("replay", k) for k, role in PERSISTENT_ROLES if role == "state"} <= set(_SCALARS)
+
+
+def check_reset_scalars(learner):
+    """The reset key and count come as a pair: both (this format) or neither (a manifest written before they existed).  A
+    count without its key would resume the reset schedule with the live key, a key without a count with index 0."""
+    if (learner.get("reset_seed") is None) != (learner.get("reset_count") is None):
+        raise _Error("manifest learner.reset_seed and learner.reset_count must be given together (or both be absent)")
 
 
 def _validate(agent, mem, man):
@@ -464,6 +484,7 @@ def _validate(agent, mem, man):
         v = (man.get(section) or {}).get(key)
         if not ok(v, mem):
             raise _Error(f"manifest {section}.{key} = {v!r} is missing or out of range")
+    check_reset_scalars(man["learner"])
     cap = man["learner"]["learn_stats_capacity"]
     expected = {n: _spec(t) for n, t in _learner_arrays(agent).items() if n != "learn_stats.ring"}
     if cap:
@@ -537,6 +558,9 @@ def _restore(agent, mem, d, staging):
     # (DESIGN.md §4), so marking them stale here would make that path draw one update early
     on._eps_stale, tg._eps_stale = learner["online_eps_stale"], learner["target_eps_stale"]
     agent._learn_calls = learner["learn_calls"]
+    agent.reset_count = learner.get("reset_count") or 0
+    if learner.get("reset_seed") is not None:
+        agent.reset_seed = learner["reset_seed"]
     if agent._stats is not None:
         agent._stats["read"], agent._stats["last"] = learner["learn_stats_read"], None
     if mem is not None:

@@ -14,6 +14,7 @@
 // __fmul_rn/__fadd_rn/__fsub_rn/__fdiv_rn intrinsics).
 
 #include <cuda_runtime.h>
+#include <float.h>
 #include <math_constants.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -614,8 +615,8 @@ k_gather_shift(const uint8_t* __restrict__ frames, const int32_t* __restrict__ t
 //   copy j multiplier  (c_lo, c_hi, b, INTS_STREAM + j): box_muller(x, y).x -> the state's, box_muller(z, w).x -> the next
 //                      state's.
 // The streams in use: sampling 0x5A4D504C, noise 0x4E4F4953 + i (i < RB_MAX_NOISY_LAYERS), shift 0x53484654 + j and
-// intensity 0x494E5453 + j (j < RB_MAX_AUG_COPIES): the four ranges [0x494E5453, 0x494E545A], [0x4E4F4953, 0x4E4F495A],
-// [0x53484654, 0x5348465B] and {0x5A4D504C} are disjoint.
+// intensity 0x494E5453 + j (j < RB_MAX_AUG_COPIES), parameter reset 0x52534554 ("RSET", k_param_reset): the five ranges
+// [0x494E5453, 0x494E545A], [0x4E4F4953, 0x4E4F495A], {0x52534554}, [0x53484654, 0x5348465B] and {0x5A4D504C} are disjoint.
 constexpr uint32_t INTS_STREAM = 0x494E5453u;        // "INTS"
 
 __device__ __forceinline__ float4 aug4(const uint8_t* s_frame, int y, int x, int dy, int dx, bool scaled, float mult) {
@@ -1856,6 +1857,72 @@ int adam_ctas(int64_t P) {
   return (int)want;
 }
 
+// ================================================================================================
+// K8  target_ema : Polyak target update t = fma(tau, p, fl32(1 - tau) * t) on the flat buffers, after clip + Adam.
+// ================================================================================================
+// Same grid-stride shape as k_clip_adam: float4 when both pointers are 16-byte aligned (plus a scalar tail for n % 4),
+// scalar otherwise.  A gate reading 0 (rejected batch) returns before anything is read or written.
+__device__ __forceinline__ float ema_one(float t, float p, float tau, float keep) {
+  return __fmaf_rn(tau, p, __fmul_rn(keep, t));
+}
+
+__global__ void __launch_bounds__(ADAM_THREADS)
+k_target_ema(float* __restrict__ target, const float* __restrict__ param, int64_t n, float tau,
+             const int32_t* __restrict__ gate) {
+  if (gate && *gate == 0) return;
+  const float keep = __fsub_rn(1.0f, tau);
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if ((((uintptr_t)target | (uintptr_t)param) & 15) == 0) {
+    const int64_t n4 = n >> 2;
+    for (int64_t i = i0; i < n4; i += stride) {
+      float4 t = reinterpret_cast<float4*>(target)[i];
+      const float4 p = __ldg(reinterpret_cast<const float4*>(param) + i);
+      t = make_float4(ema_one(t.x, p.x, tau, keep), ema_one(t.y, p.y, tau, keep), ema_one(t.z, p.z, tau, keep),
+                      ema_one(t.w, p.w, tau, keep));
+      reinterpret_cast<float4*>(target)[i] = t;
+    }
+    const int64_t j = (n4 << 2) + i0;       // the n % 4 elements past the last full float4
+    if (j < n) target[j] = ema_one(target[j], param[j], tau, keep);
+  } else {
+    for (int64_t i = i0; i < n; i += stride) target[i] = ema_one(target[i], param[i], tau, keep);
+  }
+}
+
+// ================================================================================================
+// K9  param_reset : shrink-and-perturb of segments of the flat parameter buffer, theta0 drawn from Philox.
+// ================================================================================================
+// Grid (x: quads of 4 elements, grid-stride; y: segment).  One Philox4x32-10 call per aligned quad j >> 2 gives the words of
+// its four elements; the elements of the quad outside the segment are skipped (padding between tensors is never written).
+constexpr uint32_t RESET_STREAM = 0x52534554u;       // "RSET"
+constexpr int RESET_THREADS = 256;
+
+struct ResetPlan {
+  rb_reset_segment seg[RB_MAX_RESET_SEGMENTS];
+};
+
+__global__ void __launch_bounds__(RESET_THREADS)
+k_param_reset(float* __restrict__ param, const __grid_constant__ ResetPlan plan, uint64_t seed, uint64_t reset_index) {
+  const rb_reset_segment& s = plan.seg[blockIdx.y];
+  const int64_t lo = s.offset, hi = s.offset + s.count;
+  const float alpha = s.alpha, keep = __fsub_rn(1.0f, s.alpha), bound = s.bound, constant = s.constant;
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t q = (lo >> 2) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; (q << 2) < hi; q += stride) {
+    const uint4 r = philox4x32_10(make_uint4((uint32_t)reset_index, (uint32_t)(reset_index >> 32), (uint32_t)q, RESET_STREAM),
+                                  key);
+    const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int64_t j = (q << 2) + e;
+      if (j < lo || j >= hi) continue;
+      const float u = (float)(w[e] >> 8) * 0x1.0p-24f;
+      const float theta0 = __fmaf_rn(bound, __fmaf_rn(2.0f, u, -1.0f), constant);
+      param[j] = __fmaf_rn(alpha, param[j], __fmul_rn(keep, theta0));
+    }
+  }
+}
+
 // The launch of rb_append and rb_append_batch, after each has checked its own arguments.
 int append_launch(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
                   float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max, const AppendBatch& ab,
@@ -2323,6 +2390,47 @@ int rb_clip_adam(float* param, const float* grad, float* exp_avg, float* exp_avg
                                                                beta1, beta2, eps, step_count, partial_sums, ctas, norm_out,
                                                                reinterpret_cast<unsigned int*>(partial_sums + ADAM_MAX_CTAS), gate); }
   return check_launch("rb_clip_adam");
+}
+
+int rb_target_ema(float* target, const float* param, int64_t n, float tau, const int32_t* gate, rb_stream_t stream) {
+  if (!target || !param) return fail(RB_ERR_INVAL, "rb_target_ema: null pointer");
+  if (n < 0) return fail(RB_ERR_INVAL, "rb_target_ema: n must not be negative");
+  if (!(tau > 0.0f && tau <= 1.0f)) return fail(RB_ERR_RANGE, "rb_target_ema: tau outside (0, 1]");
+  const uintptr_t t0 = (uintptr_t)target, p0 = (uintptr_t)param, bytes = (uintptr_t)n * sizeof(float);
+  if (n > 0 && t0 < p0 + bytes && p0 < t0 + bytes) return fail(RB_ERR_INVAL, "rb_target_ema: target and param overlap");
+  if (n == 0) return RB_OK;
+  const int ctas = adam_ctas(n);
+  { ProfScope prof_(RB_K_TARGET_EMA, (cudaStream_t)stream);
+    k_target_ema<<<ctas, ADAM_THREADS, 0, (cudaStream_t)stream>>>(target, param, n, tau, gate); }
+  return check_launch("rb_target_ema");
+}
+
+int rb_param_reset(float* param, int64_t n, const rb_reset_segment* segs, int n_segs, uint64_t seed, uint64_t reset_index,
+                   rb_stream_t stream) {
+  if (!param || !segs) return fail(RB_ERR_INVAL, "rb_param_reset: null pointer");
+  if (n_segs < 1 || n_segs > RB_MAX_RESET_SEGMENTS)
+    return fail(RB_ERR_RANGE, "rb_param_reset: n_segs outside [1, RB_MAX_RESET_SEGMENTS]");
+  ResetPlan plan;
+  memset(&plan, 0, sizeof(plan));
+  int64_t end = 0, widest = 0;
+  for (int i = 0; i < n_segs; ++i) {
+    const rb_reset_segment& s = segs[i];
+    if (s.count <= 0 || s.offset < end || s.offset > n - s.count)
+      return fail(RB_ERR_RANGE, "rb_param_reset: segment empty, outside [0, n), unsorted or overlapping");
+    if (!(s.bound >= 0.0f && s.bound <= FLT_MAX) || !(s.constant >= 0.0f && s.constant <= FLT_MAX))
+      return fail(RB_ERR_RANGE, "rb_param_reset: bound and constant must be finite and non-negative");
+    if (!(s.alpha >= 0.0f && s.alpha <= 1.0f)) return fail(RB_ERR_RANGE, "rb_param_reset: alpha outside [0, 1]");
+    plan.seg[i] = s;
+    end = s.offset + s.count;
+    const int64_t quads = ((end - 1) >> 2) - (s.offset >> 2) + 1;
+    if (quads > widest) widest = quads;
+  }
+  int64_t ctas = (widest + RESET_THREADS - 1) / RESET_THREADS;
+  if (ctas > rbi::SM_COUNT * 4) ctas = rbi::SM_COUNT * 4;
+  dim3 grid((unsigned)ctas, (unsigned)n_segs);
+  { ProfScope prof_(RB_K_PARAM_RESET, (cudaStream_t)stream);
+    k_param_reset<<<grid, RESET_THREADS, 0, (cudaStream_t)stream>>>(param, plan, seed, reset_index); }
+  return check_launch("rb_param_reset");
 }
 
 }  // extern "C"
