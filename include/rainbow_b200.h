@@ -61,6 +61,7 @@ extern "C" {
 #define RB_MAX_SHIFT_PAD 16      /* largest pad of rb_gather_shift */
 #define RB_MAX_AUG_COPIES 8      /* most copies of a state (M) or next state (K) in rb_gather_aug */
 #define RB_MAX_RESET_SEGMENTS 32 /* most parameter tensors one rb_param_reset call covers */
+#define RB_MAX_ANNEAL_STEPS 65536 /* longest horizon schedule (T) of rb_horizon_advance */
 
 /* status words written by rb_tree_sample (int32[4]): status[0] = 1 if the batch now in the output buffers passed the
  * whole-batch validity test (memory.py:131), 0 otherwise; status[1] = draws used; status[2] = number of device-RNG
@@ -168,6 +169,40 @@ int rb_gather_aug(const uint8_t* frames, const int32_t* timestep, const int32_t*
                   const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
                   float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
                   const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream);
+
+/* An annealed update horizon (BBF, Schwarzer et al. 2023; no reference counterpart): one row per update step u of the
+ * schedule, built on the host.  n = n_u (>= 1), gamma_n = fl32(gamma_u ** n_u), gamma_pow[k] = fl32(gamma_u ** k) for
+ * k < n_u and 0 beyond.  A table holds T + 1 rows, u = 0 .. T. */
+typedef struct rb_horizon {
+  int32_t n;
+  float gamma_n;
+  float gamma_pow[RB_MAX_WINDOW];
+} rb_horizon;
+
+/* One thread: *current = table[min(*counter, T)] (a negative counter reads row 0), then *counter += 1 (int64, device).
+ * The update graph's first node when the horizon is annealed; it has no profiling id (time it with events around the
+ * launch).  RB_ERR_INVAL: a NULL pointer; RB_ERR_RANGE: T outside
+ * [1, RB_MAX_ANNEAL_STEPS].  A refused call launches nothing. */
+int rb_horizon_advance(const rb_horizon* table, int T, int64_t* counter, rb_horizon* current, rb_stream_t stream);
+
+/* rb_gather, rb_gather_shift and rb_gather_aug with the horizon read from the device row *current (as
+ * rb_horizon_advance left it) instead of the arguments n and gamma_pow.  n_max sizes the window: the replay must have
+ * been sampled for n_max (rb_tree_sample with n = n_max), and the row's n is clamped into [1, n_max].  With n_t, gamma_pow
+ * and gamma_n of the row, every output is bitwise what the fixed-horizon kernel writes with n = n_t and that gamma_pow,
+ * except nonterminals, which come in discount form: fl32(nonterminal * gamma_n), i.e. gamma_n or +0.  A loss kernel
+ * (rb_c51_*) launched on them with gamma_n = 1 computes what it computes on 0 / 1 nonterminals with the row's gamma_n.
+ * The augmentation arguments select the kernel as the Python sampler does: pad 0, intensity 0 and M = K = 1 gathers like
+ * rb_gather (rng_counter, shifts and scales may be NULL); pad > 0 with intensity 0 and M = K = 1 like rb_gather_shift
+ * (shifts int32[2][B][2]; scales may be NULL); anything else like rb_gather_aug, with its layouts and its draws.
+ * RB_ERR_RANGE: pad outside [0, RB_MAX_SHIFT_PAD], intensity outside [0, 0.5] or NaN, copies outside
+ * [1, RB_MAX_AUG_COPIES], plus every check of rb_gather with n = n_max; RB_ERR_INVAL: a NULL pointer the selected kernel
+ * needs.  A refused call launches nothing.  Profiled under the id of the gather it stands for (RB_K_GATHER,
+ * RB_K_GATHER_SHIFT or RB_K_GATHER_AUG). */
+int rb_gather_horizon(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                      const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n_max,
+                      const rb_horizon* current, float* states, float* next_states, int64_t* actions, float* returns,
+                      float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
+                      const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream);
 
 /* memory.py:166-178 ReplayMemory.__next__, batched: states for current_idx = first .. first+count-1,
  * backward-only blanking, negative indices wrap.  out is float32[count][history][84*84]. */

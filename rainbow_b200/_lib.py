@@ -30,6 +30,11 @@ class ResetSegment(C.Structure):
                 ("alpha", C.c_float)]
 
 
+class Horizon(C.Structure):
+    """rb_horizon: one row of an annealed-horizon table (n, gamma ** n, gamma ** k for k < n then zeros)."""
+    _fields_ = [("n", C.c_int32), ("gamma_n", C.c_float), ("gamma_pow", C.c_float * 64)]
+
+
 _hp, _hg = C.POINTER(HeadParams), C.POINTER(HeadGrads)
 
 # name -> (restype, argtypes); must list every symbol declared in include/rainbow_b200.h
@@ -47,6 +52,9 @@ SIGNATURES = {
                                   _u64, _vp, _vp, _vp]),
     "rb_gather_aug": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32,
                                 _f32, _i32, _i32, _u64, _vp, _vp, _vp, _vp]),
+    "rb_horizon_advance": (C.c_int, [_vp, _i32, _vp, _vp, _vp]),
+    "rb_gather_horizon": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                    _i32, _f32, _i32, _i32, _u64, _vp, _vp, _vp, _vp]),
     "rb_iter_states": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _i32, _vp, _vp]),
     "rb_append": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int32, _f32, _i32, _vp]),
     "rb_append_batch": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),

@@ -2,11 +2,15 @@
 
 One `learn(mem)` (agent.py:61-100) is:
 
+    [args.anneal_steps = T > 0: rb_horizon_advance on a side branch beside K1 -- the step's n and gamma of BBF's annealed
+     horizon (rainbow_b200.horizon), read by the gather]
     K1 rb_tree_sample + K2 rb_gather          (mem.sample, memory.py:148-155)
                                               [args.augment_shift = p > 0: rb_gather_shift instead -- random-shift
                                                augmentation of s and s' (DrQ), offsets drawn on the device;
                                                args.augment_intensity > 0 or augment_m / augment_k > 1: rb_gather_aug --
-                                               shift + intensity augmentation of M copies of s and K copies of s']
+                                               shift + intensity augmentation of M copies of s and K copies of s';
+                                               args.anneal_steps > 0: rb_gather_horizon, any of the three with the
+                                               annealed n and gamma, nonterminals as gamma^n or 0 and K3 with gamma_n = 1]
     3 x conv body (torch: cuDNN)              (agent.py:66,71,75 -> model.py:70-71)
     K6 rb_noisy_resample (target net)         (agent.py:74)
     fused noisy dueling heads (rb_head_forward) on the conv features -- online net on [s; s'], target on s'
@@ -26,7 +30,8 @@ Nothing in that chain synchronises with the host, so the whole update is capture
 (the reference issues ~600 ATen ops per update, SURVEY.md 2.1).
 
 [args.reset_interval = N > 0: after every N-th learn(), one rb_param_reset launch outside the graph -- shrink-and-perturb
- of the online parameters toward a fresh initialisation drawn on the device (Agent.reset_parameters)]
+ of the online parameters toward a fresh initialisation drawn on the device (Agent.reset_parameters); every reset also
+ restarts an annealed horizon at its first step]
 """
 import math
 import os
@@ -39,6 +44,7 @@ from torch import nn
 
 from . import _lib
 from .dist import GradSync
+from .horizon import HorizonSchedule
 from .memory import ReplayMemory, _SampleWorkspace
 from .model import DQN, FusedHead, NoisyLinear
 
@@ -268,6 +274,11 @@ class Agent:
         # Polyak target updates (tau > 0: every applied optimiser step also moves the target, DrQ(eps) / SPR / BBF) and
         # periodic shrink-and-perturb resets of the online net (SR-SPR, BBF); both off by default
         self.target_tau, self.reset_interval, self.reset_shrink = target_reset_options(args)
+        # BBF's annealed update horizon: n and gamma move from (multi_step_start, discount_start) to (multi_step, discount)
+        # over anneal_steps updates after the Agent is built and after every reset; None when args.anneal_steps is 0
+        self._horizon = HorizonSchedule.from_args(args, self.device)
+        if self._horizon is not None and self._horizon.n_max + self.history > 64:
+            raise ValueError("history_length + max(multi_step, multi_step_start) must not exceed 64")
 
         self.online_net = DQN(args, self.action_space).to(device=self.device)
         model_path = getattr(args, "model", None)
@@ -574,11 +585,11 @@ class Agent:
             if (M, K) == (1, 1):
                 loss, dz = c51_dueling_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
                                                  weights, self.support, self.Vmin, self.Vmax, self.delta_z,
-                                                 self.discount ** self.n, m_out=m)
+                                                 self._gamma_n(), m_out=m)
             else:
                 loss, dz = c51_dueling_avg_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
                                                      weights, self.support, self.Vmin, self.Vmax, self.delta_z,
-                                                     self.discount ** self.n, M, K, m_out=m)
+                                                     self._gamma_n(), M, K, m_out=m)
             stats_done = self._stats_batch(batch, loss, m, z=z_on) if m is not None else None
             wb_done = None
             if after_loss is not None:
@@ -664,7 +675,7 @@ class Agent:
             q_t = self.target_net.logits(next_states)
             m = torch.empty((q_s.shape[0], self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
             loss, grad = c51_loss_grad(q_s.detach(), q_ns, q_t, actions, returns, nonterminals, weights, self.support,
-                                       self.Vmin, self.Vmax, self.delta_z, self.discount ** self.n, m_out=m)
+                                       self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m)
             stats_done = self._stats_batch(batch, loss, m, q=q_s.detach()) if m is not None else None
         self.optimiser.zero_grad()
         q_s.backward(grad)
@@ -676,6 +687,18 @@ class Agent:
         if after_loss is not None:
             after_loss(loss)
         return loss
+
+    def _gamma_n(self):
+        """The gamma_n the loss kernels take: gamma ** n, or 1 with an annealed horizon, whose gather writes the nonterminals
+        as fl32(nonterminal * gamma_u ** n_u) -- the kernels use a nonterminal only in fl32(nonterminal * gamma_n), so
+        the products, and everything after them, are bitwise those of the fixed horizon (n_u, gamma_u)."""
+        return 1.0 if self._horizon is not None else self.discount ** self.n
+
+    def horizon(self):
+        """(n, gamma) the next update trains with: the annealed schedule's current step, or (multi_step, discount)."""
+        if self._horizon is None:
+            return self.n, self.discount
+        return self._horizon.at(self._horizon.step)
 
     def _target_ema(self):
         """args.target_tau > 0: the target follows the online parameters just stepped, t <- fma(tau, p, fl32(1 - tau) t),
@@ -693,7 +716,8 @@ class Agent:
         reset as counter: every rank draws the same theta0 and a resumed run repeats the draws.  One launch on the current
         stream, in place (captured graphs stay valid); the padding of the flat buffer, the Adam moments and step count,
         the target net, the noise and the replay are untouched (the single flat step count cannot restart Adam's bias
-        correction for a part of the buffer, so the optimiser state is kept as it is)."""
+        correction for a part of the buffer, so the optimiser state is kept as it is).  An annealed horizon restarts at its
+        first step (n0, gamma0)."""
         alphas = (float(shrink_encoder), float(shrink_head))
         if not all(0.0 <= a <= 1.0 for a in alphas):
             raise ValueError(f"shrink_encoder and shrink_head must be in [0, 1], got {alphas}")
@@ -704,6 +728,8 @@ class Agent:
         _lib.check(_lib.load().rb_param_reset(_lib.ptr(self.optimiser.flat_param), self.optimiser.numel, segs, len(segs),
                                               self.reset_seed, self.reset_count, _lib.stream()))
         self.reset_count += 1
+        if self._horizon is not None:
+            self._horizon.restart()
 
     @staticmethod
     def _copies_error(copies):
@@ -715,7 +741,7 @@ class Agent:
     def _learn_eager(self, mem):
         if isinstance(mem, ReplayMemory):
             batch = mem.sample(self.batch_size, shift_pad=self.augment_shift, intensity=self.augment_intensity,
-                               copies=self.augment_copies)
+                               copies=self.augment_copies, horizon=self._horizon)
             gate = mem.sample_gate()
             return self._update_from_batch(batch, after_loss=lambda loss: mem.update_priorities(batch[0], loss, gate=gate),
                                            gate=gate)
@@ -734,7 +760,7 @@ class Agent:
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             batch = mem.sample_into(ws, shift_pad=self.augment_shift, intensity=self.augment_intensity,
-                                    copies=self.augment_copies)
+                                    copies=self.augment_copies, horizon=self._horizon)
             loss = self._update_from_batch(batch, after_loss=lambda l: mem.update_priorities(batch[0], l, gate=ws.status),
                                            gate=ws.status)
         return graph, ws, loss
@@ -756,6 +782,10 @@ class Agent:
         if (self.augment_intensity or self.augment_copies != (1, 1)) and not isinstance(mem, ReplayMemory):
             raise _lib.RainbowB200Error("args.augment_intensity / augment_m / augment_k need a rainbow_b200 ReplayMemory: "
                                         "the augmented copies are drawn and written on the device by its gather")
+        if self._horizon is not None and not (isinstance(mem, ReplayMemory) and mem.n >= self._horizon.n_max):
+            raise _lib.RainbowB200Error(
+                f"args.anneal_steps needs a rainbow_b200 ReplayMemory built for n >= {self._horizon.n_max} (it reads "
+                "args.multi_step_start): the annealed horizon is gathered on the device")
         if self.augment_copies != (1, 1) and not self._fused_path(self.batch_size):
             raise self._copies_error(self.augment_copies)   # before sampling: a refused learn() leaves the replay as it was
         # the captured graph bakes in: this memory's buffers, the batch size and training-mode (noisy) weights
@@ -784,6 +814,8 @@ class Agent:
             mem.flush_appends()   # no-op unless the memory defers its appends
             mem.push_beta()
             graph.replay()
+            if self._horizon is not None:
+                self._horizon.step += 1   # the replay's rb_horizon_advance
             self.online_net._noise_pending = False
             self.online_net._eps_stale = self.online_net._eps_stale or pending
             self.last_loss, mem._last = loss, ws

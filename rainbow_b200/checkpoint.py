@@ -365,6 +365,14 @@ def _meta(agent, mem):
         hyper["reset_shrink_encoder"] = agent.reset_shrink[0]
     if agent.reset_shrink[1] != 0.0:
         hyper["reset_shrink_head"] = agent.reset_shrink[1]
+    hz = agent._horizon
+    if hz is not None:   # the annealed horizon's options (when not their defaults) and the cycle step of the next update
+        hyper["anneal_steps"] = hz.T
+        if hz.n0 != hz.n1:
+            hyper["multi_step_start"] = hz.n0
+        if hz.g0 != hz.g1:
+            hyper["discount_start"] = hz.g0
+        learner["horizon_step"] = hz.step
     # always: the key comes from the caller's torch seed, and a resumed process may have another one.  Manifests written
     # before these keys existed have neither, which load() reads as no reset yet, with the live seed.
     learner.update(reset_seed=agent.reset_seed, reset_count=agent.reset_count)
@@ -444,6 +452,7 @@ _SCALARS = {
     ("learner", "learn_stats_read"): lambda v, m: _is_int(v, 0, _U63),
     ("learner", "reset_seed"): lambda v, m: v is None or _is_int(v, 0, _U63),      # absent (both): an older manifest
     ("learner", "reset_count"): lambda v, m: v is None or _is_int(v, 0, _U63),
+    ("learner", "horizon_step"): lambda v, m: v is None or _is_int(v, 0, _U63),     # absent: annealing off, or step 0
     ("replay", "t"): lambda v, m: _is_int(v, 0, _U63),
     ("replay", "seed"): lambda v, m: _is_int(v, 0, _U64),
     ("replay", "priority_weight"): lambda v, m: isinstance(v, (int, float)) and not isinstance(v, bool) and math.isfinite(v),
@@ -561,6 +570,8 @@ def _restore(agent, mem, d, staging):
     agent.reset_count = learner.get("reset_count") or 0
     if learner.get("reset_seed") is not None:
         agent.reset_seed = learner["reset_seed"]
+    if agent._horizon is not None:
+        agent._horizon.set_step(learner.get("horizon_step") or 0)
     if agent._stats is not None:
         agent._stats["read"], agent._stats["last"] = learner["learn_stats_read"], None
     if mem is not None:

@@ -447,12 +447,14 @@ __device__ __forceinline__ float4 u8x4_to_unit(uint32_t w) {
                      __fdiv_rn((float)((w >> 16) & 0xffu), 255.0f), __fdiv_rn((float)(w >> 24), 255.0f));
 }
 
-// per-sample scalars, once per sample (memory.py:140-145)
+// per-sample scalars, once per sample (memory.py:140-145).  HZ (rb_gather_horizon): the nonterminal is written in discount
+// form, fl32(nonterminal * gamma_n), i.e. gamma_n or +0.
+template <bool HZ>
 __device__ __forceinline__ void gather_scalars(uint64_t first, const int32_t* __restrict__ action, const float* __restrict__ reward,
                                                const uint8_t* __restrict__ nonterminal, int64_t size, int64_t idx, int b,
                                                int history, int n, const float* __restrict__ gamma_pow,
                                                int64_t* __restrict__ actions, float* __restrict__ returns,
-                                               float* __restrict__ nonterminals) {
+                                               float* __restrict__ nonterminals, float gamma_n) {
   const int sa = history - 1;
   actions[b] = (int64_t)__ldg(action + pymod(idx, size));  // slot H-1 is never blanked
   float acc = 0.0f;
@@ -463,19 +465,30 @@ __device__ __forceinline__ void gather_scalars(uint64_t first, const int32_t* __
   }
   returns[b] = acc;
   const int sl = history + n - 1;
-  nonterminals[b] = slot_blank(first, sl, history) ? 0.0f : (__ldg(nonterminal + pymod(idx + n, size)) ? 1.0f : 0.0f);
+  const float nt = slot_blank(first, sl, history) ? 0.0f : (__ldg(nonterminal + pymod(idx + n, size)) ? 1.0f : 0.0f);
+  if constexpr (HZ) nonterminals[b] = __fmul_rn(nt, gamma_n);
+  else nonterminals[b] = nt;
 }
 
-__global__ void __launch_bounds__(GATHER_THREADS)
-k_gather(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
-         const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
-         const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
-         float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
-         float* __restrict__ returns, float* __restrict__ nonterminals, int split) {
+// rb_gather_horizon: the three gather bodies below take n (the n_max the grid and the blanking window are sized for) and
+// gamma_pow from their arguments when HZ is false, and n_t = clamp(hz->n, 1, n_max), gamma_pow and gamma_n from the
+// schedule's current row when it is true.  Window slots the grid holds for n_max but n_t does not use -- used slots
+// >= H + min(n_t, H) -- exit at once; the rest map as for a launch with n = n_t.  A slot's blanking depends only on the
+// slots between it and slot H - 1, so the wider ballot changes nothing.
+template <bool HZ>
+__device__ __forceinline__ void
+gather_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+            const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+            const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+            float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+            float* __restrict__ returns, float* __restrict__ nonterminals, int split, const rb_horizon* __restrict__ hz) {
   __shared__ uint64_t s_first;
   const int b = blockIdx.y;
   const int W = history + n;
+  float gamma_n = 1.0f;
+  if constexpr (HZ) { n = min(max(__ldg(&hz->n), 1), n); gamma_pow = hz->gamma_pow; gamma_n = __ldg(&hz->gamma_n); }
   const int used = blockIdx.x / split, part = blockIdx.x % split;
+  if (HZ && used >= history + min(n, history)) return;
   // used-slot -> window slot: slots [0,H) feed `states`, [n,n+H) feed `next_states`
   const int s = (n >= history && used >= history) ? n + (used - history) : used;
   const int64_t idx = data_idx[b];
@@ -509,7 +522,28 @@ k_gather(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timeste
     }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0)
-    gather_scalars(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns, nonterminals);
+    gather_scalars<HZ>(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns,
+                       nonterminals, gamma_n);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+         const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+         const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+         float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+         float* __restrict__ returns, float* __restrict__ nonterminals, int split) {
+  gather_body<false>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states,
+                     next_states, actions, returns, nonterminals, split, nullptr);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+            const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+            const int64_t* __restrict__ data_idx, int B, int history, int n_max, const rb_horizon* __restrict__ hz,
+            float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+            float* __restrict__ returns, float* __restrict__ nonterminals, int split) {
+  gather_body<true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, nullptr, states,
+                    next_states, actions, returns, nonterminals, split, hz);
 }
 
 // ================================================================================================
@@ -541,18 +575,24 @@ __device__ __forceinline__ float4 shifted4(const uint8_t* s_frame, int y, int x,
                      __fdiv_rn((float)row[clamp_px(x + 2 + dx)], 255.0f), __fdiv_rn((float)row[clamp_px(x + 3 + dx)], 255.0f));
 }
 
-__global__ void __launch_bounds__(GATHER_THREADS)
-k_gather_shift(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
-               const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
-               const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
-               float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
-               float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
-               const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
+template <bool HZ>
+__device__ __forceinline__ void
+gather_shift_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep,
+                  const int32_t* __restrict__ action, const float* __restrict__ reward,
+                  const uint8_t* __restrict__ nonterminal, int64_t size, const int64_t* __restrict__ data_idx, int B,
+                  int history, int n, const float* __restrict__ gamma_pow, float* __restrict__ states,
+                  float* __restrict__ next_states, int64_t* __restrict__ actions, float* __restrict__ returns,
+                  float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
+                  const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts,
+                  const rb_horizon* __restrict__ hz) {
   __shared__ uint64_t s_first;
   __shared__ __align__(16) uint8_t s_frame[RB_FRAME_BYTES];
   const int b = blockIdx.y;
   const int W = history + n;
+  float gamma_n = 1.0f;
+  if constexpr (HZ) { n = min(max(__ldg(&hz->n), 1), n); gamma_pow = hz->gamma_pow; gamma_n = __ldg(&hz->gamma_n); }
   const int used = blockIdx.x / split, part = blockIdx.x % split;
+  if (HZ && used >= history + min(n, history)) return;
   const int s = (n >= history && used >= history) ? n + (used - history) : used;
   const int64_t idx = data_idx[b];
   const int64_t pos = pymod(idx - (history - 1) + s, size);
@@ -593,12 +633,36 @@ k_gather_shift(const uint8_t* __restrict__ frames, const int32_t* __restrict__ t
     if (dst_n) __stcs(dst_n + i, blank ? zero : shifted4(s_frame, y, x, oy_n - pad, ox_n - pad));
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    gather_scalars(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns, nonterminals);
+    gather_scalars<HZ>(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns,
+                       nonterminals, gamma_n);
     int32_t* sh_s = shifts + 2 * (size_t)b;          // int32 [2][B][2]: (side, sample, (oy, ox))
     int32_t* sh_n = shifts + 2 * ((size_t)B + b);
     sh_s[0] = oy_s; sh_s[1] = ox_s;
     sh_n[0] = oy_n; sh_n[1] = ox_n;
   }
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_shift(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+               const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+               const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+               float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+               float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
+               const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
+  gather_shift_body<false>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states,
+                           next_states, actions, returns, nonterminals, split, pad, seed, rng_counter, shifts, nullptr);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_shift_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep,
+                  const int32_t* __restrict__ action, const float* __restrict__ reward,
+                  const uint8_t* __restrict__ nonterminal, int64_t size, const int64_t* __restrict__ data_idx, int B,
+                  int history, int n_max, const rb_horizon* __restrict__ hz, float* __restrict__ states,
+                  float* __restrict__ next_states, int64_t* __restrict__ actions, float* __restrict__ returns,
+                  float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
+                  const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
+  gather_shift_body<true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, nullptr, states,
+                          next_states, actions, returns, nonterminals, split, pad, seed, rng_counter, shifts, hz);
 }
 
 // ================================================================================================
@@ -629,22 +693,26 @@ __device__ __forceinline__ float intensity_mult(float s, float normal) {
   return __fmaf_rn(s, fminf(fmaxf(normal, -2.0f), 2.0f), 1.0f);
 }
 
-__global__ void __launch_bounds__(GATHER_THREADS)
-k_gather_aug(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
-             const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
-             const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
-             float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
-             float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, float intensity, int m_copies,
-             int k_copies, uint64_t seed, const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts,
-             float* __restrict__ scales) {
+template <bool HZ>
+__device__ __forceinline__ void
+gather_aug_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+                const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+                const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+                float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+                float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, float intensity,
+                int m_copies, int k_copies, uint64_t seed, const unsigned long long* __restrict__ rng_counter,
+                int32_t* __restrict__ shifts, float* __restrict__ scales, const rb_horizon* __restrict__ hz) {
   __shared__ uint64_t s_first;
   __shared__ int s_off[2][RB_MAX_AUG_COPIES][2];   // (side, copy, (dy, dx)) = offset - pad
   __shared__ float s_mult[2][RB_MAX_AUG_COPIES];
   __shared__ __align__(16) uint8_t s_frame[RB_FRAME_BYTES];
   const int b = blockIdx.y;
   const int W = history + n;
+  float gamma_n = 1.0f;
+  if constexpr (HZ) { n = min(max(__ldg(&hz->n), 1), n); gamma_pow = hz->gamma_pow; gamma_n = __ldg(&hz->gamma_n); }
   const int copies = max(m_copies, k_copies);
   const int used = blockIdx.x / split, part = blockIdx.x % split;
+  if (HZ && used >= history + min(n, history)) return;
   const int s = (n >= history && used >= history) ? n + (used - history) : used;
   const int64_t idx = data_idx[b];
   const int64_t pos = pymod(idx - (history - 1) + s, size);
@@ -715,7 +783,49 @@ k_gather_aug(const uint8_t* __restrict__ frames, const int32_t* __restrict__ tim
     }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0)
-    gather_scalars(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns, nonterminals);
+    gather_scalars<HZ>(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns,
+                       nonterminals, gamma_n);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_aug(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+             const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+             const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+             float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+             float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, float intensity, int m_copies,
+             int k_copies, uint64_t seed, const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts,
+             float* __restrict__ scales) {
+  gather_aug_body<false>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states,
+                         next_states, actions, returns, nonterminals, split, pad, intensity, m_copies, k_copies, seed,
+                         rng_counter, shifts, scales, nullptr);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_aug_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+                const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+                const int64_t* __restrict__ data_idx, int B, int history, int n_max, const rb_horizon* __restrict__ hz,
+                float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+                float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, float intensity,
+                int m_copies, int k_copies, uint64_t seed, const unsigned long long* __restrict__ rng_counter,
+                int32_t* __restrict__ shifts, float* __restrict__ scales) {
+  gather_aug_body<true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, nullptr, states,
+                        next_states, actions, returns, nonterminals, split, pad, intensity, m_copies, k_copies, seed,
+                        rng_counter, shifts, scales, hz);
+}
+
+// One thread: current <- table[min(*counter, T)] (a negative counter reads row 0), then ++*counter.  The first node of an
+// update that anneals its horizon; it runs beside rb_tree_sample, and the gather waits for it.
+__global__ void __launch_bounds__(1)
+k_horizon_advance(const rb_horizon* __restrict__ table, int T, long long* __restrict__ counter,
+                  rb_horizon* __restrict__ current) {
+  const long long u = *counter;
+  const int row = u <= 0 ? 0 : (u >= T ? T : (int)u);
+  const rb_horizon* __restrict__ src = table + row;
+  current->n = src->n;
+  current->gamma_n = src->gamma_n;
+#pragma unroll
+  for (int k = 0; k < RB_MAX_WINDOW; ++k) current->gamma_pow[k] = src->gamma_pow[k];
+  *counter = u + 1;
 }
 
 // memory.py:166-178 validation iterator, batched: grid = (history, count)
@@ -2104,6 +2214,55 @@ int rb_gather_aug(const uint8_t* frames, const int32_t* timestep, const int32_t*
       returns, nonterminals, split, pad, intensity, m_copies, k_copies, seed, (const unsigned long long*)rng_counter, shifts,
       scales); }
   return check_launch("rb_gather_aug");
+}
+
+int rb_horizon_advance(const rb_horizon* table, int T, int64_t* counter, rb_horizon* current, rb_stream_t stream) {
+  if (!table || !counter || !current) return fail(RB_ERR_INVAL, "rb_horizon_advance: null pointer");
+  if (T < 1 || T > RB_MAX_ANNEAL_STEPS) return fail(RB_ERR_RANGE, "rb_horizon_advance: T outside [1, RB_MAX_ANNEAL_STEPS]");
+  k_horizon_advance<<<1, 1, 0, (cudaStream_t)stream>>>(table, T, (long long*)counter, current);
+  return check_launch("rb_horizon_advance");
+}
+
+int rb_gather_horizon(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                      const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n_max,
+                      const rb_horizon* current, float* states, float* next_states, int64_t* actions, float* returns,
+                      float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
+                      const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream) {
+  if (!current) return fail(RB_ERR_INVAL, "rb_gather_horizon: null pointer");
+  const int rc = gather_check("rb_gather_horizon", frames, timestep, action, reward, nonterminal, size, data_idx, B, history,
+                              n_max, reinterpret_cast<const float*>(current), states, next_states, actions, returns,
+                              nonterminals);
+  if (rc != RB_OK) return rc;
+  if (pad < 0 || pad > RB_MAX_SHIFT_PAD) return fail(RB_ERR_RANGE, "rb_gather_horizon: pad outside [0, RB_MAX_SHIFT_PAD]");
+  if (!(intensity >= 0.0f && intensity <= 0.5f)) return fail(RB_ERR_RANGE, "rb_gather_horizon: intensity outside [0, 0.5]");
+  if (m_copies < 1 || m_copies > RB_MAX_AUG_COPIES || k_copies < 1 || k_copies > RB_MAX_AUG_COPIES)
+    return fail(RB_ERR_RANGE, "rb_gather_horizon: copies outside [1, RB_MAX_AUG_COPIES]");
+  const bool plain = pad == 0 && intensity == 0.0f && m_copies == 1 && k_copies == 1;
+  const bool shift = !plain && intensity == 0.0f && m_copies == 1 && k_copies == 1;
+  if (!plain && (!rng_counter || !shifts || (!shift && !scales)))
+    return fail(RB_ERR_INVAL, "rb_gather_horizon: null pointer");
+  // the grid of a launch with n = n_max; k_*_hz retire the slots the current n does not use
+  const int used = (history + n_max < 2 * history) ? history + n_max : 2 * history;
+  const int split = gather_split(used * B);
+  dim3 grid(used * split, B);
+  const unsigned long long* ctr = (const unsigned long long*)rng_counter;
+  cudaStream_t s = (cudaStream_t)stream;
+  // profiled under the id of the gather this launch stands for
+  { ProfScope prof_(plain ? RB_K_GATHER : shift ? RB_K_GATHER_SHIFT : RB_K_GATHER_AUG, s);
+    if (plain)
+      k_gather_hz<<<grid, GATHER_THREADS, 0, s>>>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history,
+                                                  n_max, current, states, next_states, actions, returns, nonterminals,
+                                                  split);
+    else if (shift)
+      k_gather_shift_hz<<<grid, GATHER_THREADS, 0, s>>>(frames, timestep, action, reward, nonterminal, size, data_idx, B,
+                                                        history, n_max, current, states, next_states, actions, returns,
+                                                        nonterminals, split, pad, seed, ctr, shifts);
+    else
+      k_gather_aug_hz<<<grid, GATHER_THREADS, 0, s>>>(frames, timestep, action, reward, nonterminal, size, data_idx, B,
+                                                      history, n_max, current, states, next_states, actions, returns,
+                                                      nonterminals, split, pad, intensity, m_copies, k_copies, seed, ctr,
+                                                      shifts, scales); }
+  return check_launch("rb_gather_horizon");
 }
 
 int rb_iter_states(const uint8_t* frames, const int32_t* timestep, int64_t size, int64_t first, int count, int history,

@@ -10,7 +10,8 @@ called through the C ABI in include/rainbow_b200.h:
                           rb_gather        (K2)   memory.py:111-121, 134-146
                           (rb_gather_shift with shift_pad > 0: the same plus random-shift augmentation, no reference
                           counterpart; rb_gather_aug with intensity > 0 or copies != (1, 1): shift and intensity
-                          augmentation of M copies of s and K of s')
+                          augmentation of M copies of s and K of s'; rb_gather_horizon with an annealed horizon, see
+                          rainbow_b200.horizon)
     update_priorities  -> rb_tree_update   (K4)   memory.py:157-159, 23-48
     __next__           -> rb_iter_states          memory.py:166-178
 
@@ -253,6 +254,8 @@ class ReplayMemory:
         self.history = int(args.history_length)
         self.discount = args.discount
         self.n = int(args.multi_step)
+        if getattr(args, "anneal_steps", None):   # an annealed horizon (rainbow_b200.horizon): the window of its longest n
+            self.n = max(self.n, int(getattr(args, "multi_step_start", None) or self.n))
         self.priority_weight = args.priority_weight  # beta; main.py:161 overwrites this attribute every step
         self.priority_exponent = args.priority_exponent
         if self.history + self.n > 64:
@@ -402,8 +405,11 @@ class ReplayMemory:
                              "(the reference has no augmentation, so there is no numpy stream to reproduce)")
         return shift_pad, intensity, (M, K)
 
-    def _launch_gather(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1)):
+    def _launch_gather(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1), horizon=None):
         tr = self.transitions
+        if horizon is not None:
+            self._launch_gather_horizon(ws, shift_pad, intensity, copies, horizon)
+            return
         common = (_lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action), _lib.ptr(tr.reward),
                   _lib.ptr(tr.nonterminal), tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, self.n,
                   _lib.ptr(self.n_step_scaling), _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions),
@@ -426,7 +432,53 @@ class ReplayMemory:
                                            _lib.ptr(self._rng_counter), _lib.ptr(ws.shifts), _lib.ptr(ws.scales),
                                            _lib.stream()))
 
-    def sample_into(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1)):
+    def _aug_buffers(self, ws, shift_pad, intensity, copies):
+        """ws.shifts / ws.scales shaped for the gather these settings select (None where it writes none)."""
+        if not shift_pad and not intensity and copies == (1, 1):
+            return None, None
+        if not intensity and copies == (1, 1):
+            if ws.shifts is None or ws.shifts.shape != (2, ws.B, 2):
+                ws.shifts = torch.empty((2, ws.B, 2), dtype=torch.int32, device=self.device)
+            return ws.shifts, None
+        c = max(copies)
+        if ws.shifts is None or ws.shifts.shape != (2, c, ws.B, 2):
+            ws.shifts = torch.empty((2, c, ws.B, 2), dtype=torch.int32, device=self.device)
+        if ws.scales is None or ws.scales.shape != (2, c, ws.B):
+            ws.scales = torch.empty((2, c, ws.B), dtype=torch.float32, device=self.device)
+        return ws.shifts, ws.scales
+
+    def _check_horizon(self, horizon):
+        if horizon is not None and horizon.n_max > self.n:
+            raise ValueError(f"the horizon reaches n = {horizon.n_max}, this replay was built for n = {self.n} "
+                             "(set args.multi_step_start before building it)")
+
+    def _launch_gather_horizon(self, ws, shift_pad, intensity, copies, horizon):
+        tr = self.transitions
+        shifts, scales = self._aug_buffers(ws, shift_pad, intensity, copies)
+        _lib.check(self._lib.rb_gather_horizon(
+            _lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action), _lib.ptr(tr.reward), _lib.ptr(tr.nonterminal),
+            tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, horizon.n_max, _lib.ptr(horizon.current),
+            _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions), _lib.ptr(ws.returns),
+            _lib.ptr(ws.nonterminals), shift_pad, intensity, copies[0], copies[1], self.seed, _lib.ptr(self._rng_counter),
+            _lib.ptr(shifts), _lib.ptr(scales), _lib.stream()))
+
+    def _sample_horizon(self, ws, shift_pad, intensity, copies, horizon):
+        """rb_horizon_advance on a side branch beside rb_tree_sample (which does not read the horizon), joined before the
+        gather through the horizon's current row."""
+        main = torch.cuda.current_stream(self.device)
+        side = horizon.side_stream()
+        fork = torch.cuda.Event()
+        fork.record(main)
+        with torch.cuda.stream(side):
+            side.wait_event(fork)
+            horizon.advance()
+            done = torch.cuda.Event()
+            done.record(side)
+        self._launch_sample(ws)
+        main.wait_event(done)
+        self._launch_gather_horizon(ws, shift_pad, intensity, copies, horizon)
+
+    def sample_into(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1), horizon=None):
         """Device-RNG sample into caller-owned buffers: two launches, no synchronisation (graph capturable).
         The caller is responsible for push_beta() and flush_appends() (outside any graph capture).
         shift_pad = p > 0 (at most MAX_SHIFT_PAD) augments the states and next states by random shifts (DrQ): each
@@ -434,21 +486,30 @@ class ReplayMemory:
         (rb_gather_shift); `ws.shifts` receives the offsets.  0 gathers exactly as the reference does.
         intensity = s > 0 (at most MAX_INTENSITY) multiplies every observation by 1 + s * clip(N(0, 1), -2, 2) (SPR), and
         copies = (M, K) writes M augmented copies of every state and K of every next state (DrQ's K / M): both go through
-        rb_gather_aug, whose draws land in `ws.shifts` and `ws.scales`.  `ws` must have been made for these copies."""
+        rb_gather_aug, whose draws land in `ws.shifts` and `ws.scales`.  `ws` must have been made for these copies.
+        horizon = s (a rainbow_b200.horizon.HorizonSchedule): one step of the annealed horizon.  rb_horizon_advance runs on
+        a side branch beside the sampling, and rb_gather_horizon gathers with that step's n and gamma: the returns and next
+        states of n_u steps, and the nonterminals in discount form fl32(nonterminal * gamma_u ** n_u), for a loss launched
+        with gamma_n = 1.  The sampling itself uses this replay's n (at least s.n_max).  None gathers as before."""
         shift_pad, intensity, copies = self._check_augmentation(shift_pad, intensity, copies)
         if ws.copies != copies:
             raise ValueError(f"the workspace holds copies {ws.copies}, the call asks for {copies}")
-        self._launch_sample(ws)
-        self._launch_gather(ws, shift_pad, intensity, copies)
+        self._check_horizon(horizon)
+        if horizon is None:
+            self._launch_sample(ws)
+            self._launch_gather(ws, shift_pad, intensity, copies)
+        else:
+            self._sample_horizon(ws, shift_pad, intensity, copies, horizon)
         self._last = ws
         return ws.as_tuple()
 
-    def sample(self, batch_size, shift_pad=0, intensity=0.0, copies=(1, 1)):
+    def sample(self, batch_size, shift_pad=0, intensity=0.0, copies=(1, 1), horizon=None):
         """memory.py:148-155.  Returns (tree_idxs, states, actions, returns, next_states, nonterminals, weights),
         all device tensors (the reference returns tree_idxs as numpy; update_priorities takes either).
         shift_pad, intensity, copies: augmentation as in sample_into(); needs rng="philox" (ValueError otherwise).  With
-        copies = (M, K) the states are [M B, ...] and the next states [K B, ...], copy-major."""
+        copies = (M, K) the states are [M B, ...] and the next states [K B, ...], copy-major.  horizon: as in sample_into()."""
         shift_pad, intensity, copies = self._check_augmentation(shift_pad, intensity, copies)
+        self._check_horizon(horizon)
         ws = _SampleWorkspace(int(batch_size), self.history, self.device, copies)
         self.flush_appends()
         self.push_beta()
@@ -461,10 +522,12 @@ class ReplayMemory:
                     break
             else:  # pragma: no cover
                 raise _lib.RainbowB200Error("no valid batch after 100000 draws")
-            self._launch_gather(ws)
+            if horizon is not None:
+                horizon.advance()
+            self._launch_gather(ws, horizon=horizon)
             self._last = ws
             return ws.as_tuple()
-        out = self.sample_into(ws, shift_pad, intensity, copies)
+        out = self.sample_into(ws, shift_pad, intensity, copies, horizon)
         if self.strict:
             self.check_last_sample()
         return out
