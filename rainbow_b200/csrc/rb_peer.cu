@@ -15,7 +15,7 @@
 // ld.acquire.sys); nothing spins on the host.  All buffers handed in as `peer_*[rank]` pointers must be mapped on
 // every GPU (torch symmetric memory in rainbow_b200/peer.py).
 //
-// tools/peer_adam_check.py compares it against NCCL all-reduce + rb_clip_adam on a multi-GPU node.
+// tests/test_gpu_peer_f64.py checks every stage against a float64 reference, W = 1..8 ranks emulated on one GPU.
 
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -10,9 +10,10 @@ Per update (csrc/rb_peer.cu)
 cross-GPU ordering is epoch flags in the same symmetric allocation, never the host.  Replaces
 `all_reduce(flat_grad); rb_clip_adam` (replicated 192 MB optimiser pass on every rank).
 
-tools/peer_adam_check.py compares it against the NCCL path on a multi-GPU node (parameters after several steps, ranks
-bit-identical).  `args.peer_optimizer`: True | "auto" (falls back to the NCCL all-reduce when symmetric memory cannot be set
-up; bench.py's default for world > 1) | False.
+tests/test_gpu_peer_f64.py checks every stage against a float64 reference with W = 1, 2, 4 and 8 ranks emulated on one
+GPU, and this class over real symmetric memory on a host with 2+ GPUs; tools/peer_adam_check.py compares it against the
+NCCL path on a multi-GPU node.  `args.peer_optimizer`: True | "auto" (falls back to the NCCL all-reduce when symmetric
+memory cannot be set up; bench.py's default for world > 1) | False.
 """
 import ctypes as C
 
