@@ -388,6 +388,31 @@ int rb_clip_adam(float* param, const float* grad, float* exp_avg, float* exp_avg
                  float max_norm, float lr, float beta1, float beta2, float eps, int64_t* step_count,
                  double* partial_sums, float* norm_out, const int32_t* gate, rb_stream_t stream);
 
+/* rb_clip_adam with decoupled weight decay (AdamW, torch.optim.AdamW) and Adam state per parameter GROUP.  The groups
+ * tile [0, P) in order; group g has weight decay lambda_g and its own bias-correction count group_steps[g] (device
+ * int64[n_groups], steps already taken by that group).  The norm, clip coefficient and grad_scale are rb_clip_adam's (one
+ * global norm, decay not part of it).  For an element of group g, with t_g = group_steps[g] + 1:
+ *   p = p * fl32(1 - lr lambda_g)           (rounded on its own; torch's param.mul_(1 - lr wd) before the moments)
+ *   then rb_clip_adam's Adam step with the bias corrections of t_g.
+ * The call advances *step_count (applied steps, as rb_clip_adam) and every group_steps[g].  A gate reading 0 writes only
+ * norm_out.  With every lambda_g = 0 and every group_steps[g] == *step_count the result is rb_clip_adam's, bitwise.
+ * A restart of group g's Adam state is the caller zeroing its moment range and group_steps[g].
+ * groups: HOST array of n_groups entries, copied into the launch.  partial_sums as for rb_clip_adam.  Profiled under
+ * RB_K_SQNORM and RB_K_CLIP_ADAM.
+ * RB_ERR_INVAL: a NULL pointer (norm_out and gate may be NULL) or P <= 0; RB_ERR_RANGE: n_groups outside
+ * [1, RB_MAX_ADAM_GROUPS], groups that do not tile [0, P) (a gap, an overlap, unsorted, empty, or a last end other than
+ * P), a begin that is not a multiple of 4, lambda negative or not finite, fl32(lr) fl32(lambda) >= 1.  A refused call
+ * launches nothing. */
+#define RB_MAX_ADAM_GROUPS 4
+typedef struct rb_adam_group {
+  int64_t begin, end;      /* flat elements [begin, end) */
+  float weight_decay;      /* lambda >= 0 */
+} rb_adam_group;
+int rb_clip_adamw(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t P, float grad_scale,
+                  float max_norm, float lr, float beta1, float beta2, float eps, const rb_adam_group* groups, int n_groups,
+                  int64_t* step_count, int64_t* group_steps, double* partial_sums, float* norm_out, const int32_t* gate,
+                  rb_stream_t stream);
+
 /* Polyak (soft) target update over FLAT float32 buffers of n elements (no reference counterpart; the reference only copies
  * the online net into the target, agent.py:102-103).  For every i < n:
  *   target[i] = fmaf(tau, param[i], fl32(1 - tau) * target[i])
@@ -442,6 +467,17 @@ int rb_peer_adam_gather(float* const* peer_param, uint64_t* const* peer_flags, d
                         int n_seg, const int64_t* seg_begin, const int64_t* seg_len, const float* gred, float* exp_avg,
                         float* exp_avg_sq, float max_norm, float lr, float beta1, float beta2, float eps, int64_t* step_count,
                         uint64_t* epoch, void* scratch, float* norm_out, float* multicast_param, rb_stream_t stream);
+/* rb_peer_adam_gather with rb_clip_adamw's decoupled weight decay and Adam state per SEGMENT: seg_weight_decay (HOST
+ * float[n_seg]) and seg_steps (device int64[n_seg], each segment's bias-correction count, advanced with step_count).  The
+ * segments are the groups; the moment shards of a segment restart when the caller zeroes them and its count.  Refused
+ * as rb_peer_adam_gather, and also for a NULL seg_weight_decay / seg_steps (RB_ERR_INVAL) or a lambda negative, not
+ * finite or with fl32(lr) fl32(lambda) >= 1 (RB_ERR_RANGE).  With every lambda = 0 and every seg_steps[s] == *step_count
+ * the result is rb_peer_adam_gather's, bitwise. */
+int rb_peer_adamw_gather(float* const* peer_param, uint64_t* const* peer_flags, double* const* peer_norms, int world, int rank,
+                         int n_seg, const int64_t* seg_begin, const int64_t* seg_len, const float* seg_weight_decay,
+                         const float* gred, float* exp_avg, float* exp_avg_sq, float max_norm, float lr, float beta1,
+                         float beta2, float eps, int64_t* step_count, int64_t* seg_steps, uint64_t* epoch, void* scratch,
+                         float* norm_out, float* multicast_param, rb_stream_t stream);
 int rb_peer_clip_adam(const float* const* peer_grad, float* const* peer_param, uint64_t* const* peer_flags,
                       double* const* peer_norms, int world, int rank, int64_t P, float* gred, float* exp_avg,
                       float* exp_avg_sq, float grad_scale, float max_norm, float lr, float beta1, float beta2, float eps,

@@ -30,6 +30,14 @@ class ResetSegment(C.Structure):
                 ("alpha", C.c_float)]
 
 
+class AdamGroup(C.Structure):
+    """rb_adam_group: one parameter group of rb_clip_adamw, flat elements [begin, end) with weight decay lambda."""
+    _fields_ = [("begin", C.c_int64), ("end", C.c_int64), ("weight_decay", C.c_float)]
+
+
+MAX_ADAM_GROUPS = 4   # RB_MAX_ADAM_GROUPS
+
+
 class Horizon(C.Structure):
     """rb_horizon: one row of an annealed-horizon table (n, gamma ** n, gamma ** k for k < n then zeros)."""
     _fields_ = [("n", C.c_int32), ("gamma_n", C.c_float), ("gamma_pow", C.c_float * 64)]
@@ -82,10 +90,14 @@ SIGNATURES = {
     "rb_peer_reduce": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i64, _i64, _f32, _vp, _vp, _vp, _vp]),
     "rb_peer_adam_gather": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32,
                                       _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rb_peer_adamw_gather": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32,
+                                       _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rb_peer_clip_adam": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32, _f32,
                                     _vp, _vp, _vp, _vp, _vp]),
     "rb_clip_adam_scratch_elems": (C.c_int, []),
     "rb_clip_adam": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
+    "rb_clip_adamw": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _f32, C.POINTER(AdamGroup), _i32,
+                                _vp, _vp, _vp, _vp, _vp, _vp]),
     "rb_target_ema": (C.c_int, [_vp, _vp, _i64, _f32, _vp, _vp]),
     "rb_param_reset": (C.c_int, [_vp, _i64, C.POINTER(ResetSegment), _i32, _u64, _u64, _vp]),
     "rb_q_values": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),

@@ -20,6 +20,8 @@ One `learn(mem)` (agent.py:61-100) is:
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
+                                              [args.weight_decay > 0 or args.reset_optimizer: rb_clip_adamw -- AdamW's
+                                               decoupled decay, Adam state per group (encoder, head) that resets restart]
     [args.target_tau = tau > 0: rb_target_ema -- Polyak target update t <- tau p + (1 - tau) t, gated like K7]
     K4 rb_tree_update                         (agent.py:100 -> memory.py:157-159)
     [args.learn_stats = R > 0: rb_learn_stats_batch on a side stream after K3, rb_learn_stats_write after K7 -- one record
@@ -148,16 +150,39 @@ def target_reset_options(args):
     return tau, int(interval), tuple(shrink)
 
 
+def optimizer_options(args):
+    """(weight_decay, reset_optimizer) from `args`, checked: weight_decay finite and >= 0 (0 or absent = plain Adam) with
+    fl32(learning_rate) fl32(weight_decay) < 1, the condition rb_clip_adamw takes it under; reset_optimizer a bool."""
+    wd = getattr(args, "weight_decay", None)
+    wd = 0.0 if wd is None else float(wd)
+    if not (math.isfinite(wd) and wd >= 0.0):
+        raise ValueError(f"weight_decay must be finite and >= 0, got {wd}")
+    lr = float(np.float32(args.learning_rate))
+    if wd > 0.0 and not lr * float(np.float32(wd)) < 1.0:
+        raise ValueError(f"learning_rate * weight_decay must be < 1 (as fp32), got {args.learning_rate} * {wd}")
+    restart = getattr(args, "reset_optimizer", None)
+    restart = False if restart is None else restart
+    if not isinstance(restart, bool):
+        raise ValueError(f"reset_optimizer must be a bool, got {restart!r}")
+    return wd, restart
+
+
 class FusedClipAdam:
     """clip_grad_norm_ + Adam (agent.py:46,97-98) over ONE flat parameter buffer.
 
     The network's parameters are re-pointed at slices of `flat_param` (each slice starts on a 256-byte
     boundary; padding stays zero), their .grad at slices of `flat_grad`, so the optimiser step is two kernel
-    launches (sum of squares, then clip+Adam) and the multi-GPU gradient exchange is a single all-reduce."""
+    launches (sum of squares, then clip+Adam) and the multi-GPU gradient exchange is a single all-reduce.
+
+    `weight_decay` > 0 or `group_state` = True: the group optimiser (rb_clip_adamw / rb_peer_adamw_gather).  The buffer is
+    split into the groups ENCODER = [0, conv_end) and HEAD = [conv_end, numel), each with its own bias-correction count
+    (`group_steps`, device int64[2]) that restart_group() resets together with the group's moments; `weight_decay` is
+    AdamW's decoupled decay of every parameter, torch.optim.AdamW(params, weight_decay=...).  Both off: plain
+    rb_clip_adam / rb_peer_adam_gather, and no group state."""
 
     ALIGN = 64  # elements
 
-    def __init__(self, net, lr, eps, max_norm, betas=(0.9, 0.999), peer=False):
+    def __init__(self, net, lr, eps, max_norm, betas=(0.9, 0.999), peer=False, weight_decay=0.0, group_state=False):
         named = [(n, p) for n, p in net.named_parameters() if p.requires_grad]
         self.params = [p for _, p in named]
         dev = self.params[0].device
@@ -188,12 +213,45 @@ class FusedClipAdam:
         self.grad_norm = self.peer.grad_norm if self.peer is not None else torch.zeros(1, dtype=torch.float32, device=dev)
         self._lib = _lib.load()
         self._partial = torch.zeros(self._lib.rb_clip_adam_scratch_elems(), dtype=torch.float64, device=dev)
+        self.weight_decay = float(weight_decay)
+        self.grouped = self.weight_decay > 0.0 or bool(group_state)
+        if self.grouped:
+            if not 0 < self.conv_end < off:
+                raise _lib.RainbowB200Error("the group optimiser needs both an encoder and a head group")
+            self.groups = [(0, self.conv_end), (self.conv_end, off)]     # indexed by ENCODER, HEAD
+            # group_steps in the order of the groups the kernel takes: ENCODER, HEAD; or the peer segments' HEAD, ENCODER
+            self._slot = (1, 0) if self.peer is not None else (0, 1)
+            self.group_steps = torch.zeros(2, dtype=torch.int64, device=dev)
+            self._groups_c = (_lib.AdamGroup * 2)(*[_lib.AdamGroup(b, e, self.weight_decay) for b, e in self.groups])
         with torch.no_grad():
             for p, o in zip(self.params, self.offsets):
                 n = p.numel()
                 self.flat_param[o:o + n].copy_(p.reshape(-1))
                 p.data = self.flat_param[o:o + n].view_as(p)
                 p.grad = self.flat_grad[o:o + n].view_as(p)
+
+    def group_step_counts(self):
+        """[ENCODER count, HEAD count] of the group optimiser (one device read)."""
+        steps = self.group_steps.tolist()
+        return [steps[self._slot[0]], steps[self._slot[1]]]
+
+    def set_group_step_counts(self, counts):
+        for g, c in enumerate(counts):
+            self.group_steps[self._slot[g]].fill_(int(c))
+
+    def restart_group(self, g):
+        """Restart Adam for group g (ENCODER or HEAD): its exp_avg / exp_avg_sq range -- under the peer optimiser this rank's
+        shard of the group's segment -- zeroed and its bias-correction count set to 0, so the next step is a first step
+        for it.  Plain fills on the current stream, in place (captured update graphs stay valid)."""
+        if not self.grouped:
+            raise _lib.RainbowB200Error("restarting a group's Adam state needs the group optimiser")
+        if self.peer is not None:
+            rng = self.peer.shard_slices()[self._slot[g]][1]
+        else:
+            rng = slice(*self.groups[g])
+        self.exp_avg[rng].zero_()
+        self.exp_avg_sq[rng].zero_()
+        self.group_steps[self._slot[g]].zero_()
 
     def zero_grad(self):
         self.flat_grad.zero_()
@@ -207,7 +265,18 @@ class FusedClipAdam:
         the device (single-GPU only: data-parallel ranks must step in lock step, there a rejected batch simply contributes
         a zero gradient through its zeroed importance weights)."""
         if self.peer is not None:   # reduce-scatter + clip + Adam + all-gather over peer memory (1/world folded in)
-            self.peer.step(self.max_norm, self.lr, self.betas, self.eps)
+            if self.grouped:
+                self.peer.step(self.max_norm, self.lr, self.betas, self.eps, weight_decay=self.weight_decay,
+                               seg_steps=self.group_steps)
+            else:
+                self.peer.step(self.max_norm, self.lr, self.betas, self.eps)
+            return
+        if self.grouped:
+            _lib.check(self._lib.rb_clip_adamw(
+                _lib.ptr(self.flat_param), _lib.ptr(self.flat_grad), _lib.ptr(self.exp_avg), _lib.ptr(self.exp_avg_sq),
+                self.numel, float(grad_scale), self.max_norm, self.lr, self.betas[0], self.betas[1], self.eps,
+                self._groups_c, 2, _lib.ptr(self.step_count), _lib.ptr(self.group_steps), _lib.ptr(self._partial),
+                _lib.ptr(self.grad_norm), _lib.ptr(gate), _lib.stream()))
             return
         _lib.check(self._lib.rb_clip_adam(
             _lib.ptr(self.flat_param), _lib.ptr(self.flat_grad), _lib.ptr(self.exp_avg), _lib.ptr(self.exp_avg_sq),
@@ -274,6 +343,10 @@ class Agent:
         # Polyak target updates (tau > 0: every applied optimiser step also moves the target, DrQ(eps) / SPR / BBF) and
         # periodic shrink-and-perturb resets of the online net (SR-SPR, BBF); both off by default
         self.target_tau, self.reset_interval, self.reset_shrink = target_reset_options(args)
+        # AdamW's decoupled weight decay (BBF: 0.1) and the restart of a group's Adam state when a reset moves it; either
+        # turns on the group optimiser (FusedClipAdam, rb_clip_adamw); both off by default
+        self.weight_decay, self.reset_optimizer = optimizer_options(args)
+        opt_kw = dict(weight_decay=self.weight_decay, group_state=self.reset_optimizer)
         # BBF's annealed update horizon: n and gamma move from (multi_step_start, discount_start) to (multi_step, discount)
         # over anneal_steps updates after the Agent is built and after every reset; None when args.anneal_steps is 0
         self._horizon = HorizonSchedule.from_args(args, self.device)
@@ -311,7 +384,7 @@ class Agent:
             err = None
             try:
                 self.optimiser = FusedClipAdam(self.online_net, lr=args.learning_rate, eps=args.adam_eps, max_norm=self.norm_clip,
-                                               peer=True)
+                                               peer=True, **opt_kw)
             except Exception as e:   # noqa: BLE001 -- whatever went wrong, all ranks must take the same path
                 err = e
             ok = torch.tensor([0 if err is not None else 1], dtype=torch.int32, device=self.device)
@@ -323,7 +396,7 @@ class Agent:
                 self.peer_optimizer, self.optimiser = False, None
         if self.optimiser is None:
             self.optimiser = FusedClipAdam(self.online_net, lr=args.learning_rate, eps=args.adam_eps, max_norm=self.norm_clip,
-                                           peer=False)
+                                           peer=False, **opt_kw)
         self.sync.broadcast_(self.optimiser.flat_param)  # identical initial parameters on every rank
         if self.peer_optimizer:
             self.sync.exchange = False   # the optimiser step does the gradient exchange itself
@@ -708,25 +781,36 @@ class Agent:
                                                  self.optimiser.numel, self.target_tau, _lib.ptr(self._step_gate),
                                                  _lib.stream()))
 
-    def reset_parameters(self, shrink_encoder=1.0, shrink_head=0.0):
+    def reset_parameters(self, shrink_encoder=1.0, shrink_head=0.0, restart_optimizer=None):
         """Shrink-and-perturb the online net toward a fresh initialisation theta0 (Ash & Adams 2020; Nikishin et al. 2022;
         SR-SPR and BBF): theta <- fma(alpha, theta, fl32(1 - alpha) theta0), alpha = shrink_encoder for the conv layers and
         shrink_head for the four noisy layers.  The defaults re-initialise the head and keep the encoder.  theta0 follows
         the network's own initialisation (reset_table), drawn by rb_param_reset from the reset seed with the index of this
         reset as counter: every rank draws the same theta0 and a resumed run repeats the draws.  One launch on the current
-        stream, in place (captured graphs stay valid); the padding of the flat buffer, the Adam moments and step count,
-        the target net, the noise and the replay are untouched (the single flat step count cannot restart Adam's bias
-        correction for a part of the buffer, so the optimiser state is kept as it is).  An annealed horizon restarts at its
-        first step (n0, gamma0)."""
+        stream, in place (captured graphs stay valid); the padding of the flat buffer, the target net, the noise and the
+        replay are untouched.
+        `restart_optimizer` (None: args.reset_optimizer): every group the reset moves (alpha < 1) restarts Adam -- its
+        exp_avg / exp_avg_sq range zeroed and its bias-correction count set to 0, so the re-drawn weights take first
+        steps of their own (FusedClipAdam.restart_group); a group with alpha = 1 keeps its state bitwise.  It needs the
+        group optimiser (args.reset_optimizer or args.weight_decay > 0).  Without a restart the Adam moments and counts
+        are kept as they are.  An annealed horizon restarts at its first step (n0, gamma0)."""
         alphas = (float(shrink_encoder), float(shrink_head))
         if not all(0.0 <= a <= 1.0 for a in alphas):
             raise ValueError(f"shrink_encoder and shrink_head must be in [0, 1], got {alphas}")
+        restart = self.reset_optimizer if restart_optimizer is None else bool(restart_optimizer)
+        if restart and not self.optimiser.grouped:
+            raise _lib.RainbowB200Error("restart_optimizer needs the group optimiser: build the Agent with "
+                                        "args.reset_optimizer = True or args.weight_decay > 0")
         if self._reset_base is None:
             self._reset_base = reset_table(self.online_net, self.optimiser.offsets)
         segs = (_lib.ResetSegment * len(self._reset_base))(
             *[_lib.ResetSegment(off, n, b, c, alphas[g]) for off, n, b, c, g in self._reset_base])
         _lib.check(_lib.load().rb_param_reset(_lib.ptr(self.optimiser.flat_param), self.optimiser.numel, segs, len(segs),
                                               self.reset_seed, self.reset_count, _lib.stream()))
+        if restart:
+            for g in (ENCODER, HEAD):
+                if alphas[g] < 1.0:
+                    self.optimiser.restart_group(g)
         self.reset_count += 1
         if self._horizon is not None:
             self._horizon.restart()

@@ -365,6 +365,12 @@ def _meta(agent, mem):
         hyper["reset_shrink_encoder"] = agent.reset_shrink[0]
     if agent.reset_shrink[1] != 0.0:
         hyper["reset_shrink_head"] = agent.reset_shrink[1]
+    if agent.weight_decay:
+        hyper["weight_decay"] = agent.weight_decay
+    if agent.reset_optimizer:
+        hyper["reset_optimizer"] = True
+    if opt.grouped:   # the group optimiser's bias-correction counts, [encoder, head]
+        learner["optimiser_group_steps"] = opt.group_step_counts()
     hz = agent._horizon
     if hz is not None:   # the annealed horizon's options (when not their defaults) and the cycle step of the next update
         hyper["anneal_steps"] = hz.T
@@ -470,6 +476,18 @@ def check_reset_scalars(learner):
         raise _Error("manifest learner.reset_seed and learner.reset_count must be given together (or both be absent)")
 
 
+def check_group_steps(learner):
+    """learner.optimiser_group_steps, when present: [encoder, head], two ints in [0, optimiser_step] (a group's count
+    restarts at a reset and never passes the applied steps).  Absent: a manifest of a run without the group optimiser,
+    which loads with both counts equal to optimiser_step."""
+    v = learner.get("optimiser_group_steps")
+    if v is None:
+        return
+    step = learner.get("optimiser_step")
+    if not (isinstance(v, list) and len(v) == 2 and _is_int(step, 0, _U63) and all(_is_int(c, 0, step + 1) for c in v)):
+        raise _Error(f"manifest learner.optimiser_group_steps = {v!r} must be two ints in [0, optimiser_step = {step!r}]")
+
+
 def _validate(agent, mem, man):
     """Every check of load(), none of which writes anything; returns the expected {array name: (dtype, shape)}."""
     world, rank = agent.sync.world_size, agent.sync.rank
@@ -494,6 +512,7 @@ def _validate(agent, mem, man):
         if not ok(v, mem):
             raise _Error(f"manifest {section}.{key} = {v!r} is missing or out of range")
     check_reset_scalars(man["learner"])
+    check_group_steps(man["learner"])
     cap = man["learner"]["learn_stats_capacity"]
     expected = {n: _spec(t) for n, t in _learner_arrays(agent).items() if n != "learn_stats.ring"}
     if cap:
@@ -561,6 +580,8 @@ def _restore(agent, mem, d, staging):
 
     on, tg, opt = agent.online_net, agent.target_net, agent.optimiser
     opt.step_count.fill_(learner["optimiser_step"])
+    if opt.grouped:
+        opt.set_group_step_counts(learner.get("optimiser_group_steps") or [learner["optimiser_step"]] * 2)
     on.noise_seed, tg.noise_seed = learner["online_noise_seed"], learner["target_noise_seed"]
     on._noise_pending, tg._noise_pending = learner["online_noise_pending"], False
     # the saved epsilon buffers come with their stale flag: the library head reads them without launching a pending draw

@@ -30,6 +30,14 @@ inline int check_launch(const char* what) {
   return RB_OK;
 }
 
+// ---- AdamW's decoupled weight decay (rb_clip_adamw, rb_peer_adamw_gather) ---------------------
+// lambda finite and >= 0, fl32(lr) fl32(lambda) < 1: the factor fl32(1 - lr lambda) the kernels multiply p by is in (0, 1]
+inline int adamw_decay_check(float lr, float weight_decay, const char* who) {
+  if (!(weight_decay >= 0.0f && weight_decay <= 3.402823466e38f) || !((double)lr * (double)weight_decay < 1.0))
+    return fail(RB_ERR_RANGE, who);
+  return RB_OK;
+}
+
 // ---- opt-in to more than 48 KB of dynamic shared memory, once per (device, kernel, size) ---------------
 // cudaFuncSetAttribute is not a stream operation; calling it again and again (e.g. while a CUDA graph is being
 // captured) is avoided by remembering the largest size already granted per device.

@@ -1891,14 +1891,42 @@ __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, 
   p = fmaf(-step_size * m, fast_rcp(denom), p);  // param.addcdiv_(exp_avg, denom, value=-step_size)
 }
 
-__global__ void __launch_bounds__(ADAM_THREADS)
-k_clip_adam(float* __restrict__ param, const float* __restrict__ grad, float* __restrict__ exp_avg,
-            float* __restrict__ exp_avg_sq, int64_t P, float grad_scale, float max_norm, float lr, float b1, float b2,
-            float eps, int64_t* __restrict__ step_count, const double* __restrict__ partial, int n_partial,
-            float* __restrict__ norm_out, unsigned int* __restrict__ done_ticket, const int32_t* __restrict__ gate) {
+// rb_clip_adamw's group table, by value: groups tile [0, P) in order, each begins on a multiple of 4
+struct AdamGroupPlan {
+  rb_adam_group g[RB_MAX_ADAM_GROUPS];
+  int n;
+};
+
+// rb_clip_adamw: the body below takes one step size, 1 / sqrt(bc2) and count from step_count when GROUPS is false, and per
+// group g -- bias corrections from group_steps[g] + 1, decay factor d_g = fl32(1 - lr lambda_g) applied as p = p * d_g
+// (rounded on its own, never contracted) before adam_one -- when it is true.  The factors are formed once per CTA into
+// shared memory; a float4 finds its group with three compares against the later groups' begins (a begin is a multiple of 4,
+// so no float4 straddles two groups).  d_g = 1 for lambda_g = 0 leaves p bitwise as it is.
+template <bool GROUPS>
+__device__ __forceinline__ void
+clip_adam_body(float* __restrict__ param, const float* __restrict__ grad, float* __restrict__ exp_avg,
+               float* __restrict__ exp_avg_sq, int64_t P, float grad_scale, float max_norm, float lr, float b1, float b2,
+               float eps, int64_t* __restrict__ step_count, const double* __restrict__ partial, int n_partial,
+               float* __restrict__ norm_out, unsigned int* __restrict__ done_ticket, const int32_t* __restrict__ gate,
+               const AdamGroupPlan* plan, int64_t* __restrict__ group_steps) {
   const bool skip = gate && *gate == 0;   // rejected sample batch: no parameter update, no step (see k_tree_sample)
   __shared__ double s_red[ADAM_THREADS / 32];
   __shared__ float s_coef;
+  __shared__ float s_step_size[GROUPS ? RB_MAX_ADAM_GROUPS : 1], s_bc2_sqrt[GROUPS ? RB_MAX_ADAM_GROUPS : 1],
+      s_decay[GROUPS ? RB_MAX_ADAM_GROUPS : 1];
+  __shared__ int64_t s_t[GROUPS ? RB_MAX_ADAM_GROUPS : 1];
+  if constexpr (GROUPS) {
+    if (threadIdx.x < plan->n) {
+      const int k = threadIdx.x;
+      const int64_t t = group_steps[k] + 1;
+      const double bc1 = 1.0 - pow((double)b1, (double)t);
+      const double bc2 = 1.0 - pow((double)b2, (double)t);
+      s_step_size[k] = (float)((double)lr / bc1);
+      s_bc2_sqrt[k] = (float)(1.0 / sqrt(bc2));
+      s_decay[k] = (float)(1.0 - (double)lr * (double)plan->g[k].weight_decay);
+      s_t[k] = t;
+    }
+  }
   // every CTA re-reduces the (few hundred) partial sums in the same order: deterministic, no atomics
   double acc = 0.0;
   for (int i = threadIdx.x; i < n_partial; i += ADAM_THREADS) acc += partial[i];
@@ -1917,10 +1945,18 @@ k_clip_adam(float* __restrict__ param, const float* __restrict__ grad, float* __
   __syncthreads();
   const float coef = s_coef;
   const int64_t step = *step_count + 1;
-  const double bc1 = 1.0 - pow((double)b1, (double)step);
-  const double bc2 = 1.0 - pow((double)b2, (double)step);
-  const float step_size = (float)((double)lr / bc1);
-  const float bc2_sqrt = (float)(1.0 / sqrt(bc2));  // passed to adam_one as the reciprocal
+  float step_size, bc2_sqrt;  // bc2_sqrt is passed to adam_one as the reciprocal
+  int64_t lim1 = INT64_MAX, lim2 = INT64_MAX, lim3 = INT64_MAX;   // begins of groups 1..3 (none: never reached)
+  if constexpr (GROUPS) {
+    if (plan->n > 1) lim1 = plan->g[1].begin;
+    if (plan->n > 2) lim2 = plan->g[2].begin;
+    if (plan->n > 3) lim3 = plan->g[3].begin;
+  } else {
+    const double bc1 = 1.0 - pow((double)b1, (double)step);
+    const double bc2 = 1.0 - pow((double)b2, (double)step);
+    step_size = (float)((double)lr / bc1);
+    bc2_sqrt = (float)(1.0 / sqrt(bc2));
+  }
 
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1930,6 +1966,14 @@ k_clip_adam(float* __restrict__ param, const float* __restrict__ grad, float* __
     for (; i < (P >> 2); i += stride) {
       float4 p = reinterpret_cast<float4*>(param)[i], g = __ldg(reinterpret_cast<const float4*>(grad) + i),
              m = reinterpret_cast<float4*>(exp_avg)[i], v = reinterpret_cast<float4*>(exp_avg_sq)[i];
+      if constexpr (GROUPS) {
+        const int64_t e = i << 2;
+        const int k = (e >= lim1) + (e >= lim2) + (e >= lim3);
+        step_size = s_step_size[k];
+        bc2_sqrt = s_bc2_sqrt[k];
+        const float d = s_decay[k];
+        p.x = __fmul_rn(p.x, d); p.y = __fmul_rn(p.y, d); p.z = __fmul_rn(p.z, d); p.w = __fmul_rn(p.w, d);
+      }
       adam_one(p.x, g.x, m.x, v.x, coef, b1, b2, step_size, bc2_sqrt, eps);
       adam_one(p.y, g.y, m.y, v.y, coef, b1, b2, step_size, bc2_sqrt, eps);
       adam_one(p.z, g.z, m.z, v.z, coef, b1, b2, step_size, bc2_sqrt, eps);
@@ -1941,23 +1985,53 @@ k_clip_adam(float* __restrict__ param, const float* __restrict__ grad, float* __
   } else {
     for (; i < P; i += stride) {
       float p = param[i], m = exp_avg[i], v = exp_avg_sq[i];
+      if constexpr (GROUPS) {
+        const int k = (i >= lim1) + (i >= lim2) + (i >= lim3);
+        step_size = s_step_size[k];
+        bc2_sqrt = s_bc2_sqrt[k];
+        p = __fmul_rn(p, s_decay[k]);
+      }
       adam_one(p, grad[i], m, v, coef, b1, b2, step_size, bc2_sqrt, eps);
       param[i] = p;
       exp_avg[i] = m;
       exp_avg_sq[i] = v;
     }
   }
-  // every CTA has read *step_count above; the last one to get here advances it (self-resetting ticket), which saves a
-  // dependent 1-thread launch on the critical path
+  // every CTA has read *step_count (and the group counts) above; the last one to get here advances them (self-resetting
+  // ticket), which saves a dependent 1-thread launch on the critical path
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();
     const unsigned int t = atomicAdd(done_ticket, 1u);
     if (t == gridDim.x - 1) {
       *done_ticket = 0u;
-      if (!skip) *step_count = step;
+      if (!skip) {
+        *step_count = step;
+        if constexpr (GROUPS) {
+          for (int k = 0; k < plan->n; ++k) group_steps[k] = s_t[k];
+        }
+      }
     }
   }
+}
+
+__global__ void __launch_bounds__(ADAM_THREADS)
+k_clip_adam(float* __restrict__ param, const float* __restrict__ grad, float* __restrict__ exp_avg,
+            float* __restrict__ exp_avg_sq, int64_t P, float grad_scale, float max_norm, float lr, float b1, float b2,
+            float eps, int64_t* __restrict__ step_count, const double* __restrict__ partial, int n_partial,
+            float* __restrict__ norm_out, unsigned int* __restrict__ done_ticket, const int32_t* __restrict__ gate) {
+  clip_adam_body<false>(param, grad, exp_avg, exp_avg_sq, P, grad_scale, max_norm, lr, b1, b2, eps, step_count, partial,
+                        n_partial, norm_out, done_ticket, gate, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(ADAM_THREADS)
+k_clip_adamw(float* __restrict__ param, const float* __restrict__ grad, float* __restrict__ exp_avg,
+             float* __restrict__ exp_avg_sq, int64_t P, float grad_scale, float max_norm, float lr, float b1, float b2,
+             float eps, int64_t* __restrict__ step_count, const double* __restrict__ partial, int n_partial,
+             float* __restrict__ norm_out, unsigned int* __restrict__ done_ticket, const int32_t* __restrict__ gate,
+             const __grid_constant__ AdamGroupPlan plan, int64_t* __restrict__ group_steps) {
+  clip_adam_body<true>(param, grad, exp_avg, exp_avg_sq, P, grad_scale, max_norm, lr, b1, b2, eps, step_count, partial,
+                       n_partial, norm_out, done_ticket, gate, &plan, group_steps);
 }
 
 int adam_ctas(int64_t P) {
@@ -2549,6 +2623,44 @@ int rb_clip_adam(float* param, const float* grad, float* exp_avg, float* exp_avg
                                                                beta1, beta2, eps, step_count, partial_sums, ctas, norm_out,
                                                                reinterpret_cast<unsigned int*>(partial_sums + ADAM_MAX_CTAS), gate); }
   return check_launch("rb_clip_adam");
+}
+
+int rb_clip_adamw(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t P, float grad_scale,
+                  float max_norm, float lr, float beta1, float beta2, float eps, const rb_adam_group* groups, int n_groups,
+                  int64_t* step_count, int64_t* group_steps, double* partial_sums, float* norm_out, const int32_t* gate,
+                  rb_stream_t stream) {
+  if (!param || !grad || !exp_avg || !exp_avg_sq || !groups || !step_count || !group_steps || !partial_sums)
+    return fail(RB_ERR_INVAL, "rb_clip_adamw: null pointer");
+  if (P <= 0) return fail(RB_ERR_INVAL, "rb_clip_adamw: P must be positive");
+  if (n_groups < 1 || n_groups > RB_MAX_ADAM_GROUPS)
+    return fail(RB_ERR_RANGE, "rb_clip_adamw: n_groups outside [1, RB_MAX_ADAM_GROUPS]");
+  AdamGroupPlan plan;
+  memset(&plan, 0, sizeof(plan));
+  plan.n = n_groups;
+  int64_t end = 0;
+  for (int k = 0; k < n_groups; ++k) {
+    const rb_adam_group& g = groups[k];
+    if (g.begin != end || g.end <= g.begin || g.end > P)
+      return fail(RB_ERR_RANGE, "rb_clip_adamw: groups must tile [0, P) in order, each non-empty");
+    if (g.begin % 4) return fail(RB_ERR_RANGE, "rb_clip_adamw: a group must begin on a multiple of 4");
+    int rc = rbi::adamw_decay_check(lr, g.weight_decay,"rb_clip_adamw: weight_decay must be finite, >= 0 and lr * weight_decay < 1");
+    if (rc != RB_OK) return rc;
+    plan.g[k] = g;
+    end = g.end;
+  }
+  if (end != P) return fail(RB_ERR_RANGE, "rb_clip_adamw: groups must tile [0, P) in order, each non-empty");
+  const int ctas = adam_ctas(P);
+  { ProfScope prof_(RB_K_SQNORM, (cudaStream_t)stream);
+    k_sqnorm<<<ctas, ADAM_THREADS, 0, (cudaStream_t)stream>>>(grad, P, grad_scale, partial_sums); }
+  int rc = check_launch("rb_clip_adamw(norm)");
+  if (rc != RB_OK) return rc;
+  { ProfScope prof_(RB_K_CLIP_ADAM, (cudaStream_t)stream);
+    k_clip_adamw<<<ctas, ADAM_THREADS, 0, (cudaStream_t)stream>>>(param, grad, exp_avg, exp_avg_sq, P, grad_scale, max_norm,
+                                                                lr, beta1, beta2, eps, step_count, partial_sums, ctas,
+                                                                norm_out,
+                                                                reinterpret_cast<unsigned int*>(partial_sums + ADAM_MAX_CTAS),
+                                                                gate, plan, group_steps); }
+  return check_launch("rb_clip_adamw");
 }
 
 int rb_target_ema(float* target, const float* param, int64_t n, float tau, const int32_t* gate, rb_stream_t stream) {

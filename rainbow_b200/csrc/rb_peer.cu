@@ -130,12 +130,19 @@ __device__ __forceinline__ void multimem_st4(float* mc_addr, const float4& v) {
                : "memory");
 }
 
-__global__ void __launch_bounds__(PEER_THREADS)
-k_peer_adam(const __grid_constant__ PeerBufs pb, const __grid_constant__ Segs sg, uint64_t* __restrict__ epoch_ptr,
-            const float* __restrict__ gred, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
-            const double* __restrict__ seg_norm, float max_norm, float lr, float b1, float b2, float eps,
-            int64_t* __restrict__ step_count, float* __restrict__ norm_out, unsigned int* __restrict__ ticket,
-            float* __restrict__ mc_param) {
+struct SegDecay {   // rb_peer_adamw_gather: lambda of each segment
+  float wd[PEER_SEGS];
+};
+
+// GROUPS (rb_peer_adamw_gather): the bias corrections of segment s come from seg_steps[s] + 1 instead of step_count + 1,
+// and p = p * fl32(1 - lr lambda_s), rounded on its own, before the moments; the last CTA advances seg_steps too.
+template <bool GROUPS>
+__device__ __forceinline__ void
+peer_adam_body(const PeerBufs& pb, const Segs& sg, uint64_t* __restrict__ epoch_ptr, const float* __restrict__ gred,
+               float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq, const double* __restrict__ seg_norm,
+               float max_norm, float lr, float b1, float b2, float eps, int64_t* __restrict__ step_count,
+               float* __restrict__ norm_out, unsigned int* __restrict__ ticket, float* __restrict__ mc_param,
+               const SegDecay* decay, int64_t* __restrict__ seg_steps) {
   const uint64_t epoch = *epoch_ptr + 1;
   const int W = pb.world, r = pb.rank;
   if (blockIdx.x == 0 && threadIdx.x < W) {   // this rank's share of the squared norm, to every rank
@@ -153,13 +160,22 @@ k_peer_adam(const __grid_constant__ PeerBufs pb, const __grid_constant__ Segs sg
   const float coef = fminf(max_norm / (norm + 1e-6f), 1.0f);
   if (norm_out && blockIdx.x == 0 && threadIdx.x == 0) *norm_out = norm;
   const int64_t step = *step_count + 1;
-  const float step_size = (float)((double)lr / (1.0 - pow((double)b1, (double)step)));
-  const float inv_bc2_sqrt = (float)(1.0 / sqrt(1.0 - pow((double)b2, (double)step)));
+  float step_size, inv_bc2_sqrt, d = 1.0f;
+  if constexpr (!GROUPS) {
+    step_size = (float)((double)lr / (1.0 - pow((double)b1, (double)step)));
+    inv_bc2_sqrt = (float)(1.0 / sqrt(1.0 - pow((double)b2, (double)step)));
+  }
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   int64_t shard_off = 0;   // offset of the segment's part inside gred / exp_avg / exp_avg_sq
   for (int s = 0; s < sg.n; ++s) {
     const int64_t part = sg.len[s] / W, base = sg.begin[s] + (int64_t)r * part;
     const float* my_param = pb.param[r] + base;
+    if constexpr (GROUPS) {
+      const int64_t t = seg_steps[s] + 1;
+      step_size = (float)((double)lr / (1.0 - pow((double)b1, (double)t)));
+      inv_bc2_sqrt = (float)(1.0 / sqrt(1.0 - pow((double)b2, (double)t)));
+      d = (float)(1.0 - (double)lr * (double)decay->wd[s]);
+    }
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (part >> 2); i += stride) {
       float4 p = reinterpret_cast<const float4*>(my_param)[i];
       const float4 g = reinterpret_cast<const float4*>(gred + shard_off)[i];
@@ -167,6 +183,7 @@ k_peer_adam(const __grid_constant__ PeerBufs pb, const __grid_constant__ Segs sg
       float* pp = &p.x; const float* gg = &g.x; float* mm = &m.x; float* vv = &v.x;
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
+        if constexpr (GROUPS) pp[c] = __fmul_rn(pp[c], d);
         const float gc = gg[c] * coef;
         mm[c] = fmaf(gc - mm[c], 1.0f - b1, mm[c]);
         vv[c] = fmaf(vv[c], b2, (1.0f - b2) * gc * gc);
@@ -192,8 +209,31 @@ k_peer_adam(const __grid_constant__ PeerBufs pb, const __grid_constant__ Segs sg
       __threadfence_system();
       for (int q = 0; q < W; ++q) st_release_sys(pb.flags[q] + FLAG_PARAM * W + r, epoch);
       *step_count = step;
+      if constexpr (GROUPS) {
+        for (int s = 0; s < sg.n; ++s) seg_steps[s] += 1;   // every CTA read them before its ticket
+      }
     }
   }
+}
+
+__global__ void __launch_bounds__(PEER_THREADS)
+k_peer_adam(const __grid_constant__ PeerBufs pb, const __grid_constant__ Segs sg, uint64_t* __restrict__ epoch_ptr,
+            const float* __restrict__ gred, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
+            const double* __restrict__ seg_norm, float max_norm, float lr, float b1, float b2, float eps,
+            int64_t* __restrict__ step_count, float* __restrict__ norm_out, unsigned int* __restrict__ ticket,
+            float* __restrict__ mc_param) {
+  peer_adam_body<false>(pb, sg, epoch_ptr, gred, exp_avg, exp_avg_sq, seg_norm, max_norm, lr, b1, b2, eps, step_count,
+                        norm_out, ticket, mc_param, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(PEER_THREADS)
+k_peer_adamw(const __grid_constant__ PeerBufs pb, const __grid_constant__ Segs sg, uint64_t* __restrict__ epoch_ptr,
+             const float* __restrict__ gred, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
+             const double* __restrict__ seg_norm, float max_norm, float lr, float b1, float b2, float eps,
+             int64_t* __restrict__ step_count, float* __restrict__ norm_out, unsigned int* __restrict__ ticket,
+             float* __restrict__ mc_param, const __grid_constant__ SegDecay decay, int64_t* __restrict__ seg_steps) {
+  peer_adam_body<true>(pb, sg, epoch_ptr, gred, exp_avg, exp_avg_sq, seg_norm, max_norm, lr, b1, b2, eps, step_count,
+                       norm_out, ticket, mc_param, &decay, seg_steps);
 }
 
 // Phase 3: every rank's parts have arrived here (so every rank has also finished reading our gradients); advance the epoch.
@@ -262,26 +302,38 @@ int rb_peer_reduce(const float* const* peer_grad, uint64_t* const* peer_flags, i
   return rbi::check_launch("rb_peer_reduce");
 }
 
+// The checks rb_peer_adam_gather and rb_peer_adamw_gather share, and the launch parameters they derive.
+static int peer_gather_setup(PeerBufs* pb, Segs* sg, int64_t* biggest, float* const* peer_param, uint64_t* const* peer_flags,
+                             double* const* peer_norms, int world, int rank, int n_seg, const int64_t* seg_begin,
+                             const int64_t* seg_len, const float* gred, float* exp_avg, float* exp_avg_sq,
+                             int64_t* step_count, uint64_t* epoch, void* scratch) {
+  if (!peer_param || !peer_norms || !seg_begin || !seg_len || !gred || !exp_avg || !exp_avg_sq || !step_count || !epoch || !scratch)
+    return rbi::fail(RB_ERR_INVAL, "rb_peer_adam_gather: null pointer");
+  if (n_seg < 1 || n_seg > PEER_SEGS) return rbi::fail(RB_ERR_RANGE, "rb_peer_adam_gather: 1 or 2 segments");
+  int rc = fill_bufs(pb, nullptr, peer_param, peer_flags, peer_norms, world, rank, "rb_peer_adam_gather: null pointer");
+  if (rc != RB_OK) return rc;
+  sg->n = n_seg;
+  *biggest = 0;
+  for (int s = 0; s < PEER_SEGS; ++s) {
+    sg->begin[s] = s < n_seg ? seg_begin[s] : 0;
+    sg->len[s] = s < n_seg ? seg_len[s] : 0;
+    if (s < n_seg && (seg_begin[s] < 0 || seg_len[s] <= 0 || seg_len[s] % (4 * (int64_t)world) || seg_begin[s] % 4))
+      return rbi::fail(RB_ERR_INVAL, "rb_peer_adam_gather: bad segment");
+    if (sg->len[s] / world > *biggest) *biggest = sg->len[s] / world;
+  }
+  return RB_OK;
+}
+
 int rb_peer_adam_gather(float* const* peer_param, uint64_t* const* peer_flags, double* const* peer_norms, int world, int rank,
                         int n_seg, const int64_t* seg_begin, const int64_t* seg_len, const float* gred, float* exp_avg,
                         float* exp_avg_sq, float max_norm, float lr, float beta1, float beta2, float eps, int64_t* step_count,
                         uint64_t* epoch, void* scratch, float* norm_out, float* multicast_param, rb_stream_t stream) {
-  if (!peer_param || !peer_norms || !seg_begin || !seg_len || !gred || !exp_avg || !exp_avg_sq || !step_count || !epoch || !scratch)
-    return rbi::fail(RB_ERR_INVAL, "rb_peer_adam_gather: null pointer");
-  if (n_seg < 1 || n_seg > PEER_SEGS) return rbi::fail(RB_ERR_RANGE, "rb_peer_adam_gather: 1 or 2 segments");
   PeerBufs pb;
-  int rc = fill_bufs(&pb, nullptr, peer_param, peer_flags, peer_norms, world, rank, "rb_peer_adam_gather: null pointer");
-  if (rc != RB_OK) return rc;
   Segs sg;
-  sg.n = n_seg;
-  int64_t biggest = 0;
-  for (int s = 0; s < PEER_SEGS; ++s) {
-    sg.begin[s] = s < n_seg ? seg_begin[s] : 0;
-    sg.len[s] = s < n_seg ? seg_len[s] : 0;
-    if (s < n_seg && (seg_begin[s] < 0 || seg_len[s] <= 0 || seg_len[s] % (4 * (int64_t)world) || seg_begin[s] % 4))
-      return rbi::fail(RB_ERR_INVAL, "rb_peer_adam_gather: bad segment");
-    if (sg.len[s] / world > biggest) biggest = sg.len[s] / world;
-  }
+  int64_t biggest;
+  int rc = peer_gather_setup(&pb, &sg, &biggest, peer_param, peer_flags, peer_norms, world, rank, n_seg, seg_begin, seg_len,
+                             gred, exp_avg, exp_avg_sq, step_count, epoch, scratch);
+  if (rc != RB_OK) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   k_peer_adam<<<ctas_for(biggest), PEER_THREADS, 0, st>>>(pb, sg, epoch, gred, exp_avg, exp_avg_sq, scratch_seg_norm(scratch), max_norm,
                                                         lr, beta1, beta2, eps, step_count, norm_out,
@@ -290,6 +342,36 @@ int rb_peer_adam_gather(float* const* peer_param, uint64_t* const* peer_flags, d
   if (rc != RB_OK) return rc;
   k_peer_fence<<<1, 32, 0, st>>>(pb, epoch);
   return rbi::check_launch("rb_peer_adam_gather(fence)");
+}
+
+int rb_peer_adamw_gather(float* const* peer_param, uint64_t* const* peer_flags, double* const* peer_norms, int world, int rank,
+                         int n_seg, const int64_t* seg_begin, const int64_t* seg_len, const float* seg_weight_decay,
+                         const float* gred, float* exp_avg, float* exp_avg_sq, float max_norm, float lr, float beta1,
+                         float beta2, float eps, int64_t* step_count, int64_t* seg_steps, uint64_t* epoch, void* scratch,
+                         float* norm_out, float* multicast_param, rb_stream_t stream) {
+  if (!seg_weight_decay || !seg_steps) return rbi::fail(RB_ERR_INVAL, "rb_peer_adamw_gather: null pointer");
+  PeerBufs pb;
+  Segs sg;
+  int64_t biggest;
+  int rc = peer_gather_setup(&pb, &sg, &biggest, peer_param, peer_flags, peer_norms, world, rank, n_seg, seg_begin, seg_len,
+                             gred, exp_avg, exp_avg_sq, step_count, epoch, scratch);
+  if (rc != RB_OK) return rc;
+  SegDecay decay;
+  for (int s = 0; s < PEER_SEGS; ++s) {
+    decay.wd[s] = s < n_seg ? seg_weight_decay[s] : 0.0f;
+    rc = rbi::adamw_decay_check(lr, decay.wd[s],
+                                "rb_peer_adamw_gather: weight_decay must be finite, >= 0 and lr * weight_decay < 1");
+    if (rc != RB_OK) return rc;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  k_peer_adamw<<<ctas_for(biggest), PEER_THREADS, 0, st>>>(pb, sg, epoch, gred, exp_avg, exp_avg_sq, scratch_seg_norm(scratch),
+                                                         max_norm, lr, beta1, beta2, eps, step_count, norm_out,
+                                                         scratch_tickets(scratch) + PEER_SEGS, multicast_param, decay,
+                                                         seg_steps);
+  rc = rbi::check_launch("rb_peer_adamw_gather(adam)");
+  if (rc != RB_OK) return rc;
+  k_peer_fence<<<1, 32, 0, st>>>(pb, epoch);
+  return rbi::check_launch("rb_peer_adamw_gather(fence)");
 }
 
 int rb_peer_clip_adam(const float* const* peer_grad, float* const* peer_param, uint64_t* const* peer_flags,

@@ -122,13 +122,24 @@ class PeerOptimizerState:
             _lib.ptr(self.gred[off:off + self.parts[s]]), _lib.ptr(self.epoch), _lib.ptr(self._scratch), _lib.stream()))
         self._reduced[s] = True
 
-    def step(self, max_norm, lr, betas, eps):
+    def step(self, max_norm, lr, betas, eps, weight_decay=None, seg_steps=None):
+        """`seg_steps` (device int64[segments], each segment's own bias-correction count): AdamW with decoupled decay
+        `weight_decay` on every segment (rb_peer_adamw_gather); None: plain Adam (rb_peer_adam_gather)."""
         for s in range(len(self.segments)):
             if not self._reduced[s]:
                 self.reduce_segment(s)
-        _lib.check(self._lib.rb_peer_adam_gather(
-            self._peer_param, self._peer_flags, self._peer_norms, self.world, self.rank, len(self.segments), self._seg_begin,
-            self._seg_len, _lib.ptr(self.gred), _lib.ptr(self.exp_avg), _lib.ptr(self.exp_avg_sq), float(max_norm), float(lr),
-            float(betas[0]), float(betas[1]), float(eps), _lib.ptr(self.step_count), _lib.ptr(self.epoch),
-            _lib.ptr(self._scratch), _lib.ptr(self.grad_norm), self._mc_param, _lib.stream()))
+        if seg_steps is not None:
+            n = len(self.segments)
+            _lib.check(self._lib.rb_peer_adamw_gather(
+                self._peer_param, self._peer_flags, self._peer_norms, self.world, self.rank, n, self._seg_begin,
+                self._seg_len, (C.c_float * n)(*([float(weight_decay or 0.0)] * n)), _lib.ptr(self.gred),
+                _lib.ptr(self.exp_avg), _lib.ptr(self.exp_avg_sq), float(max_norm), float(lr), float(betas[0]),
+                float(betas[1]), float(eps), _lib.ptr(self.step_count), _lib.ptr(seg_steps), _lib.ptr(self.epoch),
+                _lib.ptr(self._scratch), _lib.ptr(self.grad_norm), self._mc_param, _lib.stream()))
+        else:
+            _lib.check(self._lib.rb_peer_adam_gather(
+                self._peer_param, self._peer_flags, self._peer_norms, self.world, self.rank, len(self.segments),
+                self._seg_begin, self._seg_len, _lib.ptr(self.gred), _lib.ptr(self.exp_avg), _lib.ptr(self.exp_avg_sq),
+                float(max_norm), float(lr), float(betas[0]), float(betas[1]), float(eps), _lib.ptr(self.step_count),
+                _lib.ptr(self.epoch), _lib.ptr(self._scratch), _lib.ptr(self.grad_norm), self._mc_param, _lib.stream()))
         self._reduced = [False] * len(self.segments)
