@@ -62,6 +62,9 @@ extern "C" {
 #define RB_MAX_AUG_COPIES 8      /* most copies of a state (M) or next state (K) in rb_gather_aug */
 #define RB_MAX_RESET_SEGMENTS 32 /* most parameter tensors one rb_param_reset call covers */
 #define RB_MAX_ANNEAL_STEPS 65536 /* longest horizon schedule (T) of rb_horizon_advance */
+#define RB_MAX_REDO_LAYERS 8     /* most scored layers of rb_redo_mask / rb_redo_recycle */
+#define RB_MAX_REDO_BLOCKS 4     /* most incoming, and most outgoing, parameter blocks of one scored layer */
+#define RB_REDO_RECORD_WORDS (2 + 2 * RB_MAX_REDO_LAYERS) /* int64 words of rb_redo_mask's record */
 
 /* status words written by rb_tree_sample (int32[4]): status[0] = 1 if the batch now in the output buffers passed the
  * whole-batch validity test (memory.py:131), 0 otherwise; status[1] = draws used; status[2] = number of device-RNG
@@ -439,6 +442,62 @@ typedef struct rb_reset_segment {
 } rb_reset_segment;
 int rb_param_reset(float* param, int64_t n, const rb_reset_segment* segs, int n_segs, uint64_t seed, uint64_t reset_index,
                    rb_stream_t stream);
+
+/* Dormant-neuron statistics and ReDo recycling (Sokar et al. 2023, "The Dormant Neuron Phenomenon in Deep RL"; no reference
+ * counterpart).  Nothing here synchronises or reads back: the sums, the mask and the rewrite stay on the device.
+ *
+ * rb_neuron_scores: sums[c] = sum_{r < R, p < HW} act[r][c][p] for post-ReLU activations act [R][C][HW] (a linear layer:
+ * HW = 1), one CTA per neuron: fp32 partial sums over chunks of 64 addends, added into float64, a fixed order (an eager
+ * launch and a replay agree bitwise).  |sums[c] - exact| <= 63 * 2^-24 * exact for non-negative activations.
+ * RB_ERR_INVAL: a NULL pointer, or R, C or HW <= 0. */
+int rb_neuron_scores(const float* act, int R, int C, int HW, double* sums, rb_stream_t stream);
+
+/* rb_redo_mask: one launch over every scored layer.  Layer l owns neurons [offset_l, offset_l + neurons_l) of sums and
+ * mask; its scores are s_i = sums[i] / count_l (count_l = rows * HW behind each sum, over all ranks after an all-reduce of
+ * the sums), its mean the float64 sum of the s_i in neuron order over neurons_l, and
+ *   mask[i] = s_i <= (double)tau * mean        (tau = 0: exactly-dead neurons; a layer of mean 0 is all dormant).
+ * record (device int64[RB_REDO_RECORD_WORDS]): {pass_index, n_layers, then (neurons_l, dormant_l) per layer}.
+ * layers: HOST array, sorted by offset and non-overlapping, copied into the launch.
+ * RB_ERR_INVAL: a NULL pointer; RB_ERR_RANGE: n_layers outside [1, RB_MAX_REDO_LAYERS], tau outside [0, 1] or NaN, a
+ * negative pass_index, a layer empty, unsorted or overlapping, count outside [1, 2^53].  A refused call launches nothing. */
+typedef struct rb_redo_scored {
+  int32_t offset, neurons;
+  double count;
+} rb_redo_scored;
+int rb_redo_mask(const double* sums, const rb_redo_scored* layers, int n_layers, float tau, uint8_t* mask, int64_t* record,
+                 int64_t pass_index, rb_stream_t stream);
+
+/* rb_redo_recycle: ReDo (Algorithm 1) on the FLAT float32 parameter buffer of n elements and the two Adam moment buffers
+ * laid out like it, one launch.  For every neuron i of layer l with mask[mask_offset_l + i] != 0:
+ *   incoming block {offset, per_neuron, bound, constant}: elements j in [offset + i per_neuron, offset + (i + 1) per_neuron)
+ *     become theta0(j) = fmaf(bound, 2u - 1, constant), u = (w >> 8) * 2^-24, w = word (j & 3) of Philox4x32-10 with key
+ *     `seed` and counter (k_lo, k_hi, j >> 2, 0x5245444F), k = pass_index: rb_param_reset's draw on a stream word of its own.
+ *     src_span > 0: element e of the neuron's block reads from neuron e / src_span of the layer whose mask begins at
+ *     src_mask_offset; where that neuron is dormant the element is left to the outgoing rule (it becomes +0);
+ *   outgoing block {offset, rows, row_stride, span}: elements [offset + r row_stride + i span, ... + span) of every row
+ *     r < rows become +0;
+ *   exp_avg and exp_avg_sq of every element written become +0.
+ * Nothing else is written; a table whose mask is all zero writes nothing.  layers: HOST array copied into the launch.
+ * RB_ERR_INVAL: a NULL pointer; RB_ERR_RANGE: n_layers outside [1, RB_MAX_REDO_LAYERS], a layer without neurons (or more
+ * than 65535), n_in outside [1, RB_MAX_REDO_BLOCKS], n_out outside [0, RB_MAX_REDO_BLOCKS], a block empty or outside
+ * [0, n), rows of an outgoing block overlapping (row_stride < neurons * span), two incoming or two outgoing blocks
+ * overlapping, two layers' mask ranges overlapping, a negative or non-finite bound or constant, a src_span that does not
+ * divide per_neuron or names no other layer of the table.  A refused call launches nothing. */
+typedef struct rb_redo_in {
+  int64_t offset, per_neuron, src_span;
+  int32_t src_mask_offset;
+  float bound, constant;
+} rb_redo_in;
+typedef struct rb_redo_out {
+  int64_t offset, rows, row_stride, span;
+} rb_redo_out;
+typedef struct rb_redo_layer {
+  int32_t neurons, mask_offset, n_in, n_out;
+  rb_redo_in in[RB_MAX_REDO_BLOCKS];
+  rb_redo_out out[RB_MAX_REDO_BLOCKS];
+} rb_redo_layer;
+int rb_redo_recycle(float* param, float* exp_avg, float* exp_avg_sq, int64_t n, const rb_redo_layer* layers, int n_layers,
+                    const uint8_t* mask, uint64_t seed, uint64_t pass_index, rb_stream_t stream);
 
 /* Multi-GPU replacement of "all-reduce the flat gradient, then rb_clip_adam on every rank" (agent.py:97-98 under data
  * parallelism; no reference counterpart): reduce-scatter by peer loads + clip + Adam on the owned 1/world parts (moments

@@ -37,6 +37,31 @@ class AdamGroup(C.Structure):
 
 MAX_ADAM_GROUPS = 4   # RB_MAX_ADAM_GROUPS
 
+MAX_REDO_LAYERS, MAX_REDO_BLOCKS = 8, 4        # RB_MAX_REDO_LAYERS, RB_MAX_REDO_BLOCKS
+REDO_RECORD_WORDS = 2 + 2 * MAX_REDO_LAYERS    # RB_REDO_RECORD_WORDS
+
+
+class RedoScored(C.Structure):
+    """rb_redo_scored: one scored layer of rb_redo_mask (its neurons in the sums / mask, activations behind each sum)."""
+    _fields_ = [("offset", C.c_int32), ("neurons", C.c_int32), ("count", C.c_double)]
+
+
+class RedoIn(C.Structure):
+    """rb_redo_in: one incoming parameter block of a scored layer (re-drawn for a dormant neuron)."""
+    _fields_ = [("offset", C.c_int64), ("per_neuron", C.c_int64), ("src_span", C.c_int64), ("src_mask_offset", C.c_int32),
+                ("bound", C.c_float), ("constant", C.c_float)]
+
+
+class RedoOut(C.Structure):
+    """rb_redo_out: one outgoing strided parameter block of a scored layer (zeroed for a dormant neuron)."""
+    _fields_ = [("offset", C.c_int64), ("rows", C.c_int64), ("row_stride", C.c_int64), ("span", C.c_int64)]
+
+
+class RedoLayer(C.Structure):
+    """rb_redo_layer: one scored layer of rb_redo_recycle's table."""
+    _fields_ = [("neurons", C.c_int32), ("mask_offset", C.c_int32), ("n_in", C.c_int32), ("n_out", C.c_int32),
+                ("incoming", RedoIn * MAX_REDO_BLOCKS), ("outgoing", RedoOut * MAX_REDO_BLOCKS)]
+
 
 class Horizon(C.Structure):
     """rb_horizon: one row of an annealed-horizon table (n, gamma ** n, gamma ** k for k < n then zeros)."""
@@ -100,6 +125,9 @@ SIGNATURES = {
                                 _vp, _vp, _vp, _vp, _vp, _vp]),
     "rb_target_ema": (C.c_int, [_vp, _vp, _i64, _f32, _vp, _vp]),
     "rb_param_reset": (C.c_int, [_vp, _i64, C.POINTER(ResetSegment), _i32, _u64, _u64, _vp]),
+    "rb_neuron_scores": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp]),
+    "rb_redo_mask": (C.c_int, [_vp, C.POINTER(RedoScored), _i32, _f32, _vp, _vp, _i64, _vp]),
+    "rb_redo_recycle": (C.c_int, [_vp, _vp, _vp, _i64, C.POINTER(RedoLayer), _i32, _vp, _u64, _u64, _vp]),
     "rb_q_values": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "rb_learn_stats_scratch_elems": (C.c_int, []),
     "rb_learn_stats_batch": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),

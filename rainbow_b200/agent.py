@@ -150,6 +150,82 @@ def target_reset_options(args):
     return tau, int(interval), tuple(shrink)
 
 
+def redo_options(args):
+    """(redo_interval, redo_tau) from `args`, checked: interval an integer >= 0 (0 or absent = no recycling), tau in [0, 1]
+    (default 0.1, ReDo's)."""
+    interval = getattr(args, "redo_interval", None)
+    interval = 0 if interval is None else interval
+    if isinstance(interval, bool) or not isinstance(interval, (int, float)) or int(interval) != interval or interval < 0:
+        raise ValueError(f"redo_interval must be an integer >= 0, got {interval!r}")
+    tau = getattr(args, "redo_tau", None)
+    tau = 0.1 if tau is None else float(tau)
+    if not 0.0 <= tau <= 1.0:
+        raise ValueError(f"redo_tau must be in [0, 1], got {tau}")
+    return int(interval), tau
+
+
+def redo_table(net, offsets):
+    """The scored layers of `net` -- every conv layer (a channel is a neuron), then the hidden layers fc_h_v and fc_h_a -- as
+    rb_redo_recycle takes them: a list of dicts
+      name, neurons, mask_offset (first neuron in the score / mask vectors; fc_h_v and fc_h_a follow each other like the
+                                  columns of the fused head's h),
+      incoming [(flat offset, elements per neuron, src_span, src_mask_offset, bound, constant)]: the neuron's own
+                parameters with reset_table's initialisation; src_span elements read from one neuron of the scored layer
+                below (whose mask begins at src_mask_offset), 0 where nothing scored feeds the block,
+      outgoing [(flat offset, rows, row stride, elements per neuron)]: what the neuron feeds: the next conv weight's
+                [:, i, :, :], or columns [i HW, (i + 1) HW) of weight_mu and weight_sigma of fc_h_v and fc_h_a, or column i
+                of weight_mu and weight_sigma of the stream's fc_z_*."""
+    init = {name: row for (name, _), row in zip(net.named_parameters(), reset_table(net, offsets))}
+    conv_names = [n for n, m in net.convs.named_children() if isinstance(m, nn.Conv2d)]
+    convs = net.conv_layers()
+    layers, mask_offset = [], 0
+
+    def incoming(name, per_neuron, src_span=0, src_mask_offset=0):
+        off, _, bound, constant, _ = init[name]
+        return (off, per_neuron, src_span, src_mask_offset, bound, constant)
+
+    for li, (cn, m) in enumerate(zip(conv_names, convs)):
+        kk = m.kernel_size[0] * m.kernel_size[1]
+        below = layers[-1]["mask_offset"] if li else 0
+        layer = dict(name=f"convs.{cn}", neurons=m.out_channels, mask_offset=mask_offset,
+                     incoming=[incoming(f"convs.{cn}.weight", m.in_channels * kk, kk if li else 0, below),
+                               incoming(f"convs.{cn}.bias", 1)])
+        if li + 1 < len(convs):
+            nxt = convs[li + 1]
+            nkk = nxt.kernel_size[0] * nxt.kernel_size[1]
+            layer["outgoing"] = [(init[f"convs.{conv_names[li + 1]}.weight"][0], nxt.out_channels, nxt.in_channels * nkk, nkk)]
+        else:
+            hw = net.conv_output_size // m.out_channels
+            layer["outgoing"] = [(init[f"{fc}.{kind}"][0], net.hidden_size, net.conv_output_size, hw)
+                                 for fc in ("fc_h_v", "fc_h_a") for kind in ("weight_mu", "weight_sigma")]
+        layers.append(layer)
+        mask_offset += m.out_channels
+    last, hw = layers[-1], net.conv_output_size // convs[-1].out_channels
+    for fc, fz in (("fc_h_v", "fc_z_v"), ("fc_h_a", "fc_z_a")):
+        out_features = getattr(net, fz).out_features
+        layers.append(dict(
+            name=fc, neurons=net.hidden_size, mask_offset=mask_offset,
+            incoming=[incoming(f"{fc}.weight_mu", net.conv_output_size, hw, last["mask_offset"]),
+                      incoming(f"{fc}.weight_sigma", net.conv_output_size, hw, last["mask_offset"]),
+                      incoming(f"{fc}.bias_mu", 1), incoming(f"{fc}.bias_sigma", 1)],
+            outgoing=[(init[f"{fz}.{kind}"][0], out_features, net.hidden_size, 1) for kind in ("weight_mu", "weight_sigma")]))
+        mask_offset += net.hidden_size
+    return layers
+
+
+def redo_layers_c(table):
+    """`redo_table`'s rows as the rb_redo_layer array of rb_redo_recycle."""
+    arr = (_lib.RedoLayer * len(table))()
+    for dst, row in zip(arr, table):
+        dst.neurons, dst.mask_offset = row["neurons"], row["mask_offset"]
+        dst.n_in, dst.n_out = len(row["incoming"]), len(row["outgoing"])
+        for b, blk in enumerate(row["incoming"]):
+            dst.incoming[b] = _lib.RedoIn(*blk)
+        for b, blk in enumerate(row["outgoing"]):
+            dst.outgoing[b] = _lib.RedoOut(*blk)
+    return arr
+
+
 def optimizer_options(args):
     """(weight_decay, reset_optimizer) from `args`, checked: weight_decay finite and >= 0 (0 or absent = plain Adam) with
     fl32(learning_rate) fl32(weight_decay) < 1, the condition rb_clip_adamw takes it under; reset_optimizer a bool."""
@@ -416,6 +492,17 @@ class Agent:
             self.reset_seed = int(self.sync.broadcast_(seed).item())
         self.reset_count = 0
         self._reset_base = None
+        # ReDo: every redo_interval updates the dormant neurons (score <= redo_tau x their layer's mean) are recycled; the
+        # draws share the reset key, with the index of the recycling pass as counter; off by default
+        self.redo_interval, self.redo_tau = redo_options(args)
+        if self.redo_interval and self.peer_optimizer:
+            raise _lib.RainbowB200Error("args.redo_interval needs the replicated optimiser: the peer-memory optimiser shards "
+                                        "the Adam moments a recycling pass zeroes (scoring alone, "
+                                        "recycle_dormant(recycle=False), works with it)")
+        self.redo_count = 0
+        self._redo = None           # device buffers and tables of the passes, built by the first one
+        self._redo_states = None    # the rows of s the most recent update trained on
+        self._redo_passed = False
         self.update_target_net()
         self.target_net.train()
         for p in self.target_net.parameters():
@@ -815,6 +902,88 @@ class Agent:
         if self._horizon is not None:
             self._horizon.restart()
 
+    def _redo_buffers(self):
+        if self._redo is None:
+            table = redo_table(self.online_net, self.optimiser.offsets)
+            total = table[-1]["mask_offset"] + table[-1]["neurons"]
+            self._redo = dict(table=table, layers_c=redo_layers_c(table),
+                              sums=torch.zeros(total, dtype=torch.float64, device=self.device),
+                              mask=torch.zeros(total, dtype=torch.uint8, device=self.device),
+                              record=torch.zeros(_lib.REDO_RECORD_WORDS, dtype=torch.int64, device=self.device),
+                              host=torch.zeros(_lib.REDO_RECORD_WORDS, dtype=torch.int64).pin_memory())
+        return self._redo
+
+    def recycle_dormant(self, tau=None, recycle=True):
+        """Score every ReLU neuron of the online net on the rows of s the most recent update trained on (augmented copies
+        included) and, with `recycle`, apply ReDo (Sokar et al. 2023) to the dormant ones.
+        Score of neuron i of a layer: its mean post-ReLU activation over rows and positions; dormant iff score <= tau x the
+        layer's mean score (tau None: args.redo_tau; 0 counts exactly-dead neurons).  The scoring forward runs without
+        gradients on the current stream with the parameters as they are now: the conv body, then the hidden layer in eval
+        mode (mu only: no noise draw is used or consumed).  Under data parallelism the ranks' score sums are all-reduced,
+        so every rank forms the same mask.
+        Recycling, per dormant neuron, in place in the flat parameter buffer: its incoming weights and bias re-drawn from
+        the network's own initialisation (reset_table; the draws are rb_param_reset's, keyed by reset_seed with redo_count
+        as counter, so replicas agree and a resumed run repeats them), its outgoing weights -- mu and sigma -- set to +0, and
+        exp_avg / exp_avg_sq of every such element set to 0.  Target net, noise, replay, step counts and captured graphs are
+        untouched.  `recycle=False` only scores: nothing in the net changes.  Nothing here synchronises; read the counts
+        with dormant_stats()."""
+        tau = self.redo_tau if tau is None else float(tau)
+        if not 0.0 <= tau <= 1.0:
+            raise ValueError(f"tau must be in [0, 1], got {tau}")
+        if self._redo_states is None:
+            raise _lib.RainbowB200Error("recycle_dormant needs the batch of an update: call learn() first")
+        if recycle and self.optimiser.peer is not None:
+            raise _lib.RainbowB200Error("recycling needs the replicated optimiser: the peer-memory optimiser shards the Adam "
+                                        "moments a pass zeroes (recycle=False scores without it)")
+        on, lib = self.online_net, _lib.load()
+        states = self._redo_states
+        if not on.manual_conv_ok(states):
+            raise _lib.RainbowB200Error("the scoring forward runs the conv body through cuDNN on a CUDA device")
+        rd = self._redo_buffers()
+        table, sums = rd["table"], rd["sums"]
+        R = states.shape[0]
+        with torch.no_grad():
+            acts = on.conv_forward_saving(states)
+            for row, a in zip(table, acts[1:]):
+                a = a.contiguous()
+                _lib.check(lib.rb_neuron_scores(_lib.ptr(a), R, a.shape[1], a.shape[2] * a.shape[3],
+                                                sums.data_ptr() + 8 * row["mask_offset"], _lib.stream()))
+            feats = acts[-1].reshape(R, -1)
+            if self.use_fused_head and on.fused_ok(R):
+                _, h, _ = on.head().forward(feats, noisy=False)      # h [R, 2 hidden]: fc_h_v's neurons, then fc_h_a's
+            else:
+                h = torch.cat([torch.relu(nn.functional.linear(feats, m.weight_mu, m.bias_mu))
+                               for m in (on.fc_h_v, on.fc_h_a)], dim=1).contiguous()
+            _lib.check(lib.rb_neuron_scores(_lib.ptr(h), R, h.shape[1], 1,
+                                            sums.data_ptr() + 8 * table[len(acts) - 1]["mask_offset"], _lib.stream()))
+        if self.sync.enabled:
+            torch.distributed.all_reduce(sums, op=torch.distributed.ReduceOp.SUM, group=self.sync.group)
+        rows = R * self.sync.world_size
+        scored = (_lib.RedoScored * len(table))(*[
+            _lib.RedoScored(row["mask_offset"], row["neurons"], float(rows * (a.shape[2] * a.shape[3] if a is not None else 1)))
+            for row, a in zip(table, acts[1:] + [None, None])])
+        _lib.check(lib.rb_redo_mask(_lib.ptr(sums), scored, len(table), tau, _lib.ptr(rd["mask"]), _lib.ptr(rd["record"]),
+                                    self.redo_count, _lib.stream()))
+        self._redo_passed = True
+        if recycle:
+            opt = self.optimiser
+            _lib.check(lib.rb_redo_recycle(_lib.ptr(opt.flat_param), _lib.ptr(opt.exp_avg), _lib.ptr(opt.exp_avg_sq), opt.numel,
+                                           rd["layers_c"], len(table), _lib.ptr(rd["mask"]), self.reset_seed, self.redo_count,
+                                           _lib.stream()))
+            self.redo_count += 1
+
+    def dormant_stats(self):
+        """([(layer name, neurons, dormant neurons)], pass index) of the most recent recycle_dormant() pass -- the index
+        is the redo_count its draws used (or would have used) -- or ([], None) before the first.  One device-to-host copy
+        and one stream synchronisation."""
+        if not self._redo_passed:
+            return [], None
+        rd = self._redo
+        rd["host"].copy_(rd["record"], non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        rec = rd["host"].tolist()
+        return [(row["name"], rec[2 + 2 * l], rec[3 + 2 * l]) for l, row in enumerate(rd["table"])], rec[0]
+
     @staticmethod
     def _copies_error(copies):
         return _lib.RainbowB200Error(
@@ -826,10 +995,12 @@ class Agent:
         if isinstance(mem, ReplayMemory):
             batch = mem.sample(self.batch_size, shift_pad=self.augment_shift, intensity=self.augment_intensity,
                                copies=self.augment_copies, horizon=self._horizon)
+            self._redo_states = batch[1]
             gate = mem.sample_gate()
             return self._update_from_batch(batch, after_loss=lambda loss: mem.update_priorities(batch[0], loss, gate=gate),
                                            gate=gate)
         batch = mem.sample(self.batch_size)
+        self._redo_states = batch[1]
         loss = self._update_from_batch(batch)
         mem.update_priorities(batch[0], loss.detach().cpu().numpy())  # a foreign (reference-style, host) memory: agent.py:100
         return loss
@@ -903,9 +1074,12 @@ class Agent:
             self.online_net._noise_pending = False
             self.online_net._eps_stale = self.online_net._eps_stale or pending
             self.last_loss, mem._last = loss, ws
+            self._redo_states = ws.states
         self._learn_calls += 1
         if self.reset_interval and self._learn_calls % self.reset_interval == 0:
             self.reset_parameters(*self.reset_shrink)
+        if self.redo_interval and self._learn_calls % self.redo_interval == 0:
+            self.recycle_dormant()
         if self._learn_calls % 4096 == 0 and isinstance(mem, ReplayMemory):
             # diagnostics only (the device already skipped such updates): how many batches stayed invalid after
             # max_attempts redraws -- a ring that is too empty around the write head, or zero-priority leaves

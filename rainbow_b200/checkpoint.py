@@ -369,6 +369,12 @@ def _meta(agent, mem):
         hyper["weight_decay"] = agent.weight_decay
     if agent.reset_optimizer:
         hyper["reset_optimizer"] = True
+    if agent.redo_interval:
+        hyper["redo_interval"] = agent.redo_interval
+    if agent.redo_tau != 0.1:
+        hyper["redo_tau"] = agent.redo_tau
+    if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
+        learner["redo_count"] = agent.redo_count
     if opt.grouped:   # the group optimiser's bias-correction counts, [encoder, head]
         learner["optimiser_group_steps"] = opt.group_step_counts()
     hz = agent._horizon
@@ -459,6 +465,7 @@ _SCALARS = {
     ("learner", "reset_seed"): lambda v, m: v is None or _is_int(v, 0, _U63),      # absent (both): an older manifest
     ("learner", "reset_count"): lambda v, m: v is None or _is_int(v, 0, _U63),
     ("learner", "horizon_step"): lambda v, m: v is None or _is_int(v, 0, _U63),     # absent: annealing off, or step 0
+    ("learner", "redo_count"): lambda v, m: v is None or _is_int(v, 0, _U63),       # absent: no recycling pass yet
     ("replay", "t"): lambda v, m: _is_int(v, 0, _U63),
     ("replay", "seed"): lambda v, m: _is_int(v, 0, _U64),
     ("replay", "priority_weight"): lambda v, m: isinstance(v, (int, float)) and not isinstance(v, bool) and math.isfinite(v),
@@ -589,6 +596,7 @@ def _restore(agent, mem, d, staging):
     on._eps_stale, tg._eps_stale = learner["online_eps_stale"], learner["target_eps_stale"]
     agent._learn_calls = learner["learn_calls"]
     agent.reset_count = learner.get("reset_count") or 0
+    agent.redo_count = learner.get("redo_count") or 0
     if learner.get("reset_seed") is not None:
         agent.reset_seed = learner["reset_seed"]
     if agent._horizon is not None:

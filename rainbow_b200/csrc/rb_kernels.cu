@@ -679,8 +679,9 @@ k_gather_shift_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict_
 //   copy j multiplier  (c_lo, c_hi, b, INTS_STREAM + j): box_muller(x, y).x -> the state's, box_muller(z, w).x -> the next
 //                      state's.
 // The streams in use: sampling 0x5A4D504C, noise 0x4E4F4953 + i (i < RB_MAX_NOISY_LAYERS), shift 0x53484654 + j and
-// intensity 0x494E5453 + j (j < RB_MAX_AUG_COPIES), parameter reset 0x52534554 ("RSET", k_param_reset): the five ranges
-// [0x494E5453, 0x494E545A], [0x4E4F4953, 0x4E4F495A], {0x52534554}, [0x53484654, 0x5348465B] and {0x5A4D504C} are disjoint.
+// intensity 0x494E5453 + j (j < RB_MAX_AUG_COPIES), parameter reset 0x52534554 ("RSET", k_param_reset), recycling 0x5245444F
+// ("REDO", k_redo_recycle): the six ranges [0x494E5453, 0x494E545A], [0x4E4F4953, 0x4E4F495A], {0x5245444F}, {0x52534554},
+// [0x53484654, 0x5348465B] and {0x5A4D504C} are disjoint.
 constexpr uint32_t INTS_STREAM = 0x494E5453u;        // "INTS"
 
 __device__ __forceinline__ float4 aug4(const uint8_t* s_frame, int y, int x, int dy, int dx, bool scaled, float mult) {
@@ -2107,6 +2108,125 @@ k_param_reset(float* __restrict__ param, const __grid_constant__ ResetPlan plan,
   }
 }
 
+// ================================================================================================
+// K10  dormant-neuron scores, mask and ReDo recycling (Sokar et al. 2023) -- all decided and applied on the device.
+// ================================================================================================
+// k_neuron_scores: sums[c] = sum over (row, position) of act[r][c][p], one CTA per neuron.  Thread t takes the elements
+// i = r HW + p with i % 256 == t, in increasing i: fp32 partial sums over chunks of REDO_CHUNK elements, each chunk added to a
+// float64 accumulator; the 256 accumulators are summed by a fixed float64 tree in shared memory.  k_bias_grad computes the
+// same sum in one CTA per channel too, but carries it in fp32 to the end (200 000 addends at batch 512): the float64 total
+// keeps the error to that of one chunk, 63 * 2^-24 relative, whatever R is, and gives the ranks' all-reduce exact addends.
+constexpr int REDO_THREADS = 256;
+constexpr int REDO_CHUNK = 64;
+constexpr int REDO_NEURON_CTAS = 8;                   // CTAs that share one dormant neuron's elements
+constexpr uint32_t REDO_STREAM = 0x5245444Fu;        // "REDO": listed with the other stream words above INTS_STREAM
+
+__global__ void __launch_bounds__(REDO_THREADS)
+k_neuron_scores(const float* __restrict__ act, int R, int C, int HW, double* __restrict__ sums) {
+  __shared__ double s_red[REDO_THREADS];
+  const int c = blockIdx.x;
+  const int64_t total = (int64_t)R * HW;
+  double acc = 0.0;
+  float part = 0.0f;
+  int in_chunk = 0;
+  for (int64_t i = threadIdx.x; i < total; i += REDO_THREADS) {
+    const int64_t r = i / HW, p = i - r * HW;
+    part = __fadd_rn(part, __ldg(act + (r * C + c) * HW + p));
+    if (++in_chunk == REDO_CHUNK) { acc += (double)part; part = 0.0f; in_chunk = 0; }
+  }
+  acc += (double)part;
+  s_red[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = REDO_THREADS / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) s_red[threadIdx.x] += s_red[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) sums[c] = s_red[0];
+}
+
+struct RedoMaskPlan {
+  int32_t n_layers;
+  int32_t offset[RB_MAX_REDO_LAYERS];      // first neuron of the layer in sums / mask
+  int32_t neurons[RB_MAX_REDO_LAYERS];
+  double count[RB_MAX_REDO_LAYERS];        // R HW: activations behind one sum
+};
+
+// One CTA per layer.  score s_i = sums[i] / count, mean over the layer summed in float64 in neuron order (thread 0), neuron
+// i dormant iff s_i <= tau * mean.  record: int64 {pass index, n_layers, (neurons, dormant) per layer}.
+__global__ void __launch_bounds__(REDO_THREADS)
+k_redo_mask(const double* __restrict__ sums, const __grid_constant__ RedoMaskPlan plan, float tau, uint8_t* __restrict__ mask,
+            long long* __restrict__ record, long long pass_index) {
+  __shared__ double s_threshold;
+  const int l = blockIdx.x, n = plan.neurons[l];
+  const double* s = sums + plan.offset[l];
+  uint8_t* m = mask + plan.offset[l];
+  const double count = plan.count[l];
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int i = 0; i < n; ++i) t += s[i] / count;
+    s_threshold = (double)tau * (t / (double)n);
+  }
+  __syncthreads();
+  const double threshold = s_threshold;
+  int dormant = 0;
+  for (int i0 = 0; i0 < n; i0 += REDO_THREADS) {
+    const int i = i0 + threadIdx.x;
+    const int d = (i < n) && (s[i] / count <= threshold);
+    if (i < n) m[i] = (uint8_t)d;
+    dormant += __syncthreads_count(d);
+  }
+  if (threadIdx.x == 0) {
+    record[2 + 2 * l] = n;
+    record[3 + 2 * l] = dormant;
+    if (l == 0) { record[0] = pass_index; record[1] = plan.n_layers; }
+  }
+}
+
+struct RedoPlan {
+  rb_redo_layer layer[RB_MAX_REDO_LAYERS];
+};
+
+// Grid (x: chunk of the neuron's elements, y: neuron, z: layer); a CTA whose neuron is not dormant returns after one mask
+// byte.  Incoming element j of a dormant neuron gets theta0(j) -- k_param_reset's formula with REDO_STREAM -- unless the
+// upstream neuron it reads from is dormant too: that element is an outgoing element of the upstream neuron and the CTA that
+// zeroes it is its only writer.  Every written element's moments become 0.
+__global__ void __launch_bounds__(REDO_THREADS)
+k_redo_recycle(float* __restrict__ param, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
+               const __grid_constant__ RedoPlan plan, const uint8_t* __restrict__ mask, uint64_t seed, uint64_t pass_index) {
+  const rb_redo_layer& L = plan.layer[blockIdx.z];
+  const int i = blockIdx.y;
+  if (i >= L.neurons || !mask[L.mask_offset + i]) return;
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const int64_t first = (int64_t)blockIdx.x * REDO_THREADS + threadIdx.x, stride = (int64_t)gridDim.x * REDO_THREADS;
+  for (int b = 0; b < L.n_in; ++b) {
+    const rb_redo_in& in = L.in[b];
+    const uint8_t* up = in.src_span > 0 ? mask + in.src_mask_offset : nullptr;
+    for (int64_t e = first; e < in.per_neuron; e += stride) {
+      if (up && up[e / in.src_span]) continue;
+      const int64_t j = in.offset + (int64_t)i * in.per_neuron + e;
+      const uint4 r = philox4x32_10(make_uint4((uint32_t)pass_index, (uint32_t)(pass_index >> 32), (uint32_t)(j >> 2),
+                                               REDO_STREAM), key);
+      const int q = (int)(j & 3);
+      const uint32_t w = q == 0 ? r.x : q == 1 ? r.y : q == 2 ? r.z : r.w;
+      const float u = (float)(w >> 8) * 0x1.0p-24f;
+      param[j] = __fmaf_rn(in.bound, __fmaf_rn(2.0f, u, -1.0f), in.constant);
+      exp_avg[j] = 0.0f;
+      exp_avg_sq[j] = 0.0f;
+    }
+  }
+  for (int b = 0; b < L.n_out; ++b) {
+    const rb_redo_out& out = L.out[b];
+    const int64_t total = out.rows * out.span;
+    for (int64_t e = first; e < total; e += stride) {
+      const int64_t r = e / out.span, p = e - r * out.span;
+      const int64_t j = out.offset + r * out.row_stride + (int64_t)i * out.span + p;
+      param[j] = 0.0f;
+      exp_avg[j] = 0.0f;
+      exp_avg_sq[j] = 0.0f;
+    }
+  }
+}
+
 // The launch of rb_append and rb_append_batch, after each has checked its own arguments.
 int append_launch(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
                   float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max, const AppendBatch& ab,
@@ -2702,6 +2822,103 @@ int rb_param_reset(float* param, int64_t n, const rb_reset_segment* segs, int n_
   { ProfScope prof_(RB_K_PARAM_RESET, (cudaStream_t)stream);
     k_param_reset<<<grid, RESET_THREADS, 0, (cudaStream_t)stream>>>(param, plan, seed, reset_index); }
   return check_launch("rb_param_reset");
+}
+
+int rb_neuron_scores(const float* act, int R, int C, int HW, double* sums, rb_stream_t stream) {
+  if (!act || !sums) return fail(RB_ERR_INVAL, "rb_neuron_scores: null pointer");
+  if (R <= 0 || C <= 0 || HW <= 0) return fail(RB_ERR_INVAL, "rb_neuron_scores: R, C and HW must be positive");
+  k_neuron_scores<<<C, REDO_THREADS, 0, (cudaStream_t)stream>>>(act, R, C, HW, sums);
+  return check_launch("rb_neuron_scores");
+}
+
+int rb_redo_mask(const double* sums, const rb_redo_scored* layers, int n_layers, float tau, uint8_t* mask, int64_t* record,
+                 int64_t pass_index, rb_stream_t stream) {
+  if (!sums || !layers || !mask || !record) return fail(RB_ERR_INVAL, "rb_redo_mask: null pointer");
+  if (n_layers < 1 || n_layers > RB_MAX_REDO_LAYERS)
+    return fail(RB_ERR_RANGE, "rb_redo_mask: n_layers outside [1, RB_MAX_REDO_LAYERS]");
+  if (!(tau >= 0.0f && tau <= 1.0f)) return fail(RB_ERR_RANGE, "rb_redo_mask: tau outside [0, 1]");
+  if (pass_index < 0) return fail(RB_ERR_RANGE, "rb_redo_mask: pass_index must not be negative");
+  RedoMaskPlan plan;
+  memset(&plan, 0, sizeof(plan));
+  plan.n_layers = n_layers;
+  int64_t end = 0;
+  for (int l = 0; l < n_layers; ++l) {
+    const rb_redo_scored& s = layers[l];
+    if (s.neurons <= 0 || s.offset < end || (int64_t)s.offset + s.neurons > INT32_MAX)
+      return fail(RB_ERR_RANGE, "rb_redo_mask: layer empty, unsorted or overlapping");
+    if (!(s.count >= 1.0 && s.count <= 9007199254740992.0))
+      return fail(RB_ERR_RANGE, "rb_redo_mask: count must be in [1, 2^53]");
+    plan.offset[l] = s.offset; plan.neurons[l] = s.neurons; plan.count[l] = s.count;
+    end = (int64_t)s.offset + s.neurons;
+  }
+  k_redo_mask<<<n_layers, REDO_THREADS, 0, (cudaStream_t)stream>>>(sums, plan, tau, mask, (long long*)record,
+                                                                   (long long)pass_index);
+  return check_launch("rb_redo_mask");
+}
+
+int rb_redo_recycle(float* param, float* exp_avg, float* exp_avg_sq, int64_t n, const rb_redo_layer* layers, int n_layers,
+                    const uint8_t* mask, uint64_t seed, uint64_t pass_index, rb_stream_t stream) {
+  if (!param || !exp_avg || !exp_avg_sq || !layers || !mask) return fail(RB_ERR_INVAL, "rb_redo_recycle: null pointer");
+  if (n_layers < 1 || n_layers > RB_MAX_REDO_LAYERS)
+    return fail(RB_ERR_RANGE, "rb_redo_recycle: n_layers outside [1, RB_MAX_REDO_LAYERS]");
+  RedoPlan plan;
+  memset(&plan, 0, sizeof(plan));
+  // extents [begin, end) of every incoming block and of every outgoing block: each kind must be disjoint within itself (an
+  // incoming block may be another layer's outgoing block: the kernel gives such an element to the zeroing writer)
+  int64_t in_ext[RB_MAX_REDO_LAYERS * RB_MAX_REDO_BLOCKS][2], out_ext[RB_MAX_REDO_LAYERS * RB_MAX_REDO_BLOCKS][2];
+  int n_in = 0, n_out = 0, widest = 0;
+  for (int l = 0; l < n_layers; ++l) {
+    const rb_redo_layer& L = layers[l];
+    if (L.neurons <= 0 || L.mask_offset < 0 || (int64_t)L.mask_offset + L.neurons > INT32_MAX)
+      return fail(RB_ERR_RANGE, "rb_redo_recycle: layer empty or mask range invalid");
+    if (L.n_in < 1 || L.n_in > RB_MAX_REDO_BLOCKS || L.n_out < 0 || L.n_out > RB_MAX_REDO_BLOCKS)
+      return fail(RB_ERR_RANGE, "rb_redo_recycle: n_in outside [1, RB_MAX_REDO_BLOCKS] or n_out outside [0, RB_MAX_REDO_BLOCKS]");
+    for (int b = 0; b < L.n_in; ++b) {
+      const rb_redo_in& in = L.in[b];
+      if (in.per_neuron <= 0 || in.offset < 0 || in.per_neuron > n / L.neurons || in.offset > n - in.per_neuron * L.neurons)
+        return fail(RB_ERR_RANGE, "rb_redo_recycle: incoming block empty or outside [0, n)");
+      if (!(in.bound >= 0.0f && in.bound <= FLT_MAX) || !(in.constant >= 0.0f && in.constant <= FLT_MAX))
+        return fail(RB_ERR_RANGE, "rb_redo_recycle: bound and constant must be finite and non-negative");
+      if (in.src_span < 0 || (in.src_span > 0 && in.per_neuron % in.src_span))
+        return fail(RB_ERR_RANGE, "rb_redo_recycle: src_span must be 0 or divide per_neuron");
+      if (in.src_span > 0) {   // the upstream mask range must be exactly one layer's
+        bool found = false;
+        for (int u = 0; u < n_layers; ++u)
+          found = found || (u != l && layers[u].mask_offset == in.src_mask_offset &&
+                            layers[u].neurons == in.per_neuron / in.src_span);
+        if (!found) return fail(RB_ERR_RANGE, "rb_redo_recycle: src_mask_offset and src_span name no layer of the table");
+      }
+      in_ext[n_in][0] = in.offset; in_ext[n_in][1] = in.offset + in.per_neuron * L.neurons; ++n_in;
+    }
+    for (int b = 0; b < L.n_out; ++b) {
+      const rb_redo_out& out = L.out[b];
+      if (out.rows <= 0 || out.span <= 0 || out.offset < 0 || out.span > n / L.neurons ||
+          out.row_stride < out.span * L.neurons || out.row_stride > n || out.rows > n / out.row_stride + 1 ||
+          out.offset > n - ((out.rows - 1) * out.row_stride + out.span * L.neurons))
+        return fail(RB_ERR_RANGE, "rb_redo_recycle: outgoing block empty, rows overlapping or outside [0, n)");
+      out_ext[n_out][0] = out.offset;
+      out_ext[n_out][1] = out.offset + (out.rows - 1) * out.row_stride + out.span * L.neurons; ++n_out;
+    }
+    plan.layer[l] = L;
+    if (L.neurons > widest) widest = L.neurons;
+  }
+  for (int a = 0; a < n_layers; ++a)
+    for (int b = a + 1; b < n_layers; ++b)
+      if (layers[a].mask_offset < layers[b].mask_offset + layers[b].neurons &&
+          layers[b].mask_offset < layers[a].mask_offset + layers[a].neurons)
+        return fail(RB_ERR_RANGE, "rb_redo_recycle: mask ranges of two layers overlap");
+  for (int a = 0; a < n_in; ++a)
+    for (int b = a + 1; b < n_in; ++b)
+      if (in_ext[a][0] < in_ext[b][1] && in_ext[b][0] < in_ext[a][1])
+        return fail(RB_ERR_RANGE, "rb_redo_recycle: incoming blocks overlap");
+  for (int a = 0; a < n_out; ++a)
+    for (int b = a + 1; b < n_out; ++b)
+      if (out_ext[a][0] < out_ext[b][1] && out_ext[b][0] < out_ext[a][1])
+        return fail(RB_ERR_RANGE, "rb_redo_recycle: outgoing blocks overlap");
+  if (widest > 65535) return fail(RB_ERR_RANGE, "rb_redo_recycle: more than 65535 neurons in a layer");
+  dim3 grid(REDO_NEURON_CTAS, (unsigned)widest, (unsigned)n_layers);
+  k_redo_recycle<<<grid, REDO_THREADS, 0, (cudaStream_t)stream>>>(param, exp_avg, exp_avg_sq, plan, mask, seed, pass_index);
+  return check_launch("rb_redo_recycle");
 }
 
 }  // extern "C"
