@@ -373,6 +373,33 @@ int rb_c51_dueling_avg_loss_grad(const float* z_online, const float* z_target, i
                                  const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int M,
                                  int K, float* loss, float* dz, float* m_out, int64_t* astar_out, rb_stream_t stream);
 
+/* Quantile regression (QR-DQN, Dabney et al. 2018) in place of the categorical projection: atoms = N quantiles per action
+ * (2 <= N <= RB_MAX_ATOMS) at the midpoints tau_i = (2i + 1) / (2N); no support.  For sample b with taken action a:
+ *   theta_i = q_online(s, a)_i (the dueling combination model.py:75 without a softmax),
+ *   a* = argmax_a (1/N) sum_j q_online(s', a)_j (double DQN; the first maximum wins),
+ *   T_j = r + fl32(nonterminal * gamma_n) q_target(s', a*)_j,  u_ij = T_j - theta_i,
+ *   loss_b = sum_i (1/N) sum_j |tau_i - [u_ij < 0]| H_kappa(u_ij) / kappa,  H_kappa(u) = u^2 / 2 if |u| <= kappa, else
+ *            kappa (|u| - kappa / 2)   (the TD priority), and the gradient of (1/B) sum_b w_b loss_b:
+ *   g_i = -(w_b / B) (1/N) sum_j |tau_i - [u_ij < 0]| clamp(u_ij, -kappa, kappa) / kappa.
+ * rb_qr_dueling_loss_grad takes the fused heads' rows like rb_c51_dueling_loss_grad (z_online 2B rows, s then s';
+ * z_target B rows) and writes loss[B] and dz[B][atoms*(1+actions)] (dz_v = g, dz_a[a'] = g ([a' == a] - 1/A));
+ * rb_qr_loss_grad takes plain quantile rows [B][A][N] like rb_c51_loss_grad and writes grad[B][A][N] (g at the taken
+ * action, 0 elsewhere).  Optional outputs: theta_out [B][N] receives the T rows, astar_out [B] a*.  kappa must be finite
+ * and > 0.  Sums run in a fixed order (eager launches and graph replays agree bitwise).  RB_ERR_INVAL: a NULL required
+ * pointer, B, actions <= 0, atoms < 2 or a bad kappa; RB_ERR_RANGE: atoms > RB_MAX_ATOMS or rows too large for shared
+ * memory.  A refused call writes nothing.  Profiled under RB_K_C51_DUELING / RB_K_C51, the loss they stand for. */
+int rb_qr_dueling_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
+                            const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
+                            int B, float* loss, float* dz, float* theta_out, int64_t* astar_out, rb_stream_t stream);
+int rb_qr_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                    const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n, int B,
+                    int A, int N, float* loss, float* grad_q_online_s, float* theta_out, int64_t* astar_out,
+                    rb_stream_t stream);
+/* rb_q_values for quantile heads: q[m][a] = (1/N) sum_j (zv + za[a] - mean_a za)_j and its arg-max (first maximum) / max
+ * over actions, from z[M][atoms*(1+actions)].  q, best_action, best_q are each optional (not all NULL). */
+int rb_qr_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
+                   rb_stream_t stream);
+
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */
 int rb_noisy_compose(const float* mu, const float* sigma, const float* eps, int64_t count, float* out,
@@ -552,6 +579,9 @@ int rb_peer_clip_adam(const float* const* peer_grad, float* const* peer_param, u
  *   target_mean  mean_i sum_z m_iz support_z
  *   edge_mass    mean_i (m_i,0 + m_i,Z-1), the projected mass the clamp to [Vmin, Vmax] piles onto the end atoms
  *   weight_min   min_i w_i
+ * Under the quantile loss (rb_learn_stats_batch_qr) loss_i is the quantile loss, q_mean = mean_i mean_k theta_ik of the
+ * online quantiles of the taken action, target_mean = mean_i mean_k T_ik, and edge_mass is NaN: there is no support to
+ * clamp to.
  *   grad_norm    *grad_norm (the pre-clip norm written by rb_clip_adam / rb_peer_adam_gather as norm_out)
  *   clip_coef    min(1, max_norm / (grad_norm + 1e-6)), the factor rb_clip_adam scaled the gradient by
  *   applied      1 if the optimiser stepped, 0 if *gate == 0 made it skip the step */
@@ -578,6 +608,10 @@ int rb_learn_stats_batch(const float* loss, const float* weights, const int64_t*
                          const float* z, const float* q, int B, int A, int Z, double* scratch, rb_stream_t stream);
 int rb_learn_stats_write(const double* scratch, const float* grad_norm, const int32_t* gate, float max_norm,
                          rb_learn_stats_record* ring, int capacity, int64_t* counter, rb_stream_t stream);
+/* rb_learn_stats_batch for rb_qr_*_loss_grad: theta[B][N] is their theta_out (the T rows), z / q the online quantile rows
+ * in one of the two layouts above (N = atoms); no support.  Same scratch, refusals and rb_learn_stats_write. */
+int rb_learn_stats_batch_qr(const float* loss, const float* weights, const int64_t* actions, const float* theta, const float* z,
+                            const float* q, int B, int A, int N, double* scratch, rb_stream_t stream);
 int rb_learn_stats(const float* loss, const float* weights, const int64_t* actions, const float* m, const float* support,
                    const float* z, const float* q, int B, int A, int Z, const float* grad_norm, const int32_t* gate,
                    float max_norm, double* scratch, rb_learn_stats_record* ring, int capacity, int64_t* counter,

@@ -129,6 +129,11 @@ SIGNATURES = {
     "rb_redo_mask": (C.c_int, [_vp, C.POINTER(RedoScored), _i32, _f32, _vp, _vp, _i64, _vp]),
     "rb_redo_recycle": (C.c_int, [_vp, _vp, _vp, _i64, C.POINTER(RedoLayer), _i32, _vp, _u64, _u64, _vp]),
     "rb_q_values": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "rb_qr_dueling_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _vp, _vp, _vp, _vp,
+                                          _vp]),
+    "rb_qr_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "rb_qr_q_values": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "rb_learn_stats_batch_qr": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "rb_learn_stats_scratch_elems": (C.c_int, []),
     "rb_learn_stats_batch": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "rb_learn_stats_write": (C.c_int, [_vp, _vp, _vp, _f32, _vp, _i32, _vp, _vp]),

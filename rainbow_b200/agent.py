@@ -16,7 +16,9 @@ One `learn(mem)` (agent.py:61-100) is:
     fused noisy dueling heads (rb_head_forward) on the conv features -- online net on [s; s'], target on s'
     K3 rb_c51_dueling_loss_grad               (agent.py:67,72-73,76-96 + softmax halves of model.py:76-79 + model.py:75)
                                               [M or K > 1: rb_c51_dueling_avg_loss_grad -- DrQ's target averaged over
-                                               the K copies of s', loss over the M copies of s]
+                                               the K copies of s', loss over the M copies of s;
+                                               args.distribution = "quantile": rb_qr_dueling_loss_grad -- QR-DQN's
+                                               quantile Huber loss, no support or projection]
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
@@ -94,6 +96,62 @@ def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, ret
         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
         float(gamma_n), B, M, K, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), _lib.stream()))
     return loss, dz
+
+
+def qr_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, kappa, gamma_n,
+                 theta_out=None, astar_out=None):
+    """The quantile loss (rb_qr_loss_grad) on quantile rows [B,A,N]; returns (loss[B], grad[B,A,N])."""
+    B, A, N = q_online_s.shape
+    loss = torch.empty(B, dtype=torch.float32, device=q_online_s.device)
+    grad = torch.empty((B, A, N), dtype=torch.float32, device=q_online_s.device)
+    _lib.check(_lib.load().rb_qr_loss_grad(
+        _lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
+        _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, A, N, _lib.ptr(loss), _lib.ptr(grad),
+        _lib.ptr(theta_out), _lib.ptr(astar_out), _lib.stream()))
+    return loss, grad
+
+
+def qr_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, kappa, gamma_n,
+                         theta_out=None, astar_out=None):
+    """The quantile loss fed straight by the fused heads (rb_qr_dueling_loss_grad), rows as c51_dueling_loss_grad takes
+    them; returns (loss[B], dz[B, N(1+A)])."""
+    B = actions.shape[0]
+    loss = torch.empty(B, dtype=torch.float32, device=actions.device)
+    dz = torch.empty((B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
+    _lib.check(_lib.load().rb_qr_dueling_loss_grad(
+        _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+        _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, _lib.ptr(loss), _lib.ptr(dz),
+        _lib.ptr(theta_out), _lib.ptr(astar_out), _lib.stream()))
+    return loss, dz
+
+
+DISTRIBUTIONS = ("categorical", "quantile")
+
+
+def distribution_options(args):
+    """(distribution, quantile_kappa) from `args`, checked: distribution "categorical" (absent or None: C51's projection
+    onto [V_min, V_max]) or "quantile" (QR-DQN: args.atoms quantiles per action, 2 <= atoms <= 128, no support);
+    quantile_kappa, the quantile Huber threshold, finite and > 0 as an fp32 (absent or None: 1.0), and None under
+    "categorical"."""
+    dist = getattr(args, "distribution", None)
+    dist = "categorical" if dist is None else dist
+    if not isinstance(dist, str) or dist not in DISTRIBUTIONS:
+        raise ValueError(f"distribution must be one of {DISTRIBUTIONS}, got {dist!r}")
+    if dist == "categorical":
+        return dist, None
+    kappa = getattr(args, "quantile_kappa", None)
+    kappa = 1.0 if kappa is None else float(kappa)
+    with np.errstate(over="ignore"):
+        k32 = np.float32(kappa)
+    if not (math.isfinite(kappa) and kappa > 0.0 and np.isfinite(k32) and k32 > 0.0):
+        raise ValueError(f"quantile_kappa must be finite and > 0 (as an fp32), got {kappa}")
+    if not 2 <= args.atoms <= 128:
+        raise ValueError(f"distribution 'quantile' needs 2 <= atoms <= 128 quantiles, got {args.atoms}")
+    copies = (getattr(args, "augment_m", 1), getattr(args, "augment_k", 1))
+    if copies != (1, 1):
+        raise ValueError(f"augment_m / augment_k = {copies} average categorical targets; with distribution 'quantile' "
+                         f"both must be 1")
+    return dist, kappa
 
 
 ENCODER, HEAD = 0, 1   # the two groups of reset_table / Agent.reset_parameters
@@ -416,6 +474,9 @@ class Agent:
         if not all(1 <= c <= ReplayMemory.MAX_AUG_COPIES for c in self.augment_copies):
             raise ValueError(f"augment_m and augment_k must be in [1, {ReplayMemory.MAX_AUG_COPIES}], got "
                              f"{self.augment_copies}")
+        # the distributional loss: C51's categorical projection (default) or quantile regression (QR-DQN)
+        self.distribution, self.quantile_kappa = distribution_options(args)
+        self.quantile = self.distribution == "quantile"
         # Polyak target updates (tau > 0: every applied optimiser step also moves the target, DrQ(eps) / SPR / BBF) and
         # periodic shrink-and-perturb resets of the online net (SR-SPR, BBF); both off by default
         self.target_tau, self.reset_interval, self.reset_shrink = target_reset_options(args)
@@ -531,8 +592,9 @@ class Agent:
     def q_select(self, states, q_out=None):
         """Greedy action and its value for a batch of states [N, history, 84, 84] (device): conv body (cuDNN), fused
         noisy dueling head, then rb_q_values -- softmax over atoms, expectation over the support (agent.py:55) and the
-        arg-max / max over actions in one launch.  Returns device tensors (actions int64[N], values float32[N]); nothing
-        synchronises.  Falls back to plain torch ops for head shapes the fused kernels do not cover."""
+        arg-max / max over actions in one launch; under the quantile distribution rb_qr_q_values, the mean over quantiles.
+        Returns device tensors (actions int64[N], values float32[N]); nothing synchronises.  Falls back to plain torch ops
+        for head shapes the fused kernels do not cover."""
         on = self.online_net
         N = states.shape[0]
         with torch.no_grad():
@@ -541,10 +603,15 @@ class Agent:
                 z, _, _ = on.head().forward(x)
                 best_a = torch.empty(N, dtype=torch.int64, device=self.device)
                 best_q = torch.empty(N, dtype=torch.float32, device=self.device)
-                _lib.check(_lib.load().rb_q_values(_lib.ptr(z), N, self.action_space, self.atoms, _lib.ptr(self.support),
-                                                   _lib.ptr(q_out), _lib.ptr(best_a), _lib.ptr(best_q), _lib.stream()))
+                if self.quantile:
+                    _lib.check(_lib.load().rb_qr_q_values(_lib.ptr(z), N, self.action_space, self.atoms, _lib.ptr(q_out),
+                                                          _lib.ptr(best_a), _lib.ptr(best_q), _lib.stream()))
+                else:
+                    _lib.check(_lib.load().rb_q_values(_lib.ptr(z), N, self.action_space, self.atoms,
+                                                       _lib.ptr(self.support), _lib.ptr(q_out), _lib.ptr(best_a),
+                                                       _lib.ptr(best_q), _lib.stream()))
                 return best_a, best_q
-            q = (on(states) * self.support).sum(2)
+            q = on.logits(states).mean(2) if self.quantile else (on(states) * self.support).sum(2)
             if q_out is not None:
                 q_out.copy_(q)
             best_q, best_a = q.max(1)
@@ -741,8 +808,12 @@ class Agent:
                 z_on, h_on, p_on = on.head().forward(xs_d, x_ns)              # rows [0,B) = s, [B,2B) = s'
                 main.wait_event(done_tg)
         with torch.no_grad():
+            # what the statistics read besides the losses: C51's projected m, or the quantile loss's target rows T
             m = torch.empty((B, self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
-            if (M, K) == (1, 1):
+            if self.quantile:   # M = K = 1 (Agent refuses the copies)
+                loss, dz = qr_dueling_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
+                                                weights, self.quantile_kappa, self._gamma_n(), theta_out=m)
+            elif (M, K) == (1, 1):
                 loss, dz = c51_dueling_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
                                                  weights, self.support, self.Vmin, self.Vmax, self.delta_z,
                                                  self._gamma_n(), m_out=m)
@@ -834,8 +905,12 @@ class Agent:
                 self.target_net.reset_noise(*target_noise)
             q_t = self.target_net.logits(next_states)
             m = torch.empty((q_s.shape[0], self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
-            loss, grad = c51_loss_grad(q_s.detach(), q_ns, q_t, actions, returns, nonterminals, weights, self.support,
-                                       self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m)
+            if self.quantile:
+                loss, grad = qr_loss_grad(q_s.detach(), q_ns, q_t, actions, returns, nonterminals, weights,
+                                          self.quantile_kappa, self._gamma_n(), theta_out=m)
+            else:
+                loss, grad = c51_loss_grad(q_s.detach(), q_ns, q_t, actions, returns, nonterminals, weights, self.support,
+                                           self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m)
             stats_done = self._stats_batch(batch, loss, m, q=q_s.detach()) if m is not None else None
         self.optimiser.zero_grad()
         q_s.backward(grad)
@@ -1133,16 +1208,23 @@ class Agent:
 
     def _stats_batch(self, batch, loss, m, z=None, q=None):
         """rb_learn_stats_batch on a side stream as soon as the losses exist: it runs beside the backward.  Returns the
-        event _stats_write waits for.  The inputs of the latest record stay reachable in self._stats["last"]."""
+        event _stats_write waits for.  The inputs of the latest record stay reachable in self._stats["last"].  `m`: C51's
+        projected m, or under the quantile distribution the loss kernel's target rows T (rb_learn_stats_batch_qr)."""
         main = torch.cuda.current_stream(self.device)
         side = self._side_streams()[0]
         ready = torch.cuda.Event()
         ready.record(main)
         with torch.cuda.stream(side):
             side.wait_event(ready)
-            _lib.check(_lib.load().rb_learn_stats_batch(
-                _lib.ptr(loss), _lib.ptr(batch[6]), _lib.ptr(batch[2]), _lib.ptr(m), _lib.ptr(self.support), _lib.ptr(z),
-                _lib.ptr(q), loss.shape[0], self.action_space, self.atoms, _lib.ptr(self._stats["scratch"]), _lib.stream()))
+            if self.quantile:
+                _lib.check(_lib.load().rb_learn_stats_batch_qr(
+                    _lib.ptr(loss), _lib.ptr(batch[6]), _lib.ptr(batch[2]), _lib.ptr(m), _lib.ptr(z), _lib.ptr(q),
+                    loss.shape[0], self.action_space, self.atoms, _lib.ptr(self._stats["scratch"]), _lib.stream()))
+            else:
+                _lib.check(_lib.load().rb_learn_stats_batch(
+                    _lib.ptr(loss), _lib.ptr(batch[6]), _lib.ptr(batch[2]), _lib.ptr(m), _lib.ptr(self.support),
+                    _lib.ptr(z), _lib.ptr(q), loss.shape[0], self.action_space, self.atoms,
+                    _lib.ptr(self._stats["scratch"]), _lib.stream()))
             done = torch.cuda.Event()
             done.record(side)
         self._stats["last"] = dict(m=m, z=z, q=q)

@@ -373,6 +373,8 @@ def _meta(agent, mem):
         hyper["redo_interval"] = agent.redo_interval
     if agent.redo_tau != 0.1:
         hyper["redo_tau"] = agent.redo_tau
+    if agent.quantile:   # absent: categorical
+        hyper["distribution"], hyper["quantile_kappa"] = agent.distribution, agent.quantile_kappa
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
         learner["redo_count"] = agent.redo_count
     if opt.grouped:   # the group optimiser's bias-correction counts, [encoder, head]
@@ -509,6 +511,10 @@ def _validate(agent, mem, man):
     for key in want:
         if have.get(key) != want[key]:
             raise _Error(f"{key} differs: checkpoint {have.get(key)}, live {want[key]}")
+    # the parameter shapes are the same under both losses: without this a C51 net would load as quantiles, or back
+    dist = (man.get("hyper_parameters") or {}).get("distribution", "categorical")
+    if dist != agent.distribution:
+        raise _Error(f"distribution differs: checkpoint {dist!r}, live {agent.distribution!r}")
     layout = agent.optimiser.state_dict(clone=False)["layout"]
     if man.get("optimiser") != layout:
         raise _Error(f"optimiser layout differs: checkpoint {man.get('optimiser')}, this learner {layout}")

@@ -1566,6 +1566,276 @@ k_q_select(const float* __restrict__ z, int M, int A, int Z, const float* __rest
 }
 
 // ================================================================================================
+// Quantile regression (QR-DQN, Dabney et al. 2018): loss, gradient and the mean-quantile greedy values.
+// ================================================================================================
+// N quantiles per action at the midpoints tau_i = (2i + 1) / (2N).  For sample b with taken action a:
+//   theta_i = q_online(s, a)_i,  a* = argmax_a mean_j q_online(s', a)_j (first maximum wins),
+//   T_j = r + fl32(nt gamma_n) q_target(s', a*)_j,  u_ij = T_j - theta_i,
+//   loss = sum_i (1/N) sum_j |tau_i - [u_ij < 0]| H_kappa(u_ij) / kappa       (also the priority),
+//   g_i  = -(w / B) (1/N) sum_j |tau_i - [u_ij < 0]| clamp(u_ij, -kappa, kappa) / kappa.
+// One CTA of QR_T threads per sample (k_qr_dueling on the fused heads' z rows, k_qr on plain [B][A][N] rows):
+//   phase 1  warp a: the mean quantile of action a of online(s') (lane owns quantiles lane + 32 r) into s_mean[a];
+//   phase 2  a* (every thread runs the same scan of s_mean), then the rows theta and T into shared memory;
+//   phase 3  warp w takes the online quantiles i = w, w + 8, ...: each lane sums its R target quantiles, two interleaved
+//            butterflies finish sum_j; the loss sum of row i and g_i land in shared memory (qr_core);
+//   phase 4  warp 0 sums the rows' loss sums in i order; all threads write the gradient rows.
+// Every sum runs in a fixed order: an eager launch and a graph replay agree bitwise.
+constexpr int QR_T = 256;
+constexpr int QR_WARPS = QR_T / 32;
+
+// mean of one row held as x[r] = quantile lane + 32 r (0 past N); every lane returns it
+template <int R>
+__device__ __forceinline__ float qr_row_mean(const float (&x)[R], int N) {
+  float s = 0.0f;
+#pragma unroll
+  for (int r = 0; r < R; ++r) s = __fadd_rn(s, x[r]);
+  return __fdiv_rn(warp_sum(s), (float)N);
+}
+
+__device__ __forceinline__ int qr_argmax(const float* s_mean, int A) {
+  int best = 0;
+  float best_q = -CUDART_INF_F;
+  for (int a = 0; a < A; ++a) {
+    const float q = s_mean[a];
+    if (q > best_q) {  // first maximum wins, like torch.argmax
+      best_q = q;
+      best = a;
+    }
+  }
+  return best;
+}
+
+// Phases 3 and 4 (without the gradient write) from the rows s_theta, s_T [N] in shared memory: s_g [N] receives the
+// gradient row of the taken action, loss[i_sample] the loss; s_l is N floats of scratch.  s_g is complete on return.
+template <int R>
+__device__ __forceinline__ void qr_core(const float* s_theta, const float* s_T, float* s_l, float* s_g, int N, float kappa,
+                                        float wi, int i_sample, float* __restrict__ loss) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  float t[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) t[r] = (lane + 32 * r < N) ? s_T[lane + 32 * r] : 0.0f;
+  const float nk = __fmul_rn((float)N, kappa), half_k = 0.5f * kappa;
+  for (int i = warp; i < N; i += QR_WARPS) {
+    const float th = s_theta[i];
+    const float tau_lo = __fdiv_rn((float)(2 * i + 1), (float)(2 * N));        // |tau_i - 0|
+    const float tau_hi = __fdiv_rn((float)(2 * (N - i) - 1), (float)(2 * N));  // |tau_i - 1|
+    float sl = 0.0f, sg = 0.0f;
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      if (lane + 32 * r < N) {
+        const float u = __fsub_rn(t[r], th), au = fabsf(u);
+        const float tw = u < 0.0f ? tau_hi : tau_lo;
+        const float h = au <= kappa ? __fmul_rn(__fmul_rn(0.5f, u), u) : __fmul_rn(kappa, __fsub_rn(au, half_k));
+        sl = __fadd_rn(sl, __fmul_rn(tw, h));
+        sg = __fadd_rn(sg, __fmul_rn(tw, fminf(fmaxf(u, -kappa), kappa)));
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      sl = __fadd_rn(sl, __shfl_xor_sync(0xffffffffu, sl, o));
+      sg = __fadd_rn(sg, __shfl_xor_sync(0xffffffffu, sg, o));
+    }
+    if (lane == 0) {
+      s_l[i] = sl;
+      s_g[i] = -__fmul_rn(wi, __fdiv_rn(sg, nk));
+    }
+  }
+  __syncthreads();
+  if (warp == 0) {
+    float s = 0.0f;
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+      if (lane + 32 * r < N) s = __fadd_rn(s, s_l[lane + 32 * r]);
+    s = warp_sum(s);
+    if (lane == 0) loss[i_sample] = __fdiv_rn(s, nk);
+  }
+}
+
+// Dueling entry point: z rows as k_c51_dueling takes them (online 2B rows, s then s'; target B rows).
+template <int R>
+__global__ void __launch_bounds__(QR_T)
+k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
+             const float* __restrict__ returns, const float* __restrict__ nonterminals, const float* __restrict__ weights,
+             float kappa, float gamma_n, int B, int A, int N, float* __restrict__ loss, float* __restrict__ dz,
+             float* __restrict__ theta_out, int64_t* __restrict__ astar_out) {
+  extern __shared__ __align__(16) float s_dyn[];
+  const int N2 = N + A * N;
+  float* zs = s_dyn;              // [3][N2]: online(s), online(s'), target(s')
+  float* s_theta = zs + 3 * N2;   // [N] online quantiles of the taken action
+  float* s_T = s_theta + N;       // [N] target quantiles T_j
+  float* s_g = s_T + N;           // [N] gradient row
+  float* s_l = s_g + N;           // [N] loss sum of every online quantile
+  float* s_mean = s_l + N;        // [A] mean quantile of every action of online(s')
+  const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  {  // phase 0: k_c51_dueling's staging
+    const int total = 3 * N2;
+    const float* src[3] = {z_on + (size_t)i * N2, z_on + (size_t)(B + i) * N2, z_tg + (size_t)i * N2};
+    for (int base = tid; base < total; base += QR_T * 8) {
+      float v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int idx = base + u * QR_T;
+        v[u] = 0.0f;
+        if (idx < total) {
+          const int t = idx / N2;
+          v[u] = __ldg(src[t] + (idx - t * N2));
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int idx = base + u * QR_T;
+        if (idx < total) zs[idx] = v[u];
+      }
+    }
+  }
+  __syncthreads();
+  const int act = (int)actions[i];
+  {  // phase 1
+    const float* r1 = zs + N2;
+    float mean[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int c = lane + 32 * r;
+      float acc = 0.0f;
+      if (c < N)
+        for (int a = 0; a < A; ++a) acc += r1[N + a * N + c];
+      mean[r] = acc / (float)A;
+    }
+    for (int a = warp; a < A; a += QR_WARPS) {
+      float x[R];
+#pragma unroll
+      for (int r = 0; r < R; ++r) {
+        const int c = lane + 32 * r;
+        x[r] = (c < N) ? r1[c] + r1[N + a * N + c] - mean[r] : 0.0f;
+      }
+      const float q = qr_row_mean<R>(x, N);
+      if (lane == 0) s_mean[a] = q;
+    }
+  }
+  __syncthreads();
+  const int best = qr_argmax(s_mean, A);  // phase 2
+  if (astar_out && tid == 0) astar_out[i] = best;
+  const float ret = __ldg(returns + i), scale = __fmul_rn(__ldg(nonterminals + i), gamma_n);
+  for (int c = tid; c < N; c += QR_T) {
+    const float* r0 = zs;
+    const float* r2 = zs + 2 * N2;
+    float m0 = 0.0f, m2 = 0.0f;
+    for (int a = 0; a < A; ++a) {
+      m0 += r0[N + a * N + c];
+      m2 += r2[N + a * N + c];
+    }
+    s_theta[c] = r0[c] + r0[N + act * N + c] - m0 / (float)A;
+    const float T = __fadd_rn(ret, __fmul_rn(scale, r2[c] + r2[N + best * N + c] - m2 / (float)A));
+    s_T[c] = T;
+    if (theta_out) theta_out[(size_t)i * N + c] = T;
+  }
+  __syncthreads();
+  qr_core<R>(s_theta, s_T, s_l, s_g, N, kappa, __fdiv_rn(__ldg(weights + i), (float)B), i, loss);
+  {  // phase 4: dzv[c] = g[c], dza[a][c] = g[c] ([a == act] - 1/A), as k_c51_dueling
+    float* dzi = dz + (size_t)i * N2;
+    const float inv_a = 1.0f / (float)A;
+    for (int idx = tid; idx < N2; idx += QR_T) {
+      if (idx < N) {
+        dzi[idx] = s_g[idx];
+      } else {
+        const int a = (idx - N) / N, c = (idx - N) - a * N;
+        dzi[idx] = s_g[c] * ((a == act ? 1.0f : 0.0f) - inv_a);
+      }
+    }
+  }
+}
+
+// Plain entry point: quantile rows [B][A][N] of online(s), online(s') and target(s'); grad [B][A][N] is the gradient row
+// at the taken action and 0 elsewhere.
+template <int R>
+__global__ void __launch_bounds__(QR_T)
+k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
+     const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
+     const float* __restrict__ weights, float kappa, float gamma_n, int B, int A, int N, float* __restrict__ loss,
+     float* __restrict__ grad, float* __restrict__ theta_out, int64_t* __restrict__ astar_out) {
+  extern __shared__ __align__(16) float s_dyn[];
+  float* s_theta = s_dyn;
+  float* s_T = s_theta + N;
+  float* s_g = s_T + N;
+  float* s_l = s_g + N;
+  float* s_mean = s_l + N;        // [A]
+  const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const size_t row0 = (size_t)i * A;
+  for (int a = warp; a < A; a += QR_WARPS) {  // phase 1
+    float x[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int c = lane + 32 * r;
+      x[r] = (c < N) ? __ldg(q_on_ns + (row0 + a) * N + c) : 0.0f;
+    }
+    const float q = qr_row_mean<R>(x, N);
+    if (lane == 0) s_mean[a] = q;
+  }
+  __syncthreads();
+  const int act = (int)actions[i];
+  const int best = qr_argmax(s_mean, A);  // phase 2
+  if (astar_out && tid == 0) astar_out[i] = best;
+  const float ret = __ldg(returns + i), scale = __fmul_rn(__ldg(nonterminals + i), gamma_n);
+  for (int c = tid; c < N; c += QR_T) {
+    s_theta[c] = __ldg(q_on_s + (row0 + act) * N + c);
+    const float T = __fadd_rn(ret, __fmul_rn(scale, __ldg(q_tg_ns + (row0 + best) * N + c)));
+    s_T[c] = T;
+    if (theta_out) theta_out[(size_t)i * N + c] = T;
+  }
+  __syncthreads();
+  qr_core<R>(s_theta, s_T, s_l, s_g, N, kappa, __fdiv_rn(__ldg(weights + i), (float)B), i, loss);
+  float* gq = grad + row0 * N;
+  for (int idx = tid; idx < A * N; idx += QR_T) {
+    const int a = idx / N;
+    gq[idx] = (a == act) ? s_g[idx - a * N] : 0.0f;
+  }
+}
+
+// Greedy values for acting / evaluation under quantiles: k_q_select with the mean over quantiles in place of
+// softmax . support.  One warp per state; the dueling combination and the mean are k_qr_dueling's phase 1, bitwise.
+__global__ void __launch_bounds__(128)
+k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict__ q_out, int64_t* __restrict__ best_action,
+            float* __restrict__ best_q) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m = blockIdx.x * 4 + warp;
+  if (m >= M) return;
+  const float* zr = z + (size_t)m * (N + A * N);
+  constexpr int R = RB_MAX_ATOMS / 32;
+  float zv[R], mean[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const int c = lane + 32 * r;
+    zv[r] = mean[r] = 0.0f;
+    if (c < N) {
+      zv[r] = __ldg(zr + c);
+      float acc = 0.0f;
+      for (int a = 0; a < A; ++a) acc += __ldg(zr + N + a * N + c);
+      mean[r] = acc / (float)A;
+    }
+  }
+  int best = 0;
+  float best_v = -CUDART_INF_F;
+  for (int a = 0; a < A; ++a) {
+    float x[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int c = lane + 32 * r;
+      x[r] = (c < N) ? zv[r] + __ldg(zr + N + a * N + c) - mean[r] : 0.0f;
+    }
+    const float q = qr_row_mean<R>(x, N);
+    if (q_out && lane == 0) q_out[(size_t)m * A + a] = q;
+    if (q > best_v) {   // first maximum wins, like torch.argmax / max
+      best_v = q;
+      best = a;
+    }
+  }
+  if (lane == 0) {
+    if (best_action) best_action[m] = best;
+    if (best_q) best_q[m] = best_v;
+  }
+}
+
+// ================================================================================================
 // Learner statistics (agent.py:66-98 computes most of them and discards them): one record per update into a device ring.
 // ================================================================================================
 // Two launches, so that only a one-thread kernel has to wait for the optimiser step:
@@ -1626,6 +1896,50 @@ __device__ __forceinline__ void stats_combine(const double (&s_part)[7][STATS_WA
   }
 }
 
+// The CTA's accumulators v -> its partial slot; the last CTA reduces the partials in CTA order into scratch[0, 7).
+// no_edge: scratch[4] (edge_mass) is NaN.
+__device__ __forceinline__ void stats_finish(double (&s_part)[7][STATS_WARPS], bool& s_last, const double (&v)[7], int B,
+                                             double* __restrict__ scratch, bool no_edge) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  stats_store(s_part, v, warp, lane);
+  __syncthreads();
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(scratch + STATS_SCRATCH - 1);
+  if (tid == 0) {
+    double t[7];
+    stats_combine(s_part, t);
+    double* part = scratch + STATS_PART + STATS_PART * blockIdx.x;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) part[k] = t[k];
+    __threadfence();
+    s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  double p[7] = {0.0, 0.0, 0.0, 0.0, 0.0, -CUDART_INF, CUDART_INF};
+  if (tid < (int)gridDim.x) {
+    const double* part = scratch + STATS_PART + STATS_PART * tid;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) p[k] = __ldcg(part + k);
+  }
+#pragma unroll
+  for (int k = 0; k < 5; ++k) p[k] = warp_sum_f64(p[k]);
+  p[5] = warp_max_f64(p[5]);
+  p[6] = warp_min_f64(p[6]);
+  stats_store(s_part, p, warp, lane);
+  __syncthreads();
+  if (tid == 0) {
+    double t[7];
+    stats_combine(s_part, t);
+#pragma unroll
+    for (int k = 0; k < 5; ++k) scratch[k] = (double)(float)(t[k] / B);   // loss_mean, objective, q_mean, target_mean, edge_mass
+    if (no_edge) scratch[4] = CUDART_NAN;
+    scratch[5] = t[5];                                                    // loss_max
+    scratch[6] = t[6];                                                    // weight_min
+    *ticket = 0u;
+  }
+}
+
 __global__ void __launch_bounds__(STATS_THREADS)
 k_learn_stats_batch(const float* __restrict__ loss, const float* __restrict__ weights, const int64_t* __restrict__ actions,
                     const float* __restrict__ m, const float* __restrict__ support, const float* __restrict__ z,
@@ -1676,42 +1990,52 @@ k_learn_stats_batch(const float* __restrict__ loss, const float* __restrict__ we
     v[5] = fmax(v[5], (double)l);
     v[6] = fmin(v[6], (double)w);
   }
-  stats_store(s_part, v, warp, lane);
-  __syncthreads();
-  unsigned int* ticket = reinterpret_cast<unsigned int*>(scratch + STATS_SCRATCH - 1);
-  if (tid == 0) {
-    double t[7];
-    stats_combine(s_part, t);
-    double* part = scratch + STATS_PART + STATS_PART * blockIdx.x;
+  stats_finish(s_part, s_last, v, B, scratch, false);
+}
+
+// k_learn_stats_batch for the quantile loss: theta = the T rows [B][N] of the loss kernel (theta_out); per sample
+// q(s, a) = mean_i theta_i of the online quantiles of the taken action (dueling combination as k_qr_dueling forms it) and
+// the target value mean_j T_j; edge_mass is NaN (there is no support to clamp to).
+__global__ void __launch_bounds__(STATS_THREADS)
+k_learn_stats_batch_qr(const float* __restrict__ loss, const float* __restrict__ weights, const int64_t* __restrict__ actions,
+                       const float* __restrict__ theta, const float* __restrict__ z, const float* __restrict__ q, int B, int A,
+                       int N, double* __restrict__ scratch) {
+  __shared__ double s_part[7][STATS_WARPS];
+  __shared__ bool s_last;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  constexpr int R = RB_MAX_ATOMS / 32;
+  double v[7] = {0.0, 0.0, 0.0, 0.0, 0.0, -CUDART_INF, CUDART_INF};
+  const int warps = gridDim.x * STATS_WARPS;
+  for (int i = blockIdx.x * STATS_WARPS + warp; i < B; i += warps) {
+    const int act = (int)actions[i];
+    const float* tr = theta + (size_t)i * N;
+    const float l = __ldg(loss + i), w = __ldg(weights + i);
+    float t[R], x[R];
 #pragma unroll
-    for (int k = 0; k < 7; ++k) part[k] = t[k];
-    __threadfence();
-    s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    for (int r = 0; r < R; ++r) {
+      const int c = lane + 32 * r;
+      t[r] = (c < N) ? __ldg(tr + c) : 0.0f;
+      x[r] = 0.0f;
+      if (c < N) {
+        if (z) {
+          const float* zr = z + (size_t)i * (N + A * N);
+          float mean = 0.0f;
+          for (int a = 0; a < A; ++a) mean += __ldg(zr + N + a * N + c);
+          x[r] = __ldg(zr + c) + __ldg(zr + N + act * N + c) - mean / (float)A;
+        } else {
+          x[r] = __ldg(q + ((size_t)i * A + act) * N + c);
+        }
+      }
+    }
+    const float qv = qr_row_mean<R>(x, N), tv = qr_row_mean<R>(t, N);
+    v[0] += (double)l;
+    v[1] += (double)w * (double)l;
+    v[2] += (double)qv;
+    v[3] += (double)tv;
+    v[5] = fmax(v[5], (double)l);
+    v[6] = fmin(v[6], (double)w);
   }
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  double p[7] = {0.0, 0.0, 0.0, 0.0, 0.0, -CUDART_INF, CUDART_INF};
-  if (tid < (int)gridDim.x) {
-    const double* part = scratch + STATS_PART + STATS_PART * tid;
-#pragma unroll
-    for (int k = 0; k < 7; ++k) p[k] = __ldcg(part + k);
-  }
-#pragma unroll
-  for (int k = 0; k < 5; ++k) p[k] = warp_sum_f64(p[k]);
-  p[5] = warp_max_f64(p[5]);
-  p[6] = warp_min_f64(p[6]);
-  stats_store(s_part, p, warp, lane);
-  __syncthreads();
-  if (tid == 0) {
-    double t[7];
-    stats_combine(s_part, t);
-#pragma unroll
-    for (int k = 0; k < 5; ++k) scratch[k] = (double)(float)(t[k] / B);   // loss_mean, objective, q_mean, target_mean, edge_mass
-    scratch[5] = t[5];                                                    // loss_max
-    scratch[6] = t[6];                                                    // weight_min
-    *ticket = 0u;
-  }
+  stats_finish(s_part, s_last, v, B, scratch, true);
 }
 
 __global__ void k_learn_stats_record(const double* __restrict__ scratch, const float* __restrict__ grad_norm,
@@ -2663,6 +2987,84 @@ int rb_q_values(const float* z, int M, int actions, int atoms, const float* supp
   return check_launch("rb_q_values");
 }
 
+static int qr_check(const char* name, int B, int A, int N, float kappa) {
+  char msg[128];
+  if (B <= 0 || A <= 0 || N <= 1) {
+    snprintf(msg, sizeof msg, "%s: B, actions > 0 and atoms > 1 are required", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (N > RB_MAX_ATOMS) {
+    snprintf(msg, sizeof msg, "%s: atoms exceeds RB_MAX_ATOMS", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  if (!(kappa > 0.0f) || !isfinite(kappa)) {
+    snprintf(msg, sizeof msg, "%s: kappa must be finite and > 0", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  return RB_OK;
+}
+
+int rb_qr_dueling_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
+                            const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
+                            int B, float* loss, float* dz, float* theta_out, int64_t* astar_out, rb_stream_t stream) {
+  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !loss || !dz)
+    return fail(RB_ERR_INVAL, "rb_qr_dueling_loss_grad: null pointer");
+  const int N = atoms, A = actions_n;
+  int rc = qr_check("rb_qr_dueling_loss_grad", B, A, N, kappa);
+  if (rc != RB_OK) return rc;
+  const size_t smem = (size_t)(3 * (N + A * N) + 4 * N + A) * sizeof(float);
+  if (smem > 200 * 1024) return fail(RB_ERR_RANGE, "rb_qr_dueling_loss_grad: actions * atoms too large");
+  rc = rbi::ensure_dynamic_smem(k_qr_dueling<2>, smem, "rb_qr_dueling_loss_grad");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<4>, smem, "rb_qr_dueling_loss_grad");
+  if (rc != RB_OK) return rc;
+  { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
+    if (N <= 64)
+      k_qr_dueling<2><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights,
+                                                              kappa, gamma_n, B, A, N, loss, dz, theta_out, astar_out);
+    else
+      k_qr_dueling<4><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights,
+                                                              kappa, gamma_n, B, A, N, loss, dz, theta_out, astar_out); }
+  return check_launch("rb_qr_dueling_loss_grad");
+}
+
+int rb_qr_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                    const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n, int B,
+                    int A, int N, float* loss, float* grad_q_online_s, float* theta_out, int64_t* astar_out,
+                    rb_stream_t stream) {
+  if (!q_online_s || !q_online_ns || !q_target_ns || !actions || !returns || !nonterminals || !weights || !loss ||
+      !grad_q_online_s)
+    return fail(RB_ERR_INVAL, "rb_qr_loss_grad: null pointer");
+  int rc = qr_check("rb_qr_loss_grad", B, A, N, kappa);
+  if (rc != RB_OK) return rc;
+  const size_t smem = (size_t)(4 * N + A) * sizeof(float);
+  if (smem > 200 * 1024) return fail(RB_ERR_RANGE, "rb_qr_loss_grad: too many actions");
+  rc = rbi::ensure_dynamic_smem(k_qr<2>, smem, "rb_qr_loss_grad");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<4>, smem, "rb_qr_loss_grad");
+  if (rc != RB_OK) return rc;
+  { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
+    if (N <= 64)
+      k_qr<2><<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals,
+                                                      weights, kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out,
+                                                      astar_out);
+    else
+      k_qr<4><<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals,
+                                                      weights, kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out,
+                                                      astar_out); }
+  return check_launch("rb_qr_loss_grad");
+}
+
+int rb_qr_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
+                   rb_stream_t stream) {
+  if (!z) return fail(RB_ERR_INVAL, "rb_qr_q_values: null pointer");
+  if (!q && !best_action && !best_q) return fail(RB_ERR_INVAL, "rb_qr_q_values: no output requested");
+  if (M <= 0 || actions <= 0 || atoms <= 1)
+    return fail(RB_ERR_INVAL, "rb_qr_q_values: M, actions > 0 and atoms > 1 are required");
+  if (atoms > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_qr_q_values: atoms exceeds RB_MAX_ATOMS");
+  { ProfScope prof_(RB_K_Q_VALUES, (cudaStream_t)stream);
+    k_qr_select<<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, q, best_action, best_q); }
+  return check_launch("rb_qr_q_values");
+}
+
 static int stats_batch_check(const float* loss, const float* weights, const int64_t* actions, const float* m,
                              const float* support, const float* z, const float* q, int B, int A, int Z, const double* scratch) {
   if (!loss || !weights || !actions || !m || !support || !scratch) return fail(RB_ERR_INVAL, "rb_learn_stats: null pointer");
@@ -2691,6 +3093,20 @@ int rb_learn_stats_batch(const float* loss, const float* weights, const int64_t*
     k_learn_stats_batch<<<ctas, STATS_THREADS, 0, (cudaStream_t)stream>>>(loss, weights, actions, m, support, z, q, B, A, Z,
                                                                           scratch); }
   return check_launch("rb_learn_stats_batch");
+}
+
+int rb_learn_stats_batch_qr(const float* loss, const float* weights, const int64_t* actions, const float* theta, const float* z,
+                            const float* q, int B, int A, int N, double* scratch, rb_stream_t stream) {
+  if (!loss || !weights || !actions || !theta || !scratch) return fail(RB_ERR_INVAL, "rb_learn_stats_batch_qr: null pointer");
+  if ((z == nullptr) == (q == nullptr)) return fail(RB_ERR_INVAL, "rb_learn_stats_batch_qr: give exactly one of z and q");
+  if (B <= 0 || A <= 0 || N <= 1) return fail(RB_ERR_INVAL, "rb_learn_stats_batch_qr: B, A > 0 and N > 1 are required");
+  if (N > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_learn_stats_batch_qr: N exceeds RB_MAX_ATOMS");
+  int ctas = (B + STATS_WARPS - 1) / STATS_WARPS;
+  if (ctas > STATS_MAX_CTAS) ctas = STATS_MAX_CTAS;
+  { ProfScope prof_(RB_K_LEARN_STATS, (cudaStream_t)stream);
+    k_learn_stats_batch_qr<<<ctas, STATS_THREADS, 0, (cudaStream_t)stream>>>(loss, weights, actions, theta, z, q, B, A, N,
+                                                                             scratch); }
+  return check_launch("rb_learn_stats_batch_qr");
 }
 
 int rb_learn_stats_write(const double* scratch, const float* grad_norm, const int32_t* gate, float max_norm,

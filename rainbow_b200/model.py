@@ -196,7 +196,10 @@ class FusedHead:
 class DQN(nn.Module):
     def __init__(self, args, action_space):
         super().__init__()
+        from .agent import distribution_options
         self.atoms = args.atoms
+        # "quantile": the atoms outputs per stream are quantiles (QR-DQN); same layers, parameters and initialisation
+        self.quantile = distribution_options(args)[0] == "quantile"
         self.action_space = action_space
         self.hidden_size = args.hidden_size
         if args.architecture not in _ARCH:
@@ -424,5 +427,11 @@ class DQN(nn.Module):
         return v + a - a.mean(1, keepdim=True)
 
     def forward(self, x, log=False):
+        """Probabilities over the atoms [B, A, Z] (log=True: log-probabilities); under args.distribution = "quantile" the
+        quantiles [B, A, N] themselves, which have no log form."""
         q = self.logits(x)
+        if self.quantile:
+            if log:
+                raise ValueError("forward(x, log=True) is not defined for quantile outputs")
+            return q
         return F.log_softmax(q, dim=2) if log else F.softmax(q, dim=2)
