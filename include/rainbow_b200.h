@@ -339,7 +339,7 @@ int rb_q_values(const float* z, int M, int actions, int atoms, const float* supp
                 float* best_q, rb_stream_t stream);
 
 /* Bias gradient of a conv layer (the sum over batch and pixels torch computes in convolution_backward):
- * out[c] = sum_{b,p} grad_out[b][c][p], grad_out float32[B][C][HW] contiguous. */
+ * out[c] = sum_{b,p} grad_out[b][c][p], grad_out float32[B][C][HW] contiguous; B * HW < 2^31 - 256 (else RB_ERR_RANGE). */
 int rb_bias_grad(const float* grad_out, int B, int C, int HW, float* out, rb_stream_t stream);
 
 /* Weight gradient of a conv layer whose data gradient is not needed (the network's first layer; the weight half of
@@ -347,7 +347,9 @@ int rb_bias_grad(const float* grad_out, int B, int C, int HW, float* out, rb_str
  * for a square K x K kernel without padding (K in {3, 4, 5, 8}; IC * K * ceil(OC/4) <= 256).  grad_out float32
  * [B][OC][OH][OW], input float32 [B][IC][IH][IW] (OH = (IH-K)/stride + 1), out float32 [OC][IC][K][K] (overwritten),
  * bias_out (optional, may be NULL) float32 [OC] = sum_{b,y,x} grad_out (the layer's bias gradient, from the same pass),
- * partials: scratch of rb_conv_wgrad_scratch_elems(...) floats.  Two launches, fixed summation order (deterministic). */
+ * partials: scratch of rb_conv_wgrad_scratch_elems(...) floats.  Two launches, fixed summation order (deterministic).
+ * rb_conv_wgrad_scratch_elems returns 0 where the count does not fit in int, and rb_conv_wgrad refuses that B with
+ * RB_ERR_RANGE. */
 int rb_conv_wgrad_scratch_elems(int B, int IC, int IH, int OC, int K, int stride);
 int rb_conv_wgrad(const float* grad_out, const float* input, int B, int IC, int IH, int IW, int OC, int K, int stride,
                   float* partials, float* out, float* bias_out, rb_stream_t stream);

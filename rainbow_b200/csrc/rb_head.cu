@@ -1178,6 +1178,8 @@ k_conv_wgrad_first(const float* __restrict__ g, const float* __restrict__ in, in
 #pragma unroll
     for (int j = 0; j < KW; ++j) acc[i][j] = 0.0f;
   if (og * CW_OCT < OC) {
+    // OC % 4 != 0: the last group's channels past OC re-read channel OC - 1 (inside the slab); their sums are never stored
+    const int last = OC - 1 - og * CW_OCT;
     for (int yy = 0; yy < rows; ++yy) {
       const float* xrow = xs + ic * xs_ld + (yy * S + ky) * IW;
       const float* grow = gs + (og * CW_OCT) * (RB * OW) + yy * OW;
@@ -1194,7 +1196,7 @@ k_conv_wgrad_first(const float* __restrict__ g, const float* __restrict__ in, in
           for (int j = 0; j < KW; ++j) xv[j] = xrow[xx * S + j];
         }
 #pragma unroll
-        for (int i = 0; i < CW_OCT; ++i) gv[i] = grow[i * (RB * OW) + xx];
+        for (int i = 0; i < CW_OCT; ++i) gv[i] = grow[min(i, last) * (RB * OW) + xx];
 #pragma unroll
         for (int i = 0; i < CW_OCT; ++i)
 #pragma unroll
@@ -1485,6 +1487,8 @@ int rb_head_backward(const rb_head_params* p, const rb_head_grads* gr, const flo
 
 int rb_bias_grad(const float* grad_out, int B, int C, int HW, float* out, rb_stream_t stream) {
   if (!grad_out || !out || B <= 0 || C <= 0 || HW <= 0) return rbi::fail(RB_ERR_INVAL, "rb_bias_grad: bad argument");
+  if ((long long)B * HW > 0x7fffffffLL - 256)      // the kernel's int index i + 256 must not overflow
+    return rbi::fail(RB_ERR_RANGE, "rb_bias_grad: B * HW must stay below 2^31 - 256");
   {
     rbi::ProfScope prof_(RB_K_BIAS_GRAD, (cudaStream_t)stream);
     k_bias_grad<<<C, 256, 0, (cudaStream_t)stream>>>(grad_out, B, C, HW, out);
@@ -1497,7 +1501,8 @@ static int conv_wgrad_band_rows(int OH) { return OH >= 16 ? (OH + 7) / 8 : OH; }
 int rb_conv_wgrad_scratch_elems(int B, int IC, int IH, int OC, int K, int stride) {
   if (B <= 0 || IC <= 0 || OC <= 0 || K <= 0 || stride <= 0 || IH < K) return 0;
   const int OH = (IH - K) / stride + 1, RB = conv_wgrad_band_rows(OH), bands = (OH + RB - 1) / RB;
-  return B * bands * (OC * IC * K * K + OC);
+  const long long n = (long long)B * bands * ((long long)OC * IC * K * K + OC);
+  return n > 0x7fffffffLL ? 0 : (int)n;   // a count past int: 0, and rb_conv_wgrad refuses the shape
 }
 
 int rb_conv_wgrad(const float* grad_out, const float* input, int B, int IC, int IH, int IW, int OC, int K, int stride,
@@ -1509,6 +1514,8 @@ int rb_conv_wgrad(const float* grad_out, const float* input, int B, int IC, int 
   const int RB = conv_wgrad_band_rows(OH), bands = (OH + RB - 1) / RB;
   const int threads = IC * K * ((OC + CW_OCT - 1) / CW_OCT);
   if (threads > 256 || B > 65535) return rbi::fail(RB_ERR_RANGE, "rb_conv_wgrad: IC * K * ceil(OC / 4) must not exceed 256 threads");
+  if (rb_conv_wgrad_scratch_elems(B, IC, IH, OC, K, stride) == 0)
+    return rbi::fail(RB_ERR_RANGE, "rb_conv_wgrad: the partials of B samples exceed 2^31 - 1 floats");
   const size_t smem = ((size_t)IC * ((RB - 1) * stride + K) * IW + (size_t)OC * RB * OW) * sizeof(float);
   if (smem > 200 * 1024) return rbi::fail(RB_ERR_RANGE, "rb_conv_wgrad: slab does not fit in shared memory");
   cudaStream_t st = (cudaStream_t)stream;

@@ -61,7 +61,7 @@ def test_abi_argument_validation_without_gpu():
     assert lib.rb_conv_wgrad(one, None, 32, 4, 84, 84, 32, 8, 4, one, one, None, None) == -22
     assert lib.rb_conv_wgrad_scratch_elems(32, 4, 84, 32, 8, 4) == 32 * 7 * (32 * 4 * 8 * 8 + 32)   # 20 output rows in 7 bands of 3
     assert lib.rb_conv_wgrad_scratch_elems(32, 4, 4, 32, 8, 4) == 0
-    two = (C.c_void_p * 2)(8, 8)
+    two =(C.c_void_p * 2)(8, 8)
     assert lib.rb_peer_reduce(two, two, 2, 0, 2, 0, 64, 0.5, one, one, one, None) == -34            # segment id
     assert lib.rb_peer_reduce(two, two, 2, 0, 0, 0, 60, 0.5, one, one, one, None) == -22            # not a multiple of 4 * world
     assert lib.rb_peer_reduce(two, two, 2, 2, 0, 0, 64, 0.5, one, one, one, None) == -34            # rank >= world
@@ -100,6 +100,48 @@ def test_head_supported_without_gpu():
     assert lib.rb_head_supported(48, 256, 51, 6, 64, 0) == -34            # conv_features % 32
     assert lib.rb_head_supported(576, 256, 1, 6, 64, 0) == -22            # atoms > 1
     assert lib.rb_head_supported(576, 256, 51, 6, -1, 0) == -22
+
+
+def test_conv_wgrad_scratch_count_and_the_call_agree_past_int():
+    """The partial count B * bands * (OC IC K K + OC) of canonical layer 0 (7 bands of 8 224 floats) passes 2^31 - 1 at
+    B = 37 304: the size function returns 0 there instead of a wrapped count, and rb_conv_wgrad refuses the same B with
+    RB_ERR_RANGE before any launch (the B <= 65 535 grid limit alone would accept it)."""
+    from rainbow_b200 import _lib
+    lib = _lib.load()
+    one = C.c_void_p(8)                                 # never dereferenced: the refusal comes first
+    per = 7 * (32 * 4 * 8 * 8 + 32)
+    b_max = (2 ** 31 - 1) // per
+    assert b_max == 37303
+    assert lib.rb_conv_wgrad_scratch_elems(b_max, 4, 84, 32, 8, 4) == b_max * per
+    for B in (b_max + 1, 40000, 65535):
+        assert lib.rb_conv_wgrad_scratch_elems(B, 4, 84, 32, 8, 4) == 0
+        assert lib.rb_conv_wgrad(one, one, B, 4, 84, 84, 32, 8, 4, one, one, one, None) == -34
+        assert b"2^31" in lib.rb_last_error()
+    assert lib.rb_conv_wgrad(one, one, 65536, 4, 84, 84, 32, 8, 4, one, one, one, None) == -34
+    # data-efficient layer 0: 8 bands of 3 232 floats
+    per = 8 * (32 * 4 * 5 * 5 + 32)
+    assert lib.rb_conv_wgrad_scratch_elems((2 ** 31 - 1) // per, 4, 84, 32, 5, 5) == (2 ** 31 - 1) // per * per
+    assert lib.rb_conv_wgrad_scratch_elems((2 ** 31 - 1) // per + 1, 4, 84, 32, 5, 5) == 0
+    # the other refusals: kernel size, threads, shared memory, shape, pointers
+    assert lib.rb_conv_wgrad(one, one, 32, 5, 84, 84, 32, 8, 4, one, one, None, None) == -34        # 320 threads
+    assert lib.rb_conv_wgrad(one, one, 2, 2, 84, 8000, 32, 8, 4, one, one, None, None) == -34       # slab > 200 KB
+    assert lib.rb_conv_wgrad(one, one, 2, 4, 7, 84, 32, 8, 4, one, one, None, None) == -22          # IH < K
+    assert lib.rb_conv_wgrad(one, one, 2, 4, 84, 84, 32, 8, 0, one, one, None, None) == -22         # stride 0
+    assert lib.rb_conv_wgrad(one, one, 2, 4, 84, 84, 32, 8, 4, None, one, None, None) == -22        # no partials
+    assert lib.rb_conv_wgrad(one, one, 2, 4, 84, 84, 32, 8, 4, one, None, None, None) == -22        # no output
+
+
+def test_bias_grad_argument_validation_without_gpu():
+    from rainbow_b200 import _lib
+    lib = _lib.load()
+    one = C.c_void_p(8)
+    assert lib.rb_bias_grad(None, 32, 64, 81, one, None) == -22
+    assert lib.rb_bias_grad(one, 32, 64, 81, None, None) == -22
+    for B, Cc, HW in ((0, 64, 81), (32, 0, 81), (32, 64, 0), (-1, 64, 81)):
+        assert lib.rb_bias_grad(one, B, Cc, HW, one, None) == -22
+    assert lib.rb_bias_grad(one, 2 ** 16, 64, 2 ** 15, one, None) == -34                           # B HW = 2^31
+    assert lib.rb_bias_grad(one, 1, 64, 2 ** 31 - 256, one, None) == -34
+    assert b"2^31" in lib.rb_last_error()
 
 
 def test_no_cpu_fallback():

@@ -568,37 +568,6 @@ def test_fused_head_layer1_tensor_core(arch, hidden, actions, m_lo, m_hi):
     net.train()
 
 
-@pytest.mark.parametrize("B,IC,IH,OC,K,S", [(32, 4, 84, 32, 8, 4), (32, 4, 84, 32, 5, 5), (5, 4, 84, 32, 8, 4), (7, 3, 30, 16, 4, 2),
-                                            (2, 8, 13, 24, 3, 1), (64, 4, 84, 32, 8, 4)])
-def test_conv_wgrad_first_layer(B, IC, IH, OC, K, S):
-    """rb_conv_wgrad (the first conv layer's weight gradient, agent.py:96 backward) against torch's convolution_backward in
-    float64: fp32 accumulation over up to 25 600 terms per element -> within 2e-6 of the tensor's scale; deterministic."""
-    from rainbow_b200 import _lib
-    L = _lib.load()
-    torch.manual_seed(B + K)
-    x = torch.rand(B, IC, IH, IH, device=DEV)
-    OH = (IH - K) // S + 1
-    g = torch.randn(B, OC, OH, OH, device=DEV) * (torch.rand(B, OC, OH, OH, device=DEV) > 0.4)     # ReLU-masked gradient
-    w = torch.zeros(OC, IC, K, K, device=DEV)
-    _, ref, _ = torch.ops.aten.convolution_backward(g.double(), x.double(), w.double(), None, [S, S], [0, 0], [1, 1], False, [0, 0], 1,
-                                                    [False, True, False])
-    n = L.rb_conv_wgrad_scratch_elems(B, IC, IH, OC, K, S)
-    assert n > 0
-    scratch = torch.empty(n, device=DEV)
-    out = torch.full((OC, IC, K, K), 7.0, device=DEV)                  # must be overwritten
-    bias = torch.full((OC,), 7.0, device=DEV)
-    _lib.check(L.rb_conv_wgrad(g.data_ptr(), x.data_ptr(), B, IC, IH, IH, OC, K, S, scratch.data_ptr(), out.data_ptr(),
-                               bias.data_ptr(), torch.cuda.current_stream().cuda_stream))
-    scale = float(ref.abs().max())
-    np.testing.assert_allclose(cpu(out), cpu(ref), rtol=0, atol=2e-6 * scale)
-    bref = g.double().sum((0, 2, 3))
-    np.testing.assert_allclose(cpu(bias), cpu(bref), rtol=0, atol=2e-6 * float(bref.abs().max()))
-    out2 = torch.empty_like(out)
-    _lib.check(L.rb_conv_wgrad(g.data_ptr(), x.data_ptr(), B, IC, IH, IH, OC, K, S, scratch.data_ptr(), out2.data_ptr(),
-                               None, torch.cuda.current_stream().cuda_stream))
-    assert torch.equal(out, out2)
-
-
 def test_noise_factors_plus_outer_equals_resample():
     from rainbow_b200.model import resample_noise
     net = _head_net()

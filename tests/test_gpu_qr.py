@@ -20,6 +20,7 @@ import numpy as np
 import pytest
 import torch
 
+from conv_ref import conv_masks
 from helpers import assert_bits_equal
 from test_gpu_adamw import LEARNER_CASES
 from test_gpu_augment import update_graph
@@ -85,29 +86,6 @@ def _qr_objective(q_s, q_ns, q_t, actions, returns, nonterminals, weights, gamma
     return loss, (weights.double() * loss).sum() / B
 
 
-def _conv_masks(ag, ws, p_before):
-    """The ReLU sides (post-activation > 0) of every conv layer in the learner's own fp32 forward of the update's rows,
-    [s; s'], recomputed with the parameters before the update (the same cuDNN calls on the same rows, deterministic)."""
-    on, opt = ag.online_net, ag.optimiser
-    p_after = opt.flat_param.clone()
-    opt.flat_param.copy_(p_before)
-    with torch.no_grad():
-        if ag._fused_path(ws.B):
-            acts = on.conv_forward_saving(ws.both_states)[1:]
-        else:                                  # the library head runs the module chain on s and s' separately
-            acts = []
-            for x in (ws.states, ws.next_states):
-                outs = []
-                for m in on.convs:
-                    x = m(x)
-                    if isinstance(m, torch.nn.ReLU):
-                        outs.append(x)
-                acts.append(outs)
-            acts = [torch.cat(pair) for pair in zip(*acts)]
-    opt.flat_param.copy_(p_after)
-    return [(a > 0).double() for a in acts]
-
-
 def _f64_forward_masked(net, P, f, x, masks):
     """_f64_forward with each conv ReLU replaced by the fp32 forward's side: a pre-activation within rounding of zero can
     land on the other side in float64, and that one activation's gradient then shows in the conv gradients (DESIGN.md
@@ -147,7 +125,7 @@ def test_learner_gradient_is_f64_autograd(case):
         torch.cuda.synchronize()
         ws = mem._last
         B = ws.B
-        masks = _conv_masks(ag, ws, p_before)
+        masks = conv_masks(ag, ws, p_before)
         q_on = _f64_forward_masked(on, P, on.noise_factors(), ws.both_states.double(), masks)
         with torch.no_grad():
             q_t = _f64_forward(tg, T, tg.noise_factors(), ws.next_states.double())
