@@ -896,6 +896,11 @@ class Agent:
         if copies != (1, 1):
             raise self._copies_error(copies)
         idxs, states, actions, returns, next_states, nonterminals, weights = batch
+        # a deferred draw first: the rows of s (the library's NoisyLinear, which composes the epsilon buffers only when they
+        # are stale) and of s' (the fused head, which reads the factors) must see the same draw
+        self.online_net.flush_noise()
+        if torch.cuda.is_current_stream_capturing():
+            self.online_net._eps_stale = True    # the graph composes them from whatever draw precedes a replay
         q_s = self.online_net.logits(states)
         with torch.no_grad():
             q_ns = self.online_net.logits(next_states)

@@ -34,6 +34,7 @@ from helpers import assert_bits_equal
 from test_gpu_augment import GUARD, NAN, Outputs, episodic_memory, gather, update_graph
 from test_gpu_head_f64 import graph_kernels
 from test_gpu_parity import DEV, FakeEnv, cpu, make_args, synthetic_ring
+from update_ref import f64_forward, f64_projection
 
 pytestmark = pytest.mark.gpu
 
@@ -337,41 +338,6 @@ def test_identical_copies_equal_a_plain_agent():
 TOL = dict(loss=1e-5, grad_head=1e-6, grad_conv=2e-6, param_head=1e-7, param_conv=2e-7)
 
 
-def _f64_forward(net, P, f, x):
-    """q [rows][A][Z] of `net` in float64 from parameters P (name -> float64 tensor) and its noise factors f."""
-    for m, (wn, bn) in zip(net.conv_layers(), [(f"convs.{i}.weight", f"convs.{i}.bias") for i, c in enumerate(net.convs)
-                                              if isinstance(c, torch.nn.Conv2d)]):
-        x = torch.relu(torch.nn.functional.conv2d(x, P[wn], P[bn], m.stride, m.padding))
-    x = x.reshape(x.shape[0], -1)
-
-    def noisy(name, v):
-        fi, fo = (t.double() for t in f[name])
-        w = P[f"{name}.weight_mu"] + P[f"{name}.weight_sigma"] * torch.outer(fo, fi)
-        b = P[f"{name}.bias_mu"] + P[f"{name}.bias_sigma"] * fo
-        return torch.nn.functional.linear(v, w, b)
-
-    A, Z = net.action_space, net.atoms
-    v = noisy("fc_z_v", torch.relu(noisy("fc_h_v", x))).view(-1, 1, Z)
-    a = noisy("fc_z_a", torch.relu(noisy("fc_h_a", x))).view(-1, A, Z)
-    return v + a - a.mean(1, keepdim=True)
-
-
-def _f64_projection(ag, q_t, r, nt):
-    """m [B][Z] of softmax(q_t) with agent.py:79-92's arithmetic in float64 (fp32 arguments as the kernel gets them)."""
-    Z = ag.atoms
-    s = ag.support.double().unsqueeze(0)
-    vmin, vmax, dz, gn = (C.f32(v) for v in (ag.Vmin, ag.Vmax, ag.delta_z, ag.discount ** ag.n))
-    pt = torch.softmax(q_t, 1)
-    b = ((r.unsqueeze(1) + nt.view(-1, 1) * gn * s).clamp(vmin, vmax) - vmin) / dz
-    lo, up = b.floor(), b.ceil()
-    lo = torch.where((up > 0) & (lo == up), lo - 1, lo)
-    up = torch.where((lo < Z - 1) & (lo == up), up + 1, up)
-    m = torch.zeros(b.shape[0], Z + 1, dtype=torch.float64, device=b.device)
-    m.scatter_add_(1, lo.long(), pt * (up - b))
-    m.scatter_add_(1, up.long(), pt * (b - lo))
-    return m[:, :Z]
-
-
 def _f64_update(ag, ws, before, M, K):
     """The DrQ update in float64 over the update's own gathered rows: (loss [B], {name: grad}, flat parameters after
     clip + Adam)."""
@@ -379,16 +345,16 @@ def _f64_update(ag, ws, before, M, K):
     B = ws.B
     P = {n: t.double().requires_grad_() for n, t in before["online"].items()}
     T = {n: t.double() for n, t in before["target"].items()}
-    q_on = _f64_forward(on, P, on.noise_factors(), ws.both_states.double())
+    q_on = f64_forward(on, P, on.noise_factors(), ws.both_states.double())
     with torch.no_grad():
-        q_t = _f64_forward(tg, T, tg.noise_factors(), ws.next_states.double())
+        q_t = f64_forward(tg, T, tg.noise_factors(), ws.next_states.double())
         r, nt, w = ws.returns.double(), ws.nonterminals.double().view(-1), ws.weights.double()
         sup, rows = ag.support.double(), torch.arange(B, device=ws.actions.device)
         ms = []
         for k in range(K):
             q_ns = q_on[(M + k) * B:(M + k + 1) * B]
             best = (torch.softmax(q_ns, 2) * sup).sum(2).argmax(1)
-            ms.append(_f64_projection(ag, q_t[k * B:(k + 1) * B][rows, best], r, nt))
+            ms.append(f64_projection(ag, q_t[k * B:(k + 1) * B][rows, best], r, nt))
         m = sum(ms) / K
     loss = sum(-(m * torch.log_softmax(q_on[j * B:(j + 1) * B][rows, ws.actions], 1)).sum(1) for j in range(M)) / M
     ((w * loss).sum() / B).backward()

@@ -361,8 +361,8 @@ def _trajectory(graph, fused, pending, steps=7, stats=16):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("fused,pending", [(True, True), (True, False), (False, False)],
-                         ids=["fused-pending", "fused-flushed", "library-flushed"])
+@pytest.mark.parametrize("fused,pending", [(True, True), (True, False), (False, False), (False, True)],
+                         ids=["fused-pending", "fused-flushed", "library-flushed", "library-pending"])
 def test_graph_records_equal_eager_bitwise(fused, pending):
     old = torch.backends.cudnn.deterministic
     torch.backends.cudnn.deterministic = True
@@ -379,9 +379,8 @@ def test_graph_records_equal_eager_bitwise(fused, pending):
 
 @pytest.mark.gpu
 def test_library_pending_graph_records_match_its_updates():
-    """The library head with the online draw deferred into the update: here the graph replays and the eager updates
-    themselves do not agree bitwise (with the recording off as well, since it leaves the update unchanged), so each
-    record of the graph run is held to that run's own per-step losses."""
+    """The library head with the online draw deferred into the update: each record of the graph run is held to that run's
+    own per-step losses (test_graph_records_equal_eager_bitwise[library-pending] holds the run to an eager one)."""
     ag, mem = _agent(16, graph=True, fused=False), _memory()
     losses, norms = [], []
     for _ in range(7):

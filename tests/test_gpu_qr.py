@@ -24,8 +24,9 @@ from conv_ref import conv_masks
 from helpers import assert_bits_equal
 from test_gpu_adamw import LEARNER_CASES
 from test_gpu_augment import update_graph
-from test_gpu_drq import TOL, _f64_forward
+from test_gpu_drq import TOL
 from test_gpu_parity import DEV, FakeEnv, cpu, make_args, synthetic_ring
+from update_ref import f64_forward, f64_forward_masked, qr_objective
 
 pytestmark = pytest.mark.gpu
 
@@ -67,45 +68,6 @@ def _assert_snapshots(a, b, what):
         assert_bits_equal(a[k], b[k], f"{k} {what}")
 
 
-def _qr_objective(q_s, q_ns, q_t, actions, returns, nonterminals, weights, gamma_n, kappa):
-    """(per-sample loss, objective) of the quantile loss in float64 (differentiable in q_s); nonterminals enter only as
-    fl32(nt gamma_n), as in the kernels."""
-    B, _, N = q_s.shape
-    rows = torch.arange(B, device=q_s.device)
-    theta = q_s[rows, actions]
-    with torch.no_grad():
-        best = q_ns.mean(2).argmax(1)
-        sc = (nonterminals.view(-1).float() * torch.tensor(np.float32(gamma_n), device=q_s.device)).double()
-        T = returns.double().unsqueeze(1) + sc.unsqueeze(1) * q_t[rows, best]
-    u = T.unsqueeze(1) - theta.unsqueeze(2)
-    tau = (2.0 * torch.arange(N, dtype=torch.float64, device=q_s.device) + 1.0) / (2.0 * N)
-    tw = torch.where(u.detach() < 0, 1.0 - tau.view(1, N, 1), tau.view(1, N, 1))
-    au = u.abs()
-    H = torch.where(au <= kappa, 0.5 * u * u, kappa * (au - 0.5 * kappa))
-    loss = (tw * H).sum((1, 2)) / (N * kappa)
-    return loss, (weights.double() * loss).sum() / B
-
-
-def _f64_forward_masked(net, P, f, x, masks):
-    """_f64_forward with each conv ReLU replaced by the fp32 forward's side: a pre-activation within rounding of zero can
-    land on the other side in float64, and that one activation's gradient then shows in the conv gradients (DESIGN.md
-    §4); taking the learner's sides leaves only the arithmetic to compare."""
-    convs = [(f"convs.{i}.weight", f"convs.{i}.bias") for i, c in enumerate(net.convs) if isinstance(c, torch.nn.Conv2d)]
-    for m, (wn, bn), mask in zip(net.conv_layers(), convs, masks):
-        x = torch.nn.functional.conv2d(x, P[wn], P[bn], m.stride, m.padding) * mask
-    x = x.reshape(x.shape[0], -1)
-
-    def noisy(name, v):
-        fi, fo = (t.double() for t in f[name])
-        w = P[f"{name}.weight_mu"] + P[f"{name}.weight_sigma"] * torch.outer(fo, fi)
-        return torch.nn.functional.linear(v, w, P[f"{name}.bias_mu"] + P[f"{name}.bias_sigma"] * fo)
-
-    A, Z = net.action_space, net.atoms
-    v = noisy("fc_z_v", torch.relu(noisy("fc_h_v", x))).view(-1, 1, Z)
-    a = noisy("fc_z_a", torch.relu(noisy("fc_h_a", x))).view(-1, A, Z)
-    return v + a - a.mean(1, keepdim=True)
-
-
 # ---- one update against float64 autograd -----------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", list(LEARNER_CASES))
 def test_learner_gradient_is_f64_autograd(case):
@@ -126,10 +88,10 @@ def test_learner_gradient_is_f64_autograd(case):
         ws = mem._last
         B = ws.B
         masks = conv_masks(ag, ws, p_before)
-        q_on = _f64_forward_masked(on, P, on.noise_factors(), ws.both_states.double(), masks)
+        q_on = f64_forward_masked(on, P, on.noise_factors(), ws.both_states.double(), masks)
         with torch.no_grad():
-            q_t = _f64_forward(tg, T, tg.noise_factors(), ws.next_states.double())
-        loss, obj = _qr_objective(q_on[:B], q_on[B:].detach(), q_t, ws.actions, ws.returns, ws.nonterminals, ws.weights,
+            q_t = f64_forward(tg, T, tg.noise_factors(), ws.next_states.double())
+        loss, obj = qr_objective(q_on[:B], q_on[B:].detach(), q_t, ws.actions, ws.returns, ws.nonterminals, ws.weights,
                                   ag.discount ** ag.n, ag.quantile_kappa)
         obj.backward()
         assert float((ag.last_loss.double() - loss.detach()).abs().max()) <= TOL["loss"], f"loss, update {step}"
@@ -237,7 +199,7 @@ def test_acting_is_the_f64_mean_quantile_greedy():
         P = {n: p.detach().double() for n, p in on.named_parameters()}
         f = {n: (torch.zeros(m.in_features, device=DEV), torch.zeros(m.out_features, device=DEV))
              for n, m in on.named_children() if n.startswith("fc_")}
-        q = _f64_forward(on, P, f, states.double()).mean(2)              # [M][A] mean quantiles, float64
+        q = f64_forward(on, P, f, states.double()).mean(2)              # [M][A] mean quantiles, float64
     best_v, best_a = q.max(1)
     values = torch.tensor(ag.evaluate_q_memory(val), dtype=torch.float64, device=DEV)
     assert float((values - best_v).abs().max()) <= 1e-5 * float(best_v.abs().max() + 1)
