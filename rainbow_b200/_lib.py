@@ -195,6 +195,21 @@ def stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def side_branch(side, fn):
+    """Run fn() with `side` as the current stream, after everything enqueued so far on the current stream: a fork that
+    becomes a parallel branch inside a captured CUDA graph.  Returns (fn's result, an event recorded on `side` after it);
+    whoever needs the branch's work joins with current_stream().wait_event(event)."""
+    import torch
+    ready = torch.cuda.Event()
+    ready.record(torch.cuda.current_stream(side.device))
+    with torch.cuda.stream(side):
+        side.wait_event(ready)
+        out = fn()
+        done = torch.cuda.Event()
+        done.record(side)
+    return out, done
+
+
 # Every kernel id, indexed by its value in the RB_K_* enum of include/rainbow_b200.h (RB_K_FOO -> "foo"); a host test checks
 # this list against the enum, names, order and RB_KERNEL_COUNT.  A new kernel goes at the end of this one list.
 ALL_KERNEL_IDS = ["tree_update", "tree_find", "tree_sample", "gather", "iter_states", "append", "c51", "noisy_resample",

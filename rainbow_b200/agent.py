@@ -571,7 +571,6 @@ class Agent:
 
         self.use_cuda_graph = bool(getattr(args, "cuda_graph", True))
         self.use_fused_head = bool(getattr(args, "fused_head", True))
-        self.batch_online_convs = bool(getattr(args, "batch_online_convs", True))
         self._step_gate = None
         self._streams = None
         self._graphs = {}         # online-noise-pending flag -> (captured update graph, its sample workspace, its loss tensor)
@@ -640,11 +639,7 @@ class Agent:
         if not self.use_cuda_graph:
             run()
         elif g["graph"] is None and g["warm"] < 2:
-            side = torch.cuda.Stream(device=self.device)
-            side.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(side):
-                run()
-            torch.cuda.current_stream(self.device).wait_stream(side)
+            self._warm_up(run)
             g["warm"] += 1
         else:
             if g["graph"] is None:
@@ -738,150 +733,103 @@ class Agent:
             self._streams = (torch.cuda.Stream(device=self.device), torch.cuda.Stream(device=self.device))
         return self._streams
 
+    def _warm_up(self, fn):
+        """torch's warm-up recipe before a whole-step capture: fn() eagerly on a fresh side stream, joined at once."""
+        out, done = _lib.side_branch(torch.cuda.Stream(device=self.device), fn)
+        torch.cuda.current_stream(self.device).wait_event(done)
+        return out
+
     def _update_fused(self, batch, target_noise=None, after_loss=None):
-        """agent.py:66-98 with the fused head: torch only runs the conv bodies (forward x3, backward x1).
-        The three network passes are independent until the loss, and every conv kernel of this size leaves most of the
-        132 SMs of an H100 idle, so they run as three concurrent branches (fork/join with events; inside the captured CUDA graph
-        they become parallel branches): online(s) with autograd on the caller's stream, online(s') and the whole
-        target pass (noise draw, convs, head) on two side streams.
+        """agent.py:66-98 with the fused head: torch only runs the conv bodies (forward, and one backward).
+        The network passes are independent until the loss, and every conv kernel of this size leaves most of the
+        132 SMs of an H100 idle, so they run as concurrent branches (fork/join with events; inside the captured CUDA graph
+        they become parallel branches): the whole target pass (noise draw, convs, head) on a side stream, and online(s)
+        with the gradient on the caller's stream -- together with online(s') in one conv pass when the sampler laid the
+        two state blocks out back to back, else with online(s') on a second side stream.
         DrQ's K / M: `states` may hold M copies of the B sampled states and `next_states` K copies of the next states
         (copy-major); the online pass then runs over all (M + K) B rows, the target pass over K B rows, and the backward
         over the M B rows of s."""
-        idxs, states, actions, returns, next_states, nonterminals, weights = batch
+        states, next_states = batch[1], batch[4]
         on, tg = self.online_net, self.target_net
-        B = actions.shape[0]
-        Bs = states.shape[0]                 # M B rows of s
-        M, K = Bs // B, next_states.shape[0] // B
+        B, Bs, Bn = batch[2].shape[0], states.shape[0], next_states.shape[0]      # Bs = M B rows of s, Bn = K B of s'
         main = torch.cuda.current_stream(self.device)
         s_ns, s_tg = self._side_streams()
-        fork = torch.cuda.Event()
-        fork.record(main)
         noise_done = None
         if on._noise_pending:   # the online net's deferred reset_noise(): beside the sampling / conv work, not in front of it
-            with torch.cuda.stream(s_ns):
-                s_ns.wait_event(fork)
-                on.flush_noise()
-                noise_done = torch.cuda.Event()
-                noise_done.record(s_ns)
-        with torch.cuda.stream(s_tg), torch.no_grad():
-            s_tg.wait_event(fork)
-            if target_noise is None:
-                tg.reset_noise()                                            # agent.py:74
-            else:
-                tg.reset_noise(*target_noise)
-            x_t = tg.features_nograd(next_states)
-            z_t, _, _ = tg.head().forward(x_t)
-            done_tg = torch.cuda.Event()
-            done_tg.record(s_tg)
+            noise_done = _lib.side_branch(s_ns, on.flush_noise)[1]
+
+        def target_pass():
+            tg.reset_noise(*(target_noise or ()))                          # agent.py:74
+            return tg.head().forward(tg.features_nograd(next_states))[0]
+        with torch.no_grad():
+            z_t, done_tg = _lib.side_branch(s_tg, target_pass)
         manual = on.manual_conv_ok(states)
         # [s; s'] in ONE conv pass when the sampler laid both state blocks out back to back (ReplayMemory's workspaces do):
         # the online net's weights stream once, and two concurrent conv chains (online, target) share the SMs instead of three
-        both = self._adjacent(states, next_states) if (manual and self.batch_online_convs) else None
+        both = self._adjacent(states, next_states) if manual else None
         if both is not None:
             with torch.no_grad():
                 acts2 = on.conv_forward_saving(both)
-                acts = [a[:Bs] for a in acts2]             # the s rows (batch-major: contiguous slices) feed the backward
-                x_both = acts2[-1].view(Bs + next_states.shape[0], -1)
-                x_s, xs_d = x_both[:Bs], x_both[:Bs]
-                if noise_done is not None:
-                    main.wait_event(noise_done)
-                z_on, h_on, p_on = on.head().forward(x_both)              # rows [0,B) = s, [B,2B) = s'
-                main.wait_event(done_tg)
+            acts = [a[:Bs] for a in acts2]                 # the s rows (batch-major: contiguous slices) feed the backward
+            x_both = acts2[-1].view(Bs + Bn, -1)
+            x_s = xs_d = x_both[:Bs]
+            head_in = (x_both,)
         else:
-            with torch.cuda.stream(s_ns), torch.no_grad():
-                s_ns.wait_event(fork)
-                x_ns = on.features_nograd(next_states)
-                done_ns = torch.cuda.Event()
-                done_ns.record(s_ns)
-            if manual:
-                with torch.no_grad():
-                    acts = on.conv_forward_saving(states)  # library kernels, backward scheduled by hand below
-                x_s = acts[-1].view(Bs, -1)
-            else:
-                x_s = on.features(states)                  # autograd graph: convs only
             with torch.no_grad():
-                xs_d = x_s.detach()
-                main.wait_event(done_ns)
-                if noise_done is not None:
-                    main.wait_event(noise_done)
-                x_ns.record_stream(main)
-                z_on, h_on, p_on = on.head().forward(xs_d, x_ns)              # rows [0,B) = s, [B,2B) = s'
-                main.wait_event(done_tg)
+                x_ns, done_ns = _lib.side_branch(s_ns, lambda: on.features_nograd(next_states))
+                if manual:
+                    acts = on.conv_forward_saving(states)  # library kernels, backward scheduled by hand below
+            x_s = acts[-1].view(Bs, -1) if manual else on.features(states)    # else an autograd graph: convs only
+            xs_d = x_s.detach()
+            main.wait_event(done_ns)
+            x_ns.record_stream(main)
+            head_in = (xs_d, x_ns)
         with torch.no_grad():
-            # what the statistics read besides the losses: C51's projected m, or the quantile loss's target rows T
-            m = torch.empty((B, self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
-            if self.quantile:   # M = K = 1 (Agent refuses the copies)
-                loss, dz = qr_dueling_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
-                                                weights, self.quantile_kappa, self._gamma_n(), theta_out=m)
-            elif (M, K) == (1, 1):
-                loss, dz = c51_dueling_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
-                                                 weights, self.support, self.Vmin, self.Vmax, self.delta_z,
-                                                 self._gamma_n(), m_out=m)
-            else:
-                loss, dz = c51_dueling_avg_loss_grad(z_on, z_t, self.action_space, self.atoms, actions, returns, nonterminals,
-                                                     weights, self.support, self.Vmin, self.Vmax, self.delta_z,
-                                                     self._gamma_n(), M, K, m_out=m)
-            stats_done = self._stats_batch(batch, loss, m, z=z_on) if m is not None else None
+            if noise_done is not None:
+                main.wait_event(noise_done)
+            z_on, h_on, p_on = on.head().forward(*head_in)                # rows [0, Bs) = s, then s'
+            main.wait_event(done_tg)
+            loss, dz, m = self._fused_loss(z_on, z_t, batch, Bs // B, Bn // B)
+            stats_done = self._stats_batch(batch, loss, m, z=z_on)
             wb_done = None
             if after_loss is not None:
                 # the priority write-back (agent.py:100) needs nothing but the per-sample losses: it runs on a side
                 # stream beside the whole backward instead of at the end of the critical path
-                loss_ready = torch.cuda.Event()
-                loss_ready.record(main)
-                with torch.cuda.stream(s_ns):
-                    s_ns.wait_event(loss_ready)
-                    after_loss(loss)
-                    wb_done = torch.cuda.Event()
-                    wb_done.record(s_ns)
+                wb_done = _lib.side_branch(s_ns, lambda: after_loss(loss))[1]
+            hd = on.head()
             dh = torch.empty((FusedHead.dh_rows(Bs), 2 * on.hidden_size), dtype=torch.float32, device=self.device)   # dh, then its transpose
             dx = torch.empty_like(xs_d)
             if manual:
                 # dx comes back already masked by the last conv layer's ReLU; conv gradients are overwritten.
                 # The layer-2 weight gradient feeds nothing but the optimiser: it runs beside the dh -> layer-1 chain.
-                hd = on.head()
-                dz_ready = torch.cuda.Event()
-                dz_ready.record(main)
-                with torch.cuda.stream(s_tg):
-                    s_tg.wait_event(dz_ready)
-                    hd.backward(p_on, xs_d, h_on[:Bs], dz, dh, dx, parts=hd.BWD_WGRAD2)
-                    w2_done = torch.cuda.Event()
-                    w2_done.record(s_tg)
+                w2_done = _lib.side_branch(
+                    s_tg, lambda: hd.backward(p_on, xs_d, h_on[:Bs], dz, dh, dx, parts=hd.BWD_WGRAD2))[1]
                 hd.backward(p_on, xs_d, h_on[:Bs], dz, dh, dx, relu_mask_x=True, parts=hd.BWD_DH | hd.BWD_LAYER1)
                 main.wait_event(w2_done)
-                head_ready = None
+                opt = self.optimiser
                 if self.sync.enabled:
                     # 99 % of the gradient bytes (the noisy head) are final here: start their exchange on a side
                     # stream so it overlaps the conv backward; the conv slice (a few hundred KB) follows afterwards.
                     # Peer optimiser: reduce-scatter by NVLink peer loads (rb_peer_reduce); else NCCL all-reduce.
-                    head_ready = torch.cuda.Event()
-                    head_ready.record(main)
-                    with torch.cuda.stream(s_tg):
-                        s_tg.wait_event(head_ready)
-                        if self.optimiser.peer is not None:
-                            self.optimiser.peer.reduce_segment(0)
+                    def reduce_head():
+                        if opt.peer is not None:
+                            opt.peer.reduce_segment(0)
                         else:
-                            self.sync.all_reduce_(self.optimiser.flat_grad[self.optimiser.conv_end:])
-                        head_reduced = torch.cuda.Event()
-                        head_reduced.record(s_tg)
+                            self.sync.all_reduce_(opt.flat_grad[opt.conv_end:])
+                    head_reduced = _lib.side_branch(s_tg, reduce_head)[1]
                 # (a separate stream for the first layer's own weight-gradient kernel was tried and lost: it then overlaps
                 # cuDNN's wgrad of the layer above and both slow down -- r02e vs r02f timelines)
-                grads_done = on.conv_backward_into_grads(acts, dx.view_as(acts[-1]), s_ns)
-                main.wait_event(grads_done)
+                main.wait_event(on.conv_backward_into_grads(acts, dx.view_as(acts[-1]), s_ns))
                 if self.sync.enabled:
-                    self.sync.all_reduce_(self.optimiser.flat_grad[:self.optimiser.conv_end])
+                    self.sync.all_reduce_(opt.flat_grad[:opt.conv_end])
                     main.wait_event(head_reduced)
             else:
                 self.optimiser.zero_conv_grad()
-                on.head().backward(p_on, xs_d, h_on[:Bs], dz, dh, dx)      # writes the 16 head gradients + dx
+                hd.backward(p_on, xs_d, h_on[:Bs], dz, dh, dx)      # writes the 16 head gradients + dx
         if not manual:
             x_s.backward(dx)
             self.sync.all_reduce_(self.optimiser.flat_grad)
-        self.optimiser.step(grad_scale=1.0 / self.sync.world_size, gate=self._step_gate)
-        self._target_ema()
-        if stats_done is not None:
-            self._stats_write(stats_done)
-        if wb_done is not None:
-            main.wait_event(wb_done)
+        self._update_tail(stats_done, wb_done)
         return loss
 
     def _update_from_batch(self, batch, target_noise=None, after_loss=None, gate=None):
@@ -895,7 +843,7 @@ class Agent:
             return self._update_fused(batch, target_noise, after_loss)
         if copies != (1, 1):
             raise self._copies_error(copies)
-        idxs, states, actions, returns, next_states, nonterminals, weights = batch
+        states, next_states = batch[1], batch[4]
         # a deferred draw first: the rows of s (the library's NoisyLinear, which composes the epsilon buffers only when they
         # are stale) and of s' (the fused head, which reads the factors) must see the same draw
         self.online_net.flush_noise()
@@ -904,29 +852,76 @@ class Agent:
         q_s = self.online_net.logits(states)
         with torch.no_grad():
             q_ns = self.online_net.logits(next_states)
-            if target_noise is None:
-                self.target_net.reset_noise()
-            else:
-                self.target_net.reset_noise(*target_noise)
+            self.target_net.reset_noise(*(target_noise or ()))
             q_t = self.target_net.logits(next_states)
-            m = torch.empty((q_s.shape[0], self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
-            if self.quantile:
-                loss, grad = qr_loss_grad(q_s.detach(), q_ns, q_t, actions, returns, nonterminals, weights,
-                                          self.quantile_kappa, self._gamma_n(), theta_out=m)
-            else:
-                loss, grad = c51_loss_grad(q_s.detach(), q_ns, q_t, actions, returns, nonterminals, weights, self.support,
-                                           self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m)
-            stats_done = self._stats_batch(batch, loss, m, q=q_s.detach()) if m is not None else None
+            loss, grad, m = self._library_loss(q_s.detach(), q_ns, q_t, batch)
+            stats_done = self._stats_batch(batch, loss, m, q=q_s.detach())
         self.optimiser.zero_grad()
         q_s.backward(grad)
         self.sync.all_reduce_(self.optimiser.flat_grad)
+        self._update_tail(stats_done)
+        if after_loss is not None:
+            after_loss(loss)
+        return loss
+
+    def _update_tail(self, stats_done, wb_done=None):
+        """The end of every update: clip + Adam under the sample's gate, the Polyak target update, the statistics record
+        (after `stats_done`) and the join of a priority write-back on a side stream (`wb_done`)."""
         self.optimiser.step(grad_scale=1.0 / self.sync.world_size, gate=self._step_gate)
         self._target_ema()
         if stats_done is not None:
             self._stats_write(stats_done)
-        if after_loss is not None:
-            after_loss(loss)
-        return loss
+        if wb_done is not None:
+            torch.cuda.current_stream(self.device).wait_event(wb_done)
+
+    # ---- the loss and what the statistics read of it: one choice of kernel per path ----------------------------------
+    def _stats_rows(self, B):
+        """What rb_learn_stats_batch reads besides the losses -- C51's projected m, or the quantile loss's target rows T
+        -- as a loss kernel's optional output; None with the statistics off."""
+        return torch.empty((B, self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
+
+    def _fused_loss(self, z_online, z_target, batch, M, K):
+        """The loss on the fused heads' rows for M copies of s and K of s': rb_qr_dueling_loss_grad (quantile; M = K = 1,
+        the Agent refuses copies), rb_c51_dueling_loss_grad, or at M or K > 1 rb_c51_dueling_avg_loss_grad.  Returns
+        (loss[B], dz, stats rows)."""
+        _, _, actions, returns, _, nonterminals, weights = batch
+        m = self._stats_rows(actions.shape[0])
+        rows = (z_online, z_target, self.action_space, self.atoms, actions, returns, nonterminals, weights)
+        if self.quantile:
+            return (*qr_dueling_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m), m)
+        c51 = (self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n())
+        if (M, K) == (1, 1):
+            return (*c51_dueling_loss_grad(*rows, *c51, m_out=m), m)
+        return (*c51_dueling_avg_loss_grad(*rows, *c51, M, K, m_out=m), m)
+
+    def _library_loss(self, q_s, q_ns, q_t, batch):
+        """The loss on the library head's logits [B, A, Z]: rb_qr_loss_grad (quantile) or rb_c51_loss_grad.  Returns
+        (loss[B], grad[B, A, Z], stats rows)."""
+        _, _, actions, returns, _, nonterminals, weights = batch
+        m = self._stats_rows(actions.shape[0])
+        rows = (q_s, q_ns, q_t, actions, returns, nonterminals, weights)
+        if self.quantile:
+            return (*qr_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m), m)
+        return (*c51_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m), m)
+
+    def _stats_batch(self, batch, loss, m, z=None, q=None):
+        """rb_learn_stats_batch on a side stream as soon as the losses exist: it runs beside the backward.  Returns the
+        event _stats_write waits for (None with the statistics off).  The inputs of the latest record stay reachable in
+        self._stats["last"].  `m`: the loss kernel's stats rows (rb_learn_stats_batch_qr under the quantile loss)."""
+        if self._stats is None:
+            return None
+        lib, scratch = _lib.load(), _lib.ptr(self._stats["scratch"])
+        head = (_lib.ptr(loss), _lib.ptr(batch[6]), _lib.ptr(batch[2]), _lib.ptr(m))
+        tail = (_lib.ptr(z), _lib.ptr(q), loss.shape[0], self.action_space, self.atoms, scratch)
+
+        def launch():
+            if self.quantile:
+                _lib.check(lib.rb_learn_stats_batch_qr(*head, *tail, _lib.stream()))
+            else:
+                _lib.check(lib.rb_learn_stats_batch(*head, _lib.ptr(self.support), *tail, _lib.stream()))
+        done = _lib.side_branch(self._side_streams()[0], launch)[1]
+        self._stats["last"] = dict(m=m, z=z, q=q)
+        return done
 
     def _gamma_n(self):
         """The gamma_n the loss kernels take: gamma ** n, or 1 with an annealed horizon, whose gather writes the nonterminals
@@ -1071,14 +1066,22 @@ class Agent:
             f"augment_m * batch_size <= 512 and a shape the fused head takes); the library head trains on one copy of s and "
             f"s' only")
 
+    def _sample_and_update(self, mem, ws=None):
+        """One update on a batch of the ReplayMemory `mem` sampled with this agent's augmentation and horizon -- into a fresh
+        workspace (mem.sample), or into `ws` (mem.sample_into: no synchronisation, capturable) -- whose status gates the
+        optimiser step and the priority write-back.  Returns (batch, per-sample losses)."""
+        aug = dict(shift_pad=self.augment_shift, intensity=self.augment_intensity, copies=self.augment_copies,
+                   horizon=self._horizon)
+        batch = mem.sample(self.batch_size, **aug) if ws is None else mem.sample_into(ws, **aug)
+        gate = mem.sample_gate()
+        loss = self._update_from_batch(batch, after_loss=lambda l: mem.update_priorities(batch[0], l, gate=gate), gate=gate)
+        return batch, loss
+
     def _learn_eager(self, mem):
         if isinstance(mem, ReplayMemory):
-            batch = mem.sample(self.batch_size, shift_pad=self.augment_shift, intensity=self.augment_intensity,
-                               copies=self.augment_copies, horizon=self._horizon)
+            batch, loss = self._sample_and_update(mem)
             self._redo_states = batch[1]
-            gate = mem.sample_gate()
-            return self._update_from_batch(batch, after_loss=lambda loss: mem.update_priorities(batch[0], loss, gate=gate),
-                                           gate=gate)
+            return loss
         batch = mem.sample(self.batch_size)
         self._redo_states = batch[1]
         loss = self._update_from_batch(batch)
@@ -1094,10 +1097,7 @@ class Agent:
         torch.cuda.synchronize(self.device)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            batch = mem.sample_into(ws, shift_pad=self.augment_shift, intensity=self.augment_intensity,
-                                    copies=self.augment_copies, horizon=self._horizon)
-            loss = self._update_from_batch(batch, after_loss=lambda l: mem.update_priorities(batch[0], l, gate=ws.status),
-                                           gate=ws.status)
+            _, loss = self._sample_and_update(mem, ws)
         return graph, ws, loss
 
     @property
@@ -1133,11 +1133,7 @@ class Agent:
         if not graphable:
             self.last_loss = self._learn_eager(mem)
         elif not self._graphs and self._warm < self.GRAPH_WARMUP:
-            side = torch.cuda.Stream(device=self.device)
-            side.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(side):
-                self.last_loss = self._learn_eager(mem)
-            torch.cuda.current_stream(self.device).wait_stream(side)
+            self.last_loss = self._warm_up(lambda: self._learn_eager(mem))
             self._warm += 1
         else:
             # two variants of the graph: with the online net's deferred reset_noise() as a side branch (the usual
@@ -1210,30 +1206,6 @@ class Agent:
         out["dropped"] = first - st["read"]
         st["read"] = count
         return out
-
-    def _stats_batch(self, batch, loss, m, z=None, q=None):
-        """rb_learn_stats_batch on a side stream as soon as the losses exist: it runs beside the backward.  Returns the
-        event _stats_write waits for.  The inputs of the latest record stay reachable in self._stats["last"].  `m`: C51's
-        projected m, or under the quantile distribution the loss kernel's target rows T (rb_learn_stats_batch_qr)."""
-        main = torch.cuda.current_stream(self.device)
-        side = self._side_streams()[0]
-        ready = torch.cuda.Event()
-        ready.record(main)
-        with torch.cuda.stream(side):
-            side.wait_event(ready)
-            if self.quantile:
-                _lib.check(_lib.load().rb_learn_stats_batch_qr(
-                    _lib.ptr(loss), _lib.ptr(batch[6]), _lib.ptr(batch[2]), _lib.ptr(m), _lib.ptr(z), _lib.ptr(q),
-                    loss.shape[0], self.action_space, self.atoms, _lib.ptr(self._stats["scratch"]), _lib.stream()))
-            else:
-                _lib.check(_lib.load().rb_learn_stats_batch(
-                    _lib.ptr(loss), _lib.ptr(batch[6]), _lib.ptr(batch[2]), _lib.ptr(m), _lib.ptr(self.support),
-                    _lib.ptr(z), _lib.ptr(q), loss.shape[0], self.action_space, self.atoms,
-                    _lib.ptr(self._stats["scratch"]), _lib.stream()))
-            done = torch.cuda.Event()
-            done.record(side)
-        self._stats["last"] = dict(m=m, z=z, q=q)
-        return done
 
     def _stats_write(self, done):
         """rb_learn_stats_write after the optimiser step (its norm and gate are final): one thread on the caller's stream."""

@@ -406,31 +406,28 @@ class ReplayMemory:
         return shift_pad, intensity, (M, K)
 
     def _launch_gather(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1), horizon=None):
+        """The gather these settings select: rb_gather, rb_gather_shift (shifts only), rb_gather_aug (intensity or
+        copies), or with an annealed horizon rb_gather_horizon, which takes every augmentation setting."""
         tr = self.transitions
-        if horizon is not None:
-            self._launch_gather_horizon(ws, shift_pad, intensity, copies, horizon)
-            return
+        shifts, scales = self._aug_buffers(ws, shift_pad, intensity, copies)
+        # the n-step window: this replay's n and discount powers, or the horizon's n_max and its current row
+        window = (self.n, self.n_step_scaling) if horizon is None else (horizon.n_max, horizon.current)
         common = (_lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action), _lib.ptr(tr.reward),
-                  _lib.ptr(tr.nonterminal), tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, self.n,
-                  _lib.ptr(self.n_step_scaling), _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions),
+                  _lib.ptr(tr.nonterminal), tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, window[0],
+                  _lib.ptr(window[1]), _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions),
                   _lib.ptr(ws.returns), _lib.ptr(ws.nonterminals))
-        if not shift_pad and not intensity and copies == (1, 1):
-            _lib.check(self._lib.rb_gather(*common, _lib.stream()))
-            return
-        if not intensity and copies == (1, 1):
-            if ws.shifts is None or ws.shifts.shape != (2, ws.B, 2):
-                ws.shifts = torch.empty((2, ws.B, 2), dtype=torch.int32, device=self.device)
-            _lib.check(self._lib.rb_gather_shift(*common, shift_pad, self.seed, _lib.ptr(self._rng_counter),
-                                                 _lib.ptr(ws.shifts), _lib.stream()))
-            return
-        c = max(copies)
-        if ws.shifts is None or ws.shifts.shape != (2, c, ws.B, 2):
-            ws.shifts = torch.empty((2, c, ws.B, 2), dtype=torch.int32, device=self.device)
-        if ws.scales is None or ws.scales.shape != (2, c, ws.B):
-            ws.scales = torch.empty((2, c, ws.B), dtype=torch.float32, device=self.device)
-        _lib.check(self._lib.rb_gather_aug(*common, shift_pad, intensity, copies[0], copies[1], self.seed,
-                                           _lib.ptr(self._rng_counter), _lib.ptr(ws.shifts), _lib.ptr(ws.scales),
-                                           _lib.stream()))
+        aug = (shift_pad, intensity, copies[0], copies[1], self.seed, _lib.ptr(self._rng_counter), _lib.ptr(shifts),
+               _lib.ptr(scales))
+        if horizon is not None:
+            rc = self._lib.rb_gather_horizon(*common, *aug, _lib.stream())
+        elif scales is not None:
+            rc = self._lib.rb_gather_aug(*common, *aug, _lib.stream())
+        elif shifts is not None:
+            rc = self._lib.rb_gather_shift(*common, shift_pad, self.seed, _lib.ptr(self._rng_counter), _lib.ptr(shifts),
+                                           _lib.stream())
+        else:
+            rc = self._lib.rb_gather(*common, _lib.stream())
+        _lib.check(rc)
 
     def _aug_buffers(self, ws, shift_pad, intensity, copies):
         """ws.shifts / ws.scales shaped for the gather these settings select (None where it writes none)."""
@@ -452,32 +449,6 @@ class ReplayMemory:
             raise ValueError(f"the horizon reaches n = {horizon.n_max}, this replay was built for n = {self.n} "
                              "(set args.multi_step_start before building it)")
 
-    def _launch_gather_horizon(self, ws, shift_pad, intensity, copies, horizon):
-        tr = self.transitions
-        shifts, scales = self._aug_buffers(ws, shift_pad, intensity, copies)
-        _lib.check(self._lib.rb_gather_horizon(
-            _lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action), _lib.ptr(tr.reward), _lib.ptr(tr.nonterminal),
-            tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, horizon.n_max, _lib.ptr(horizon.current),
-            _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions), _lib.ptr(ws.returns),
-            _lib.ptr(ws.nonterminals), shift_pad, intensity, copies[0], copies[1], self.seed, _lib.ptr(self._rng_counter),
-            _lib.ptr(shifts), _lib.ptr(scales), _lib.stream()))
-
-    def _sample_horizon(self, ws, shift_pad, intensity, copies, horizon):
-        """rb_horizon_advance on a side branch beside rb_tree_sample (which does not read the horizon), joined before the
-        gather through the horizon's current row."""
-        main = torch.cuda.current_stream(self.device)
-        side = horizon.side_stream()
-        fork = torch.cuda.Event()
-        fork.record(main)
-        with torch.cuda.stream(side):
-            side.wait_event(fork)
-            horizon.advance()
-            done = torch.cuda.Event()
-            done.record(side)
-        self._launch_sample(ws)
-        main.wait_event(done)
-        self._launch_gather_horizon(ws, shift_pad, intensity, copies, horizon)
-
     def sample_into(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1), horizon=None):
         """Device-RNG sample into caller-owned buffers: two launches, no synchronisation (graph capturable).
         The caller is responsible for push_beta() and flush_appends() (outside any graph capture).
@@ -495,11 +466,12 @@ class ReplayMemory:
         if ws.copies != copies:
             raise ValueError(f"the workspace holds copies {ws.copies}, the call asks for {copies}")
         self._check_horizon(horizon)
-        if horizon is None:
-            self._launch_sample(ws)
-            self._launch_gather(ws, shift_pad, intensity, copies)
-        else:
-            self._sample_horizon(ws, shift_pad, intensity, copies, horizon)
+        if horizon is not None:   # beside rb_tree_sample, which does not read the horizon; joined before the gather
+            advanced = _lib.side_branch(horizon.side_stream(), horizon.advance)[1]
+        self._launch_sample(ws)
+        if horizon is not None:
+            torch.cuda.current_stream(self.device).wait_event(advanced)
+        self._launch_gather(ws, shift_pad, intensity, copies, horizon)
         self._last = ws
         return ws.as_tuple()
 

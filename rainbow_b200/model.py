@@ -230,7 +230,6 @@ class DQN(nn.Module):
         self._eps_stale = False  # weight_epsilon / bias_epsilon buffers currently equal the outer product of the factors
         self._head = None
         self.use_fused_head = True
-        self.use_own_wgrad = True     # first conv layer's weight gradient through rb_conv_wgrad (else cuDNN)
 
     # ---- noise ---------------------------------------------------------------------------------------
     def noisy_layers(self):
@@ -344,7 +343,7 @@ class DQN(nn.Module):
 
     def _own_wgrad_ok(self, m, a_in):
         k, s = m.kernel_size, m.stride
-        return (self.use_own_wgrad and k[0] == k[1] and s[0] == s[1] and k[0] in (3, 4, 5, 8) and tuple(m.padding) == (0, 0) and
+        return (k[0] == k[1] and s[0] == s[1] and k[0] in (3, 4, 5, 8) and tuple(m.padding) == (0, 0) and
                 tuple(m.dilation) == (1, 1) and m.groups == 1 and a_in.is_contiguous() and m.weight.grad.is_contiguous() and
                 m.in_channels * k[0] * ((m.out_channels + 3) // 4) <= 256 and
                 _lib.load().rb_conv_wgrad_scratch_elems(a_in.shape[0], m.in_channels, a_in.shape[2], m.out_channels, k[0], s[0]) > 0)
@@ -357,50 +356,38 @@ class DQN(nn.Module):
             self._wgrad_buf = buf
         return buf
 
-    def conv_backward_into_grads(self, acts, g_last, side_stream, first_layer_stream=None):
+    def conv_backward_into_grads(self, acts, g_last, side_stream):
         """Backward of the conv body given g_last = d loss / d (pre-activation of the last conv layer).
         The data-gradient chain (dgrad -> ReLU mask -> dgrad ...) runs on the current stream; the weight and bias
         gradients, which nothing downstream waits for except the optimiser, run on `side_stream` and are written
         straight into the parameters' .grad storage.  Returns the event the optimiser has to wait for."""
         lib = _lib.load()
-        main = torch.cuda.current_stream(g_last.device)
         layers = self.conv_layers()
         g = g_last
-        extra_done = None
         for li in range(len(layers) - 1, -1, -1):
             m, a_in = layers[li], acts[li]
-            ready = torch.cuda.Event()
-            ready.record(main)
-            own = li == 0 and self._own_wgrad_ok(m, a_in)
-            # the first layer's gradient is the last thing the chain produces: it gets its own stream so that it does not
-            # queue behind the (independent) weight gradients of the layers above on `side_stream`
-            st = first_layer_stream if (own and first_layer_stream is not None) else side_stream
-            with torch.cuda.stream(st):
-                st.wait_event(ready)
-                g.record_stream(st)
-                if own:
+
+            def weight_grads():
+                g.record_stream(side_stream)
+                st = side_stream.cuda_stream
+                if li == 0 and self._own_wgrad_ok(m, a_in):
                     # first layer: no data gradient follows, so this launch sits alone on the critical path -> own kernel
                     # (csrc/rb_head.cu k_conv_wgrad_first; weight AND bias gradient from one pass over g)
                     _lib.check(lib.rb_conv_wgrad(_lib.ptr(g), _lib.ptr(a_in), a_in.shape[0], a_in.shape[1], a_in.shape[2], a_in.shape[3],
                                                  m.out_channels, m.kernel_size[0], m.stride[0], _lib.ptr(self._wgrad_scratch(m, a_in)),
-                                                 _lib.ptr(m.weight.grad), _lib.ptr(m.bias.grad), st.cuda_stream))
+                                                 _lib.ptr(m.weight.grad), _lib.ptr(m.bias.grad), st))
                 else:   # bias first (it only needs g), then the library's weight gradient
                     _lib.check(lib.rb_bias_grad(_lib.ptr(g), g.shape[0], g.shape[1], g.shape[2] * g.shape[3],
-                                                _lib.ptr(m.bias.grad), st.cuda_stream))
+                                                _lib.ptr(m.bias.grad), st))
                     _, gw, _ = torch.ops.aten.convolution_backward(g, a_in, m.weight, None, m.stride, m.padding, m.dilation, False,
                                                                    [0, 0], m.groups, [False, True, False])
                     m.weight.grad.copy_(gw)
-                if st is not side_stream:
-                    extra_done = torch.cuda.Event()
-                    extra_done.record(st)
+
+            _, done = _lib.side_branch(side_stream, weight_grads)
             if li > 0:
                 gin, _, _ = torch.ops.aten.convolution_backward(g, a_in, m.weight, None, m.stride, m.padding, m.dilation, False,
                                                                 [0, 0], m.groups, [True, False, False])
                 g = torch.ops.aten.threshold_backward(gin, a_in, 0.0)      # ReLU of the layer below (a_in = its output)
-        if extra_done is not None:
-            side_stream.wait_event(extra_done)
-        done = torch.cuda.Event()
-        done.record(side_stream)
         return done
 
     def features_nograd(self, x):

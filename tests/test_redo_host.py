@@ -231,10 +231,19 @@ def test_redo_table_tiles_the_elements_the_semantics_name(arch, names, neurons):
                 assert blk[3] == below["mask_offset"] and blk[1] == blk[2] * below["neurons"]
             else:
                 assert blk[1] == 1 or li == 0
-    # the good table passes every host check of rb_redo_recycle except the launch (no device here)
+    # the good table passes every host check of rb_redo_recycle: without a device only the launch fails; with one the call
+    # runs -- on real buffers with an all-zero mask (nothing dormant, nothing written), never on the pointers above
     from rainbow_b200.agent import redo_layers_c
-    rc = lib().rb_redo_recycle(ONE, ONE, ONE, opt.numel, redo_layers_c(table), len(table), ONE, 7, 0, None)
-    assert rc not in (RB_ERR_INVAL, RB_ERR_RANGE)
+    if torch.cuda.is_available():
+        bufs = [torch.zeros(opt.numel, device="cuda") for _ in range(3)]
+        mask = torch.zeros(sum(neurons), dtype=torch.uint8, device="cuda")
+        rc = lib().rb_redo_recycle(*[b.data_ptr() for b in bufs], opt.numel, redo_layers_c(table), len(table),
+                                   mask.data_ptr(), 7, 0, None)
+        torch.cuda.synchronize()
+        assert rc == 0 and not any(bool(b.any()) for b in bufs)
+    else:
+        rc = lib().rb_redo_recycle(ONE, ONE, ONE, opt.numel, redo_layers_c(table), len(table), ONE, 7, 0, None)
+        assert rc not in (RB_ERR_INVAL, RB_ERR_RANGE)
 
 
 # ---- references ----------------------------------------------------------------------------------------------------------
