@@ -241,6 +241,17 @@ int rb_c51_loss_grad(const float* q_online_s, const float* q_online_ns, const fl
                      const float* weights, const float* support, float vmin, float vmax, float delta_z,
                      float gamma_n, int B, int A, int Z, float* loss, float* grad_q_online_s, float* m_out,
                      int64_t* astar_out, rb_stream_t stream);
+/* rb_c51_loss_grad under value rescaling (Pohlen et al. 2018; DESIGN.md §16): the logits are a distribution over the
+ * support in h units, h(x) = sign(x) (sqrt(|x| + 1) - 1) + eps x.  support_q[Z] = fl32(h^-1(support)) (return units)
+ * replaces the support in the double-DQN arg-max, and the target atoms are Tz_j = h(fl32(r + fl32(s support_q_j))),
+ * s = fl32(nonterminal gamma_n), clamped to [vmin, vmax] (h units) and projected as rb_c51_loss_grad projects them.
+ * RB_ERR_INVAL also for a NULL support_q and eps outside [0, 1] or NaN.  A refused call writes nothing.  Profiled under
+ * RB_K_C51. */
+int rb_c51_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                        const float* returns, const float* nonterminals, const float* weights, const float* support,
+                        float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z, float* loss,
+                        float* grad_q_online_s, float* m_out, int64_t* astar_out, const float* support_q, float eps,
+                        rb_stream_t stream);
 
 /* model.py:82-85 DQN.reset_noise -> :36-40 NoisyLinear.reset_noise -> :32-34 _scale_noise, all
  * layers of one net in one launch.  HOST arrays (length n_layers): weight_eps[l] -> float32[out][in],
@@ -361,6 +372,12 @@ int rb_c51_dueling_loss_grad(const float* z_online, const float* z_target, int a
                              const float* returns, const float* nonterminals, const float* weights, const float* support,
                              float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss, float* dz, float* m_out,
                              int64_t* astar_out, rb_stream_t stream);
+/* rb_c51_dueling_loss_grad under value rescaling: the arg-max and the target atoms as rb_c51_vt_loss_grad forms them,
+ * with its refusals.  Profiled under RB_K_C51_DUELING. */
+int rb_c51_dueling_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
+                                const float* returns, const float* nonterminals, const float* weights, const float* support,
+                                float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss, float* dz,
+                                float* m_out, int64_t* astar_out, const float* support_q, float eps, rb_stream_t stream);
 
 /* rb_c51_dueling_loss_grad with DrQ's averaging over K target copies and M online copies (Kostrikov et al. 2020,
  * Algorithm 1).  z_online has (M + K) B rows: copy j of s at row jB + i, then copy k of s' at row (M + k) B + i; z_target
@@ -374,6 +391,14 @@ int rb_c51_dueling_avg_loss_grad(const float* z_online, const float* z_target, i
                                  const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
                                  const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int M,
                                  int K, float* loss, float* dz, float* m_out, int64_t* astar_out, rb_stream_t stream);
+/* rb_c51_dueling_avg_loss_grad under value rescaling: every m_k projected as rb_c51_vt_loss_grad projects, averaged on the
+ * h-space grid; rb_c51_vt_loss_grad's refusals.  At M = K = 1 every output equals rb_c51_dueling_vt_loss_grad's, bitwise.
+ * Profiled under RB_K_C51_DUELING_AVG. */
+int rb_c51_dueling_avg_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                    const int64_t* actions, const float* returns, const float* nonterminals,
+                                    const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                    float gamma_n, int B, int M, int K, float* loss, float* dz, float* m_out,
+                                    int64_t* astar_out, const float* support_q, float eps, rb_stream_t stream);
 
 /* Quantile regression (QR-DQN, Dabney et al. 2018) in place of the categorical projection: atoms = N quantiles per action
  * (2 <= N <= RB_MAX_ATOMS) at the midpoints tau_i = (2i + 1) / (2N); no support.  For sample b with taken action a:
@@ -401,6 +426,20 @@ int rb_qr_loss_grad(const float* q_online_s, const float* q_online_ns, const flo
  * over actions, from z[M][atoms*(1+actions)].  q, best_action, best_q are each optional (not all NULL). */
 int rb_qr_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
                    rb_stream_t stream);
+/* The quantile entries under value rescaling (DESIGN.md §16): the quantiles are in h units.  x_j = h^-1(q_target(s', a*)_j),
+ * T_j = h(fl32(r + fl32(s x_j))), a* = argmax_a (1/N) sum_j h^-1(q_online(s', a)_j) (first maximum wins); theta, u, the
+ * loss, the gradient and theta_out (= T) are in h units.  rb_qr_vt_q_values: q[m][a] = (1/N) sum_j h^-1(q_j) (return
+ * units).  RB_ERR_INVAL also for eps outside [0, 1] or NaN.  A refused call writes nothing.  Profiled as their siblings. */
+int rb_qr_dueling_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
+                               const float* returns, const float* nonterminals, const float* weights, float kappa,
+                               float gamma_n, int B, float* loss, float* dz, float* theta_out, int64_t* astar_out, float eps,
+                               rb_stream_t stream);
+int rb_qr_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                       const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
+                       int B, int A, int N, float* loss, float* grad_q_online_s, float* theta_out, int64_t* astar_out,
+                       float eps, rb_stream_t stream);
+int rb_qr_vt_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
+                      float eps, rb_stream_t stream);
 
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */
@@ -614,6 +653,11 @@ int rb_learn_stats_write(const double* scratch, const float* grad_norm, const in
  * in one of the two layouts above (N = atoms); no support.  Same scratch, refusals and rb_learn_stats_write. */
 int rb_learn_stats_batch_qr(const float* loss, const float* weights, const int64_t* actions, const float* theta, const float* z,
                             const float* q, int B, int A, int N, double* scratch, rb_stream_t stream);
+/* rb_learn_stats_batch_qr under value rescaling: theta from rb_qr_*_vt_loss_grad; q_mean = mean_i mean_k h^-1(theta_ik) and
+ * target_mean = mean_i mean_k h^-1(T_ik), in return units.  RB_ERR_INVAL also for eps outside [0, 1] or NaN. */
+int rb_learn_stats_batch_qr_vt(const float* loss, const float* weights, const int64_t* actions, const float* theta,
+                               const float* z, const float* q, int B, int A, int N, double* scratch, float eps,
+                               rb_stream_t stream);
 int rb_learn_stats(const float* loss, const float* weights, const int64_t* actions, const float* m, const float* support,
                    const float* z, const float* q, int B, int A, int Z, const float* grad_norm, const int32_t* gate,
                    float max_norm, double* scratch, rb_learn_stats_record* ring, int capacity, int64_t* counter,

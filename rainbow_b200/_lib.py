@@ -139,6 +139,19 @@ SIGNATURES = {
     "rb_learn_stats_write": (C.c_int, [_vp, _vp, _vp, _f32, _vp, _i32, _vp, _vp]),
     "rb_learn_stats": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _vp, _i32, _vp,
                                  _vp]),
+    # value rescaling: each is its sibling's signature with (support_q,) eps inserted before the stream
+    "rb_c51_vt_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i32, _i32, _i32,
+                                      _vp, _vp, _vp, _vp, _vp, _f32, _vp]),
+    "rb_c51_dueling_vt_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i32,
+                                              _vp, _vp, _vp, _vp, _vp, _f32, _vp]),
+    "rb_c51_dueling_avg_vt_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32,
+                                                  _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _vp]),
+    "rb_qr_dueling_vt_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _vp, _vp, _vp,
+                                             _vp, _f32, _vp]),
+    "rb_qr_vt_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _i32, _i32, _vp, _vp, _vp, _vp,
+                                     _f32, _vp]),
+    "rb_qr_vt_q_values": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _f32, _vp]),
+    "rb_learn_stats_batch_qr_vt": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _f32, _vp]),
 }
 
 # rb_learn_stats_record of include/rainbow_b200.h (48 bytes): field name -> numpy dtype, in memory order

@@ -54,74 +54,90 @@ from .model import DQN, FusedHead, NoisyLinear
 
 
 def c51_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax,
-                  delta_z, gamma_n, loss=None, grad=None, m_out=None, astar_out=None):
-    """Launch K3 on pre-softmax logits [B,A,Z]; returns (loss[B], grad[B,A,Z])."""
+                  delta_z, gamma_n, loss=None, grad=None, m_out=None, astar_out=None, support_q=None, eps=None):
+    """Launch K3 on pre-softmax logits [B,A,Z]; returns (loss[B], grad[B,A,Z]).  eps given: value rescaling
+    (rb_c51_vt_loss_grad) with support_q = fl32(h^-1(support))."""
     B, A, Z = q_online_s.shape
     dev = q_online_s.device
     if loss is None:
         loss = torch.empty(B, dtype=torch.float32, device=dev)
     if grad is None:
         grad = torch.empty((B, A, Z), dtype=torch.float32, device=dev)
-    _lib.check(_lib.load().rb_c51_loss_grad(
+    lib = _lib.load()
+    fn, vt = (lib.rb_c51_loss_grad, ()) if eps is None else (lib.rb_c51_vt_loss_grad, (_lib.ptr(support_q), float(eps)))
+    _lib.check(fn(
         _lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
-        float(gamma_n), B, A, Z, _lib.ptr(loss), _lib.ptr(grad), _lib.ptr(m_out), _lib.ptr(astar_out), _lib.stream()))
+        float(gamma_n), B, A, Z, _lib.ptr(loss), _lib.ptr(grad), _lib.ptr(m_out), _lib.ptr(astar_out), *vt, _lib.stream()))
     return loss, grad
 
 
 def c51_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin, vmax,
-                          delta_z, gamma_n, m_out=None, astar_out=None):
+                          delta_z, gamma_n, m_out=None, astar_out=None, support_q=None, eps=None):
     """K3 fed straight by the fused heads (rb_c51_dueling_loss_grad): z_online [2B, Z(1+A)] (s rows, then s' rows),
-    z_target [B, Z(1+A)]; returns (loss[B], dz[B, Z(1+A)]) with dz = d mean(w*loss) / d (z_value | z_advantage)."""
+    z_target [B, Z(1+A)]; returns (loss[B], dz[B, Z(1+A)]) with dz = d mean(w*loss) / d (z_value | z_advantage).
+    eps given: value rescaling (rb_c51_dueling_vt_loss_grad) with support_q = fl32(h^-1(support))."""
     B = actions.shape[0]
     loss = torch.empty(B, dtype=torch.float32, device=actions.device)
     dz = torch.empty((B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
-    _lib.check(_lib.load().rb_c51_dueling_loss_grad(
+    lib = _lib.load()
+    fn, vt = ((lib.rb_c51_dueling_loss_grad, ()) if eps is None else
+              (lib.rb_c51_dueling_vt_loss_grad, (_lib.ptr(support_q), float(eps))))
+    _lib.check(fn(
         _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
-        float(gamma_n), B, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), _lib.stream()))
+        float(gamma_n), B, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), *vt, _lib.stream()))
     return loss, dz
 
 
 def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin,
-                              vmax, delta_z, gamma_n, M, K, m_out=None, astar_out=None):
+                              vmax, delta_z, gamma_n, M, K, m_out=None, astar_out=None, support_q=None, eps=None):
     """DrQ's K / M averaging (rb_c51_dueling_avg_loss_grad): z_online [(M + K) B, Z(1+A)] (M copies of s, then K copies of
     s', copy-major), z_target [K B, Z(1+A)]; returns (loss[B], dz[M B, Z(1+A)]): the loss averaged over the M online
-    copies against the target averaged over the K target copies, and its gradient for every online copy of s."""
+    copies against the target averaged over the K target copies, and its gradient for every online copy of s.  eps
+    given: value rescaling (rb_c51_dueling_avg_vt_loss_grad)."""
     B = actions.shape[0]
     loss = torch.empty(B, dtype=torch.float32, device=actions.device)
     dz = torch.empty((M * B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
-    _lib.check(_lib.load().rb_c51_dueling_avg_loss_grad(
+    lib = _lib.load()
+    fn, vt = ((lib.rb_c51_dueling_avg_loss_grad, ()) if eps is None else
+              (lib.rb_c51_dueling_avg_vt_loss_grad, (_lib.ptr(support_q), float(eps))))
+    _lib.check(fn(
         _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
-        float(gamma_n), B, M, K, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), _lib.stream()))
+        float(gamma_n), B, M, K, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), *vt, _lib.stream()))
     return loss, dz
 
 
 def qr_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, kappa, gamma_n,
-                 theta_out=None, astar_out=None):
-    """The quantile loss (rb_qr_loss_grad) on quantile rows [B,A,N]; returns (loss[B], grad[B,A,N])."""
+                 theta_out=None, astar_out=None, eps=None):
+    """The quantile loss (rb_qr_loss_grad) on quantile rows [B,A,N]; returns (loss[B], grad[B,A,N]).  eps given: value
+    rescaling (rb_qr_vt_loss_grad)."""
     B, A, N = q_online_s.shape
     loss = torch.empty(B, dtype=torch.float32, device=q_online_s.device)
     grad = torch.empty((B, A, N), dtype=torch.float32, device=q_online_s.device)
-    _lib.check(_lib.load().rb_qr_loss_grad(
+    lib = _lib.load()
+    fn, vt = (lib.rb_qr_loss_grad, ()) if eps is None else (lib.rb_qr_vt_loss_grad, (float(eps),))
+    _lib.check(fn(
         _lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
         _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, A, N, _lib.ptr(loss), _lib.ptr(grad),
-        _lib.ptr(theta_out), _lib.ptr(astar_out), _lib.stream()))
+        _lib.ptr(theta_out), _lib.ptr(astar_out), *vt, _lib.stream()))
     return loss, grad
 
 
 def qr_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, kappa, gamma_n,
-                         theta_out=None, astar_out=None):
+                         theta_out=None, astar_out=None, eps=None):
     """The quantile loss fed straight by the fused heads (rb_qr_dueling_loss_grad), rows as c51_dueling_loss_grad takes
-    them; returns (loss[B], dz[B, N(1+A)])."""
+    them; returns (loss[B], dz[B, N(1+A)]).  eps given: value rescaling (rb_qr_dueling_vt_loss_grad)."""
     B = actions.shape[0]
     loss = torch.empty(B, dtype=torch.float32, device=actions.device)
     dz = torch.empty((B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
-    _lib.check(_lib.load().rb_qr_dueling_loss_grad(
+    lib = _lib.load()
+    fn, vt = (lib.rb_qr_dueling_loss_grad, ()) if eps is None else (lib.rb_qr_dueling_vt_loss_grad, (float(eps),))
+    _lib.check(fn(
         _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
         _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, _lib.ptr(loss), _lib.ptr(dz),
-        _lib.ptr(theta_out), _lib.ptr(astar_out), _lib.stream()))
+        _lib.ptr(theta_out), _lib.ptr(astar_out), *vt, _lib.stream()))
     return loss, dz
 
 
@@ -152,6 +168,39 @@ def distribution_options(args):
         raise ValueError(f"augment_m / augment_k = {copies} average categorical targets; with distribution 'quantile' "
                          f"both must be 1")
     return dist, kappa
+
+
+def value_transform_options(args):
+    """(value_transform, eps) from `args`, checked: value_transform None (absent, None or "none": off) or "rescale" (Pohlen
+    et al. 2018's h(x) = sign(x) (sqrt(|x| + 1) - 1) + eps x: the network learns h of the return, and the Bellman target
+    is h(r + gamma_n h^-1(z'))); value_transform_eps (absent or None: 1e-3) 0 or in [FLT_MIN, 1] -- a positive eps that
+    would round to 0 or a subnormal fp32 is refused, not silently turned into another h -- returned rounded to the
+    nearest fp32 (the value the kernels compute with), and None when the transform is off.  Under "rescale" args.V_min /
+    V_max and the network's outputs are in h units; act, evaluate_q* and the learn statistics' q_mean / target_mean are
+    in return units."""
+    vt = getattr(args, "value_transform", None)
+    if vt is None or vt == "none":
+        return None, None
+    if vt != "rescale":
+        raise ValueError(f"value_transform must be None, 'none' or 'rescale', got {vt!r}")
+    eps = getattr(args, "value_transform_eps", None)
+    eps = 1e-3 if eps is None else eps
+    if isinstance(eps, bool) or not isinstance(eps, (int, float, np.floating, np.integer)):
+        raise ValueError(f"value_transform_eps must be a number, got {eps!r}")
+    eps = float(eps)
+    if not (math.isfinite(eps) and (eps == 0.0 or np.finfo(np.float32).tiny <= eps <= 1.0)):
+        raise ValueError(f"value_transform_eps must be 0 or in [{np.finfo(np.float32).tiny:g}, 1] (a normal fp32), "
+                         f"got {eps}")
+    return vt, float(np.float32(eps))   # the fp32 the kernels take: the host's float64 h^-1 uses the same eps
+
+
+def vt_hinv(y, eps):
+    """h^-1(y) = sign(y) d (d + 2), d = 2|y| / ((1 + 2 eps) + sqrt((1 + 2 eps)^2 + 4 eps |y|)), elementwise in y's dtype
+    (the cancellation-free form of DESIGN.md §16)."""
+    ay = y.abs()
+    c = 1.0 + 2.0 * eps
+    d = (2.0 * ay) / (c + (c * c + (4.0 * eps) * ay).sqrt())
+    return torch.copysign(d * (d + 2.0), y)
 
 
 ENCODER, HEAD = 0, 1   # the two groups of reset_table / Agent.reset_parameters
@@ -443,6 +492,9 @@ class Agent:
         self.device = torch.device(args.device)
         if self.device.type != "cuda":
             raise _lib.RainbowB200Error(f"rainbow_b200.Agent needs a CUDA device, got '{self.device}' (no CPU fallback)")
+        # value rescaling (off by default): the network learns in h units, V_min / V_max included; acting, evaluation and
+        # the statistics report return units
+        self.value_transform, self.value_transform_eps = value_transform_options(args)
         # Precision policy (documented switch, default = the reference's arithmetic): the learner computes in true fp32.
         # `args.tf32 = True` lets cuDNN / cuBLAS use TF32 tensor cores for the conv body (north star: "tensor cores only
         # there"); the parity tests and bench.py run with the default.  torch keeps these flags per process, so the
@@ -457,6 +509,12 @@ class Agent:
         self.Vmax = args.V_max
         self.support = torch.linspace(args.V_min, args.V_max, self.atoms).to(device=self.device)  # agent.py:18
         self.delta_z = (args.V_max - args.V_min) / (self.atoms - 1)
+        # the support in return units, fl32(h^-1(z_j)) from the fp32 support in float64 (the support itself when off): the
+        # double-DQN arg-max, the target atoms, acting and the statistics take it
+        self.q_support = self.support
+        if self.value_transform is not None:
+            sup64 = torch.from_numpy(self.support.cpu().numpy().astype(np.float64))
+            self.q_support = vt_hinv(sup64, self.value_transform_eps).float().to(self.device)
         self.batch_size = args.batch_size
         self.n = args.multi_step
         self.discount = args.discount
@@ -592,6 +650,7 @@ class Agent:
         """Greedy action and its value for a batch of states [N, history, 84, 84] (device): conv body (cuDNN), fused
         noisy dueling head, then rb_q_values -- softmax over atoms, expectation over the support (agent.py:55) and the
         arg-max / max over actions in one launch; under the quantile distribution rb_qr_q_values, the mean over quantiles.
+        Under value rescaling the values are in return units: the expectation over q_support, or rb_qr_vt_q_values.
         Returns device tensors (actions int64[N], values float32[N]); nothing synchronises.  Falls back to plain torch ops
         for head shapes the fused kernels do not cover."""
         on = self.online_net
@@ -602,15 +661,21 @@ class Agent:
                 z, _, _ = on.head().forward(x)
                 best_a = torch.empty(N, dtype=torch.int64, device=self.device)
                 best_q = torch.empty(N, dtype=torch.float32, device=self.device)
-                if self.quantile:
-                    _lib.check(_lib.load().rb_qr_q_values(_lib.ptr(z), N, self.action_space, self.atoms, _lib.ptr(q_out),
-                                                          _lib.ptr(best_a), _lib.ptr(best_q), _lib.stream()))
+                lib, outs = _lib.load(), (_lib.ptr(q_out), _lib.ptr(best_a), _lib.ptr(best_q))
+                if self.quantile and self.value_transform is not None:
+                    _lib.check(lib.rb_qr_vt_q_values(_lib.ptr(z), N, self.action_space, self.atoms, *outs,
+                                                     self.value_transform_eps, _lib.stream()))
+                elif self.quantile:
+                    _lib.check(lib.rb_qr_q_values(_lib.ptr(z), N, self.action_space, self.atoms, *outs, _lib.stream()))
                 else:
-                    _lib.check(_lib.load().rb_q_values(_lib.ptr(z), N, self.action_space, self.atoms,
-                                                       _lib.ptr(self.support), _lib.ptr(q_out), _lib.ptr(best_a),
-                                                       _lib.ptr(best_q), _lib.stream()))
+                    _lib.check(lib.rb_q_values(_lib.ptr(z), N, self.action_space, self.atoms, _lib.ptr(self.q_support),
+                                               *outs, _lib.stream()))
                 return best_a, best_q
-            q = on.logits(states).mean(2) if self.quantile else (on(states) * self.support).sum(2)
+            if self.quantile:
+                q = on.logits(states)
+                q = (q if self.value_transform is None else vt_hinv(q, self.value_transform_eps)).mean(2)
+            else:
+                q = (on(states) * self.q_support).sum(2)
             if q_out is not None:
                 q_out.copy_(q)
             best_q, best_a = q.max(1)
@@ -887,12 +952,13 @@ class Agent:
         _, _, actions, returns, _, nonterminals, weights = batch
         m = self._stats_rows(actions.shape[0])
         rows = (z_online, z_target, self.action_space, self.atoms, actions, returns, nonterminals, weights)
+        vt = self._vt_args()
         if self.quantile:
-            return (*qr_dueling_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m), m)
+            return (*qr_dueling_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"]), m)
         c51 = (self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n())
         if (M, K) == (1, 1):
-            return (*c51_dueling_loss_grad(*rows, *c51, m_out=m), m)
-        return (*c51_dueling_avg_loss_grad(*rows, *c51, M, K, m_out=m), m)
+            return (*c51_dueling_loss_grad(*rows, *c51, m_out=m, **vt), m)
+        return (*c51_dueling_avg_loss_grad(*rows, *c51, M, K, m_out=m, **vt), m)
 
     def _library_loss(self, q_s, q_ns, q_t, batch):
         """The loss on the library head's logits [B, A, Z]: rb_qr_loss_grad (quantile) or rb_c51_loss_grad.  Returns
@@ -900,14 +966,20 @@ class Agent:
         _, _, actions, returns, _, nonterminals, weights = batch
         m = self._stats_rows(actions.shape[0])
         rows = (q_s, q_ns, q_t, actions, returns, nonterminals, weights)
+        vt = self._vt_args()
         if self.quantile:
-            return (*qr_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m), m)
-        return (*c51_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m), m)
+            return (*qr_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"]), m)
+        return (*c51_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m, **vt), m)
+
+    def _vt_args(self):
+        """The loss wrappers' value-rescaling arguments: eps None (the plain entries) when the transform is off."""
+        return dict(support_q=self.q_support if self.value_transform is not None else None, eps=self.value_transform_eps)
 
     def _stats_batch(self, batch, loss, m, z=None, q=None):
         """rb_learn_stats_batch on a side stream as soon as the losses exist: it runs beside the backward.  Returns the
         event _stats_write waits for (None with the statistics off).  The inputs of the latest record stay reachable in
-        self._stats["last"].  `m`: the loss kernel's stats rows (rb_learn_stats_batch_qr under the quantile loss)."""
+        self._stats["last"].  `m`: the loss kernel's stats rows (rb_learn_stats_batch_qr under the quantile loss).  Under
+        value rescaling the record is in return units: q_support in place of the support, or rb_learn_stats_batch_qr_vt."""
         if self._stats is None:
             return None
         lib, scratch = _lib.load(), _lib.ptr(self._stats["scratch"])
@@ -915,10 +987,12 @@ class Agent:
         tail = (_lib.ptr(z), _lib.ptr(q), loss.shape[0], self.action_space, self.atoms, scratch)
 
         def launch():
-            if self.quantile:
+            if self.quantile and self.value_transform is not None:
+                _lib.check(lib.rb_learn_stats_batch_qr_vt(*head, *tail, self.value_transform_eps, _lib.stream()))
+            elif self.quantile:
                 _lib.check(lib.rb_learn_stats_batch_qr(*head, *tail, _lib.stream()))
             else:
-                _lib.check(lib.rb_learn_stats_batch(*head, _lib.ptr(self.support), *tail, _lib.stream()))
+                _lib.check(lib.rb_learn_stats_batch(*head, _lib.ptr(self.q_support), *tail, _lib.stream()))
         done = _lib.side_branch(self._side_streams()[0], launch)[1]
         self._stats["last"] = dict(m=m, z=z, q=q)
         return done

@@ -375,6 +375,8 @@ def _meta(agent, mem):
         hyper["redo_tau"] = agent.redo_tau
     if agent.quantile:   # absent: categorical
         hyper["distribution"], hyper["quantile_kappa"] = agent.distribution, agent.quantile_kappa
+    if agent.value_transform is not None:   # absent: no value rescaling
+        hyper["value_transform"], hyper["value_transform_eps"] = agent.value_transform, agent.value_transform_eps
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
         learner["redo_count"] = agent.redo_count
     if opt.grouped:   # the group optimiser's bias-correction counts, [encoder, head]
@@ -515,6 +517,11 @@ def _validate(agent, mem, man):
     dist = (man.get("hyper_parameters") or {}).get("distribution", "categorical")
     if dist != agent.distribution:
         raise _Error(f"distribution differs: checkpoint {dist!r}, live {agent.distribution!r}")
+    # likewise a net trained in h units (value rescaling) would load silently as a plain one, or under another eps
+    hyper = man.get("hyper_parameters") or {}
+    vt = (hyper.get("value_transform"), hyper.get("value_transform_eps"))
+    if vt != (agent.value_transform, agent.value_transform_eps):
+        raise _Error(f"value transform differs: checkpoint {vt}, live {(agent.value_transform, agent.value_transform_eps)}")
     layout = agent.optimiser.state_dict(clone=False)["layout"]
     if man.get("optimiser") != layout:
         raise _Error(f"optimiser layout differs: checkpoint {man.get('optimiser')}, this learner {layout}")

@@ -976,6 +976,27 @@ k_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* __restric
 }
 
 // ================================================================================================
+// Value rescaling (Pohlen et al. 2018): h(x) = sign(x) (sqrt(|x| + 1) - 1) + eps x and its inverse, in cancellation-free
+// forms (DESIGN.md §16): every step adds or multiplies nonnegative terms, each rounded explicitly (no contraction), with
+// IEEE sqrtf and __fdiv_rn.  0 <= eps <= 1 (the host entries refuse anything else).
+//   h(x)      = sign(x) |x| / (sqrt(|x| + 1) + 1) + eps x
+//   h^-1(y)   = sign(y) d (d + 2),  d = 2|y| / ((1 + 2 eps) + sqrt((1 + 2 eps)^2 + 4 eps |y|))
+// ================================================================================================
+__device__ __forceinline__ float vt_h(float x, float eps) {
+  const float ax = fabsf(x);
+  const float r = __fdiv_rn(ax, __fadd_rn(sqrtf(__fadd_rn(ax, 1.0f)), 1.0f));
+  return __fadd_rn(copysignf(r, x), __fmul_rn(eps, x));
+}
+
+__device__ __forceinline__ float vt_hinv(float y, float eps) {
+  const float ay = fabsf(y);
+  const float c = __fadd_rn(1.0f, __fmul_rn(2.0f, eps));
+  const float disc = __fadd_rn(__fmul_rn(c, c), __fmul_rn(__fmul_rn(4.0f, eps), ay));
+  const float d = __fdiv_rn(__fmul_rn(2.0f, ay), __fadd_rn(c, sqrtf(disc)));
+  return copysignf(__fmul_rn(d, __fadd_rn(d, 2.0f)), y);
+}
+
+// ================================================================================================
 // K3  c51_loss_grad : double-DQN argmax + categorical projection + IS-weighted CE loss + gradient.
 // ================================================================================================
 // One warp per sample; lane owns atoms z = lane + 32*r.  The projected distribution is built as a
@@ -1040,13 +1061,17 @@ __device__ __forceinline__ float c51_expected_value(const float (&x)[C51_R], con
 
 // q_on_ns / q_tg_ns: A rows of Z (row stride Z); q_on_s_act: the row of the taken action.
 // best_known >= 0: a* was already determined by the caller (q_on_ns is then not read, q_tg_ns points at the row of a*).
-template <int C51_R>
+// VT (value rescaling): support_q = fl32(h^-1(support)) replaces the support in the arg-max and in Tz, and the target atoms
+// are h(r + fl32(scale * support_q)) (support itself is then not read); the projection onto the h-space grid is unchanged.
+template <int C51_R, bool VT = false>
 __device__ __forceinline__ void c51_core(C51Scratch& sc, int lane, int i, int B, int A, int Z, const float* q_on_ns,
                                          const float* q_tg_ns, const float* q_on_s_act, float ret, float nonterminal,
                                          float weight, const float* __restrict__ support, float vmin, float vmax,
                                          float delta_z, float gamma_n, float* __restrict__ loss, float* __restrict__ m_out,
-                                         int64_t* __restrict__ astar_out, float (&g)[C51_R], int best_known = -1) {
+                                         int64_t* __restrict__ astar_out, float (&g)[C51_R], int best_known = -1,
+                                         const float* __restrict__ support_q = nullptr, float eps = 0.0f) {
   float sup[C51_R];
+  if constexpr (VT) support = support_q;
 #pragma unroll
   for (int r = 0; r < C51_R; ++r) {
     int z = lane + 32 * r;
@@ -1103,6 +1128,7 @@ __device__ __forceinline__ void c51_core(C51Scratch& sc, int lane, int i, int B,
     int z = lane + 32 * r;
     if (z < Z) {
       float tz = __fadd_rn(ret, __fmul_rn(scale, sup[r]));
+      if constexpr (VT) tz = vt_h(tz, eps);
       tz = fminf(fmaxf(tz, vmin), vmax);
       float bb = __fdiv_rn(__fsub_rn(tz, vmin), delta_z);
       int lo = (int)floorf(bb), up = (int)ceilf(bb);
@@ -1116,7 +1142,7 @@ __device__ __forceinline__ void c51_core(C51Scratch& sc, int lane, int i, int B,
   __syncwarp();
 
   // ---- agent.py:89-92: m, deterministic gather in index_add_ order ----
-  // Tz is non-decreasing in the atom index (support increasing, scale >= 0) and u == l + 1 after the fix-ups, so
+  // Tz is non-decreasing in the atom index (support increasing, scale >= 0, h monotone) and u == l + 1 after the fix-ups, so
   // the source atoms feeding target k on the l side form the contiguous run {j : l[j] == k} and on the u side the
   // run {j : l[j] == k - 1}: two binary searches replace the 2*Z-long scans.  The additions still happen in atom
   // order, l side first (bit-identical to the scan).  Odd inputs (NaN, decreasing support) take the full scan.
@@ -1170,22 +1196,23 @@ __device__ __forceinline__ void c51_core(C51Scratch& sc, int lane, int i, int B,
   __syncwarp();
 }
 
-template <int C51_R>
+// VT: the value-rescaled instantiation (c51_core's VT); support_q / eps are read only there.
+template <int C51_R, bool VT>
 __global__ void __launch_bounds__(C51_WARPS * 32)
 k_c51(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
       const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
       const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax, float delta_z,
       float gamma_n, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ grad, float* __restrict__ m_out,
-      int64_t* __restrict__ astar_out) {
+      int64_t* __restrict__ astar_out, const float* __restrict__ support_q, float eps) {
   __shared__ C51Scratch s_sc[C51_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i = blockIdx.x * C51_WARPS + warp;
   if (i >= B) return;
   const int act = (int)actions[i];
   float g[C51_R];
-  c51_core<C51_R>(s_sc[warp], lane, i, B, A, Z, q_on_ns + (size_t)i * A * Z, q_tg_ns + (size_t)i * A * Z,
+  c51_core<C51_R, VT>(s_sc[warp], lane, i, B, A, Z, q_on_ns + (size_t)i * A * Z, q_tg_ns + (size_t)i * A * Z,
            q_on_s + ((size_t)i * A + act) * Z, __ldg(returns + i), __ldg(nonterminals + i), __ldg(weights + i), support, vmin,
-           vmax, delta_z, gamma_n, loss, m_out, astar_out, g);
+           vmax, delta_z, gamma_n, loss, m_out, astar_out, g, -1, support_q, eps);
   float* gq = grad + (size_t)i * A * Z;
   for (int j = lane; j < A * Z; j += 32) gq[j] = 0.0f;
   __syncwarp();
@@ -1208,12 +1235,13 @@ k_c51(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const
 //   phase 3  all threads write dz:  dzv[z] = g[z],  dza[a][z] = g[z] * ([a == act] - 1/A).
 constexpr int C51D_T = 256;
 
-template <int C51_R>
+template <int C51_R, bool VT>
 __global__ void __launch_bounds__(C51D_T)
 k_c51_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
               const float* __restrict__ returns, const float* __restrict__ nonterminals, const float* __restrict__ weights,
               const float* __restrict__ support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z,
-              float* __restrict__ loss, float* __restrict__ dz, float* __restrict__ m_out, int64_t* __restrict__ astar_out) {
+              float* __restrict__ loss, float* __restrict__ dz, float* __restrict__ m_out, int64_t* __restrict__ astar_out,
+              const float* __restrict__ support_q, float eps) {
   extern __shared__ __align__(16) float s_dyn[];
   __shared__ C51Scratch s_sc;
   const int N2 = Z + A * Z;
@@ -1247,8 +1275,10 @@ k_c51_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, co
   __syncthreads();
   const int act = (int)actions[i];
   float sup[C51_R];
+  const float* sup_ev = support;   // the arg-max's support: support_q under VT (return units)
+  if constexpr (VT) sup_ev = support_q;
 #pragma unroll
-  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(sup_ev + lane + 32 * r) : 0.0f;
   {  // phase 1: expected value of every action of online(s'), one warp per action
     const float* r1 = zs + N2;
     float mean[C51_R];
@@ -1299,8 +1329,9 @@ k_c51_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, co
     }
     __syncwarp();
     float g[C51_R];
-    c51_core<C51_R>(s_sc, lane, i, B, A, Z, nullptr, q_t, q_s, __ldg(returns + i), __ldg(nonterminals + i), __ldg(weights + i),
-                    support, vmin, vmax, delta_z, gamma_n, loss, m_out, astar_out, g, best);
+    c51_core<C51_R, VT>(s_sc, lane, i, B, A, Z, nullptr, q_t, q_s, __ldg(returns + i), __ldg(nonterminals + i),
+                        __ldg(weights + i), support, vmin, vmax, delta_z, gamma_n, loss, m_out, astar_out, g, best, support_q,
+                        eps);
 #pragma unroll
     for (int r = 0; r < C51_R; ++r)
       if (lane + 32 * r < Z) s_g[lane + 32 * r] = g[r];
@@ -1359,13 +1390,14 @@ __device__ __forceinline__ float c51_loss_row(int lane, int Z, const float* q_on
 //            wi = w / (M B);
 //   phase 5  loss = (sum_j loss_j in j order) / M; dz rows jB + i get phase 3 of k_c51_dueling.
 // At M = K = 1 every output is k_c51_dueling's, bitwise.
-template <int C51_R>
+template <int C51_R, bool VT>
 __global__ void __launch_bounds__(C51D_T)
 k_c51_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
                   const float* __restrict__ returns, const float* __restrict__ nonterminals,
                   const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax, float delta_z,
                   float gamma_n, int B, int A, int Z, int M, int K, float* __restrict__ loss, float* __restrict__ dz,
-                  float* __restrict__ m_out, int64_t* __restrict__ astar_out) {
+                  float* __restrict__ m_out, int64_t* __restrict__ astar_out, const float* __restrict__ support_q,
+                  float eps) {
   extern __shared__ __align__(16) float s_dyn[];
   __shared__ C51Scratch s_sc[C51D_T / 32];
   __shared__ float s_junk[C51D_T / 32];
@@ -1408,8 +1440,10 @@ k_c51_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg
   __syncthreads();
   const int act = (int)actions[i];
   float sup[C51_R];
+  const float* sup_ev = support;   // the arg-max's support: support_q under VT (return units)
+  if constexpr (VT) sup_ev = support_q;
 #pragma unroll
-  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(sup_ev + lane + 32 * r) : 0.0f;
   for (int t = warp; t < K * A; t += WARPS) {  // phase 1
     const int k = t / A, a = t - k * A;
     const float* r1 = on_ns + (size_t)k * N2;
@@ -1450,8 +1484,9 @@ k_c51_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg
     // c51_core with sample index 0 on per-copy outputs: m_k into s_m[k], a*_k into astar_out[k][i]; its loss row
     // (fed qt again) and gradient are not used
     float g[C51_R];
-    c51_core<C51_R>(s_sc[warp], lane, 0, B, A, Z, nullptr, qt, qt, ret, nt, w, support, vmin, vmax, delta_z, gamma_n,
-                    s_junk + warp, s_m + k * Z, astar_out ? astar_out + (size_t)k * B + i : nullptr, g, best);
+    c51_core<C51_R, VT>(s_sc[warp], lane, 0, B, A, Z, nullptr, qt, qt, ret, nt, w, support, vmin, vmax, delta_z, gamma_n,
+                        s_junk + warp, s_m + k * Z, astar_out ? astar_out + (size_t)k * B + i : nullptr, g, best, support_q,
+                        eps);
   }
   __syncthreads();
   for (int c = tid; c < Z; c += C51D_T) {  // phase 3
@@ -1652,12 +1687,14 @@ __device__ __forceinline__ void qr_core(const float* s_theta, const float* s_T, 
 }
 
 // Dueling entry point: z rows as k_c51_dueling takes them (online 2B rows, s then s'; target B rows).
-template <int R>
+// VT (value rescaling, quantiles in h units): a* = argmax_a mean_j h^-1(q_online(s', a)_j) and
+// T_j = h(r + fl32(scale * h^-1(q_target(s', a*)_j))); theta, the loss and the gradient stay in h units.
+template <int R, bool VT>
 __global__ void __launch_bounds__(QR_T)
 k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
              const float* __restrict__ returns, const float* __restrict__ nonterminals, const float* __restrict__ weights,
              float kappa, float gamma_n, int B, int A, int N, float* __restrict__ loss, float* __restrict__ dz,
-             float* __restrict__ theta_out, int64_t* __restrict__ astar_out) {
+             float* __restrict__ theta_out, int64_t* __restrict__ astar_out, float eps) {
   extern __shared__ __align__(16) float s_dyn[];
   const int N2 = N + A * N;
   float* zs = s_dyn;              // [3][N2]: online(s), online(s'), target(s')
@@ -1707,6 +1744,7 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
       for (int r = 0; r < R; ++r) {
         const int c = lane + 32 * r;
         x[r] = (c < N) ? r1[c] + r1[N + a * N + c] - mean[r] : 0.0f;
+        if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
       }
       const float q = qr_row_mean<R>(x, N);
       if (lane == 0) s_mean[a] = q;
@@ -1725,7 +1763,13 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
       m2 += r2[N + a * N + c];
     }
     s_theta[c] = r0[c] + r0[N + act * N + c] - m0 / (float)A;
-    const float T = __fadd_rn(ret, __fmul_rn(scale, r2[c] + r2[N + best * N + c] - m2 / (float)A));
+    float T;
+    if constexpr (VT) {
+      const float x = vt_hinv(r2[c] + r2[N + best * N + c] - m2 / (float)A, eps);
+      T = vt_h(__fadd_rn(ret, __fmul_rn(scale, x)), eps);
+    } else {
+      T = __fadd_rn(ret, __fmul_rn(scale, r2[c] + r2[N + best * N + c] - m2 / (float)A));
+    }
     s_T[c] = T;
     if (theta_out) theta_out[(size_t)i * N + c] = T;
   }
@@ -1747,12 +1791,12 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
 
 // Plain entry point: quantile rows [B][A][N] of online(s), online(s') and target(s'); grad [B][A][N] is the gradient row
 // at the taken action and 0 elsewhere.
-template <int R>
+template <int R, bool VT>
 __global__ void __launch_bounds__(QR_T)
 k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
      const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
      const float* __restrict__ weights, float kappa, float gamma_n, int B, int A, int N, float* __restrict__ loss,
-     float* __restrict__ grad, float* __restrict__ theta_out, int64_t* __restrict__ astar_out) {
+     float* __restrict__ grad, float* __restrict__ theta_out, int64_t* __restrict__ astar_out, float eps) {
   extern __shared__ __align__(16) float s_dyn[];
   float* s_theta = s_dyn;
   float* s_T = s_theta + N;
@@ -1767,6 +1811,7 @@ k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const 
     for (int r = 0; r < R; ++r) {
       const int c = lane + 32 * r;
       x[r] = (c < N) ? __ldg(q_on_ns + (row0 + a) * N + c) : 0.0f;
+      if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
     }
     const float q = qr_row_mean<R>(x, N);
     if (lane == 0) s_mean[a] = q;
@@ -1778,7 +1823,11 @@ k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const 
   const float ret = __ldg(returns + i), scale = __fmul_rn(__ldg(nonterminals + i), gamma_n);
   for (int c = tid; c < N; c += QR_T) {
     s_theta[c] = __ldg(q_on_s + (row0 + act) * N + c);
-    const float T = __fadd_rn(ret, __fmul_rn(scale, __ldg(q_tg_ns + (row0 + best) * N + c)));
+    float T;
+    if constexpr (VT)
+      T = vt_h(__fadd_rn(ret, __fmul_rn(scale, vt_hinv(__ldg(q_tg_ns + (row0 + best) * N + c), eps))), eps);
+    else
+      T = __fadd_rn(ret, __fmul_rn(scale, __ldg(q_tg_ns + (row0 + best) * N + c)));
     s_T[c] = T;
     if (theta_out) theta_out[(size_t)i * N + c] = T;
   }
@@ -1793,9 +1842,11 @@ k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const 
 
 // Greedy values for acting / evaluation under quantiles: k_q_select with the mean over quantiles in place of
 // softmax . support.  One warp per state; the dueling combination and the mean are k_qr_dueling's phase 1, bitwise.
+// VT: the mean of h^-1 of the quantiles (return units).
+template <bool VT>
 __global__ void __launch_bounds__(128)
 k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict__ q_out, int64_t* __restrict__ best_action,
-            float* __restrict__ best_q) {
+            float* __restrict__ best_q, float eps) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m = blockIdx.x * 4 + warp;
   if (m >= M) return;
@@ -1821,6 +1872,7 @@ k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict_
     for (int r = 0; r < R; ++r) {
       const int c = lane + 32 * r;
       x[r] = (c < N) ? zv[r] + __ldg(zr + N + a * N + c) - mean[r] : 0.0f;
+      if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
     }
     const float q = qr_row_mean<R>(x, N);
     if (q_out && lane == 0) q_out[(size_t)m * A + a] = q;
@@ -1995,11 +2047,13 @@ k_learn_stats_batch(const float* __restrict__ loss, const float* __restrict__ we
 
 // k_learn_stats_batch for the quantile loss: theta = the T rows [B][N] of the loss kernel (theta_out); per sample
 // q(s, a) = mean_i theta_i of the online quantiles of the taken action (dueling combination as k_qr_dueling forms it) and
-// the target value mean_j T_j; edge_mass is NaN (there is no support to clamp to).
+// the target value mean_j T_j; edge_mass is NaN (there is no support to clamp to).  VT: both means are of h^-1 of the
+// quantiles (return units).
+template <bool VT>
 __global__ void __launch_bounds__(STATS_THREADS)
 k_learn_stats_batch_qr(const float* __restrict__ loss, const float* __restrict__ weights, const int64_t* __restrict__ actions,
                        const float* __restrict__ theta, const float* __restrict__ z, const float* __restrict__ q, int B, int A,
-                       int N, double* __restrict__ scratch) {
+                       int N, double* __restrict__ scratch, float eps) {
   __shared__ double s_part[7][STATS_WARPS];
   __shared__ bool s_last;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -2024,6 +2078,10 @@ k_learn_stats_batch_qr(const float* __restrict__ loss, const float* __restrict__
           x[r] = __ldg(zr + c) + __ldg(zr + N + act * N + c) - mean / (float)A;
         } else {
           x[r] = __ldg(q + ((size_t)i * A + act) * N + c);
+        }
+        if constexpr (VT) {
+          t[r] = vt_hinv(t[r], eps);
+          x[r] = vt_hinv(x[r], eps);
         }
       }
     }
@@ -2838,26 +2896,76 @@ int rb_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* fram
                        stream, "rb_append_batch");
 }
 
+// The value-rescaled entries' own refusals: support_q (C51) given, 0 <= eps <= 1 (NaN refused).
+static int vt_check(const char* name, bool support_q_ok, float eps) {
+  char msg[128];
+  if (!support_q_ok) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (!(eps >= 0.0f && eps <= 1.0f)) {
+    snprintf(msg, sizeof msg, "%s: eps must be in [0, 1]", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  return RB_OK;
+}
+
+extern "C++" {   // the shared launchers are templates, which cannot have C linkage
+template <bool VT>
+static int c51_launch(const char* name, const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
+                      const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                      const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z,
+                      float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, const float* support_q, float eps,
+                      rb_stream_t stream) {
+  char msg[128];
+  if (!q_online_s || !q_online_ns || !q_target_ns || !actions || !returns || !nonterminals || !weights || !support ||
+      !loss || !grad_q_online_s) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (B <= 0 || A <= 0 || Z <= 1) {
+    snprintf(msg, sizeof msg, "%s: B, A > 0 and Z > 1 are required", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (Z > RB_MAX_ATOMS) {
+    snprintf(msg, sizeof msg, "%s: Z exceeds RB_MAX_ATOMS", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  const int ctas = (B + C51_WARPS - 1) / C51_WARPS;
+  { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
+    if (Z <= 64)
+      k_c51<2, VT><<<ctas, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
+                                                                   nonterminals, weights, support, vmin, vmax, delta_z,
+                                                                   gamma_n, B, A, Z, loss, grad_q_online_s, m_out,
+                                                                   astar_out, support_q, eps);
+    else
+      k_c51<4, VT><<<ctas, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
+                                                                   nonterminals, weights, support, vmin, vmax, delta_z,
+                                                                   gamma_n, B, A, Z, loss, grad_q_online_s, m_out,
+                                                                   astar_out, support_q, eps); }
+  return check_launch(name);
+}
+}
+
 int rb_c51_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
                      const float* returns, const float* nonterminals, const float* weights, const float* support,
                      float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z, float* loss,
                      float* grad_q_online_s, float* m_out, int64_t* astar_out, rb_stream_t stream) {
-  if (!q_online_s || !q_online_ns || !q_target_ns || !actions || !returns || !nonterminals || !weights || !support ||
-      !loss || !grad_q_online_s)
-    return fail(RB_ERR_INVAL, "rb_c51_loss_grad: null pointer");
-  if (B <= 0 || A <= 0 || Z <= 1) return fail(RB_ERR_INVAL, "rb_c51_loss_grad: B, A > 0 and Z > 1 are required");
-  if (Z > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_c51_loss_grad: Z exceeds RB_MAX_ATOMS");
-  const int ctas = (B + C51_WARPS - 1) / C51_WARPS;
-  { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
-    if (Z <= 64)
-      k_c51<2><<<ctas, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
-                                                               nonterminals, weights, support, vmin, vmax, delta_z, gamma_n,
-                                                               B, A, Z, loss, grad_q_online_s, m_out, astar_out);
-    else
-      k_c51<4><<<ctas, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
-                                                               nonterminals, weights, support, vmin, vmax, delta_z, gamma_n,
-                                                               B, A, Z, loss, grad_q_online_s, m_out, astar_out); }
-  return check_launch("rb_c51_loss_grad");
+  return c51_launch<false>("rb_c51_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights,
+                           support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss, grad_q_online_s, m_out, astar_out, nullptr,
+                           0.0f, stream);
+}
+
+int rb_c51_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                        const float* returns, const float* nonterminals, const float* weights, const float* support,
+                        float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z, float* loss,
+                        float* grad_q_online_s, float* m_out, int64_t* astar_out, const float* support_q, float eps,
+                        rb_stream_t stream) {
+  int rc = vt_check("rb_c51_vt_loss_grad", support_q != nullptr, eps);
+  if (rc != RB_OK) return rc;
+  return c51_launch<true>("rb_c51_vt_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals,
+                          weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss, grad_q_online_s, m_out, astar_out,
+                          support_q, eps, stream);
 }
 
 static int noisy_launch(float* const* weight_eps, float* const* bias_eps, const int* in_features, const int* out_features,
@@ -2921,59 +3029,135 @@ int rb_noisy_outer(float* const* weight_eps, float* const* bias_eps, const int* 
   return noisy_launch(weight_eps, bias_eps, in_features, out_features, n_layers, f_in, f_out, 0, nullptr, 1, stream);
 }
 
+extern "C++" {
+template <bool VT>
+static int c51_dueling_launch(const char* name, const float* z_online, const float* z_target, int actions_n, int atoms,
+                              const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                              const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss,
+                              float* dz, float* m_out, int64_t* astar_out, const float* support_q, float eps,
+                              rb_stream_t stream) {
+  char msg[128];
+  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !support || !loss || !dz) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  const int Z = atoms, A = actions_n;
+  if (B <= 0 || A <= 0 || Z <= 1) {
+    snprintf(msg, sizeof msg, "%s: B, actions > 0 and atoms > 1 are required", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (Z > RB_MAX_ATOMS) {
+    snprintf(msg, sizeof msg, "%s: atoms exceeds RB_MAX_ATOMS", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  const size_t smem = (size_t)(3 * (Z + A * Z) + 3 * Z + A) * sizeof(float);
+  if (smem > 200 * 1024) {
+    snprintf(msg, sizeof msg, "%s: actions * atoms too large", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  int rc_s = rbi::ensure_dynamic_smem(k_c51_dueling<2, VT>, smem, name);
+  if (rc_s == RB_OK) rc_s = rbi::ensure_dynamic_smem(k_c51_dueling<4, VT>, smem, name);
+  if (rc_s != RB_OK) return rc_s;
+  { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
+    if (Z <= 64)
+      k_c51_dueling<2, VT><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                      weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z,
+                                                                      loss, dz, m_out, astar_out, support_q, eps);
+    else
+      k_c51_dueling<4, VT><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                      weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z,
+                                                                      loss, dz, m_out, astar_out, support_q, eps); }
+  return check_launch(name);
+}
+}
+
 int rb_c51_dueling_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
                              const float* returns, const float* nonterminals, const float* weights, const float* support,
                              float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss, float* dz, float* m_out,
                              int64_t* astar_out, rb_stream_t stream) {
-  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !support || !loss || !dz)
-    return fail(RB_ERR_INVAL, "rb_c51_dueling_loss_grad: null pointer");
+  return c51_dueling_launch<false>("rb_c51_dueling_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
+                                   nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, loss, dz, m_out,
+                                   astar_out, nullptr, 0.0f, stream);
+}
+
+int rb_c51_dueling_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
+                                const float* returns, const float* nonterminals, const float* weights, const float* support,
+                                float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss, float* dz,
+                                float* m_out, int64_t* astar_out, const float* support_q, float eps, rb_stream_t stream) {
+  int rc = vt_check("rb_c51_dueling_vt_loss_grad", support_q != nullptr, eps);
+  if (rc != RB_OK) return rc;
+  return c51_dueling_launch<true>("rb_c51_dueling_vt_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
+                                  nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, loss, dz, m_out, astar_out,
+                                  support_q, eps, stream);
+}
+
+extern "C++" {
+template <bool VT>
+static int c51_dueling_avg_launch(const char* name, const float* z_online, const float* z_target, int actions_n, int atoms,
+                                  const int64_t* actions, const float* returns, const float* nonterminals,
+                                  const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                  float gamma_n, int B, int M, int K, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                  const float* support_q, float eps, rb_stream_t stream) {
+  char msg[128];
+  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !support || !loss || !dz) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
   const int Z = atoms, A = actions_n;
-  if (B <= 0 || A <= 0 || Z <= 1) return fail(RB_ERR_INVAL, "rb_c51_dueling_loss_grad: B, actions > 0 and atoms > 1 are required");
-  if (Z > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_c51_dueling_loss_grad: atoms exceeds RB_MAX_ATOMS");
-  const size_t smem = (size_t)(3 * (Z + A * Z) + 3 * Z + A) * sizeof(float);
-  if (smem > 200 * 1024) return fail(RB_ERR_RANGE, "rb_c51_dueling_loss_grad: actions * atoms too large");
-  int rc_s = rbi::ensure_dynamic_smem(k_c51_dueling<2>, smem, "rb_c51_dueling_loss_grad");
-  if (rc_s == RB_OK) rc_s = rbi::ensure_dynamic_smem(k_c51_dueling<4>, smem, "rb_c51_dueling_loss_grad");
+  if (B <= 0 || A <= 0 || Z <= 1) {
+    snprintf(msg, sizeof msg, "%s: B, actions > 0 and atoms > 1 are required", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (Z > RB_MAX_ATOMS) {
+    snprintf(msg, sizeof msg, "%s: atoms exceeds RB_MAX_ATOMS", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  if (M < 1 || M > RB_MAX_AUG_COPIES || K < 1 || K > RB_MAX_AUG_COPIES) {
+    snprintf(msg, sizeof msg, "%s: copies outside [1, RB_MAX_AUG_COPIES]", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  const size_t smem = (size_t)((M + 2 * K) * (Z + A * Z) + (2 * M + 2 * K + 1) * Z + K * A + M) * sizeof(float);
+  if (smem > 200 * 1024) {
+    snprintf(msg, sizeof msg, "%s: (M + 2K) * actions * atoms too large", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  int rc_s = rbi::ensure_dynamic_smem(k_c51_dueling_avg<2, VT>, smem, name);
+  if (rc_s == RB_OK) rc_s = rbi::ensure_dynamic_smem(k_c51_dueling_avg<4, VT>, smem, name);
   if (rc_s != RB_OK) return rc_s;
-  { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
+  { ProfScope prof_(RB_K_C51_DUELING_AVG, (cudaStream_t)stream);
     if (Z <= 64)
-      k_c51_dueling<2><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights,
-                                                                  support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss, dz, m_out,
-                                                                  astar_out);
+      k_c51_dueling_avg<2, VT><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                          weights, support, vmin, vmax, delta_z, gamma_n, B,
+                                                                          A, Z, M, K, loss, dz, m_out, astar_out, support_q,
+                                                                          eps);
     else
-      k_c51_dueling<4><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights,
-                                                                  support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss, dz, m_out,
-                                                                  astar_out); }
-  return check_launch("rb_c51_dueling_loss_grad");
+      k_c51_dueling_avg<4, VT><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                          weights, support, vmin, vmax, delta_z, gamma_n, B,
+                                                                          A, Z, M, K, loss, dz, m_out, astar_out, support_q,
+                                                                          eps); }
+  return check_launch(name);
+}
 }
 
 int rb_c51_dueling_avg_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
                                  const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
                                  const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int M,
                                  int K, float* loss, float* dz, float* m_out, int64_t* astar_out, rb_stream_t stream) {
-  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !support || !loss || !dz)
-    return fail(RB_ERR_INVAL, "rb_c51_dueling_avg_loss_grad: null pointer");
-  const int Z = atoms, A = actions_n;
-  if (B <= 0 || A <= 0 || Z <= 1)
-    return fail(RB_ERR_INVAL, "rb_c51_dueling_avg_loss_grad: B, actions > 0 and atoms > 1 are required");
-  if (Z > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_c51_dueling_avg_loss_grad: atoms exceeds RB_MAX_ATOMS");
-  if (M < 1 || M > RB_MAX_AUG_COPIES || K < 1 || K > RB_MAX_AUG_COPIES)
-    return fail(RB_ERR_RANGE, "rb_c51_dueling_avg_loss_grad: copies outside [1, RB_MAX_AUG_COPIES]");
-  const size_t smem = (size_t)((M + 2 * K) * (Z + A * Z) + (2 * M + 2 * K + 1) * Z + K * A + M) * sizeof(float);
-  if (smem > 200 * 1024) return fail(RB_ERR_RANGE, "rb_c51_dueling_avg_loss_grad: (M + 2K) * actions * atoms too large");
-  int rc_s = rbi::ensure_dynamic_smem(k_c51_dueling_avg<2>, smem, "rb_c51_dueling_avg_loss_grad");
-  if (rc_s == RB_OK) rc_s = rbi::ensure_dynamic_smem(k_c51_dueling_avg<4>, smem, "rb_c51_dueling_avg_loss_grad");
-  if (rc_s != RB_OK) return rc_s;
-  { ProfScope prof_(RB_K_C51_DUELING_AVG, (cudaStream_t)stream);
-    if (Z <= 64)
-      k_c51_dueling_avg<2><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                      weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z,
-                                                                      M, K, loss, dz, m_out, astar_out);
-    else
-      k_c51_dueling_avg<4><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                      weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z,
-                                                                      M, K, loss, dz, m_out, astar_out); }
-  return check_launch("rb_c51_dueling_avg_loss_grad");
+  return c51_dueling_avg_launch<false>("rb_c51_dueling_avg_loss_grad", z_online, z_target, actions_n, atoms, actions,
+                                       returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, M, K, loss,
+                                       dz, m_out, astar_out, nullptr, 0.0f, stream);
+}
+
+int rb_c51_dueling_avg_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                    const int64_t* actions, const float* returns, const float* nonterminals,
+                                    const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                    float gamma_n, int B, int M, int K, float* loss, float* dz, float* m_out,
+                                    int64_t* astar_out, const float* support_q, float eps, rb_stream_t stream) {
+  int rc = vt_check("rb_c51_dueling_avg_vt_loss_grad", support_q != nullptr, eps);
+  if (rc != RB_OK) return rc;
+  return c51_dueling_avg_launch<true>("rb_c51_dueling_avg_vt_loss_grad", z_online, z_target, actions_n, atoms, actions,
+                                      returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, M, K, loss,
+                                      dz, m_out, astar_out, support_q, eps, stream);
 }
 
 int rb_q_values(const float* z, int M, int actions, int atoms, const float* support, float* q, int64_t* best_action,
@@ -3004,65 +3188,148 @@ static int qr_check(const char* name, int B, int A, int N, float kappa) {
   return RB_OK;
 }
 
-int rb_qr_dueling_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
-                            const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
-                            int B, float* loss, float* dz, float* theta_out, int64_t* astar_out, rb_stream_t stream) {
-  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !loss || !dz)
-    return fail(RB_ERR_INVAL, "rb_qr_dueling_loss_grad: null pointer");
+extern "C++" {
+template <bool VT>
+static int qr_dueling_launch(const char* name, const float* z_online, const float* z_target, int actions_n, int atoms,
+                             const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                             float kappa, float gamma_n, int B, float* loss, float* dz, float* theta_out, int64_t* astar_out,
+                             float eps, rb_stream_t stream) {
+  char msg[128];
+  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !loss || !dz) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
   const int N = atoms, A = actions_n;
-  int rc = qr_check("rb_qr_dueling_loss_grad", B, A, N, kappa);
+  int rc = qr_check(name, B, A, N, kappa);
   if (rc != RB_OK) return rc;
   const size_t smem = (size_t)(3 * (N + A * N) + 4 * N + A) * sizeof(float);
-  if (smem > 200 * 1024) return fail(RB_ERR_RANGE, "rb_qr_dueling_loss_grad: actions * atoms too large");
-  rc = rbi::ensure_dynamic_smem(k_qr_dueling<2>, smem, "rb_qr_dueling_loss_grad");
-  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<4>, smem, "rb_qr_dueling_loss_grad");
+  if (smem > 200 * 1024) {
+    snprintf(msg, sizeof msg, "%s: actions * atoms too large", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  rc = rbi::ensure_dynamic_smem(k_qr_dueling<2, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<4, VT>, smem, name);
   if (rc != RB_OK) return rc;
   { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
     if (N <= 64)
-      k_qr_dueling<2><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights,
-                                                              kappa, gamma_n, B, A, N, loss, dz, theta_out, astar_out);
+      k_qr_dueling<2, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                  weights, kappa, gamma_n, B, A, N, loss, dz, theta_out,
+                                                                  astar_out, eps);
     else
-      k_qr_dueling<4><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights,
-                                                              kappa, gamma_n, B, A, N, loss, dz, theta_out, astar_out); }
-  return check_launch("rb_qr_dueling_loss_grad");
+      k_qr_dueling<4, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                  weights, kappa, gamma_n, B, A, N, loss, dz, theta_out,
+                                                                  astar_out, eps); }
+  return check_launch(name);
+}
+}
+
+int rb_qr_dueling_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
+                            const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
+                            int B, float* loss, float* dz, float* theta_out, int64_t* astar_out, rb_stream_t stream) {
+  return qr_dueling_launch<false>("rb_qr_dueling_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
+                                  nonterminals, weights, kappa, gamma_n, B, loss, dz, theta_out, astar_out, 0.0f, stream);
+}
+
+int rb_qr_dueling_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms, const int64_t* actions,
+                               const float* returns, const float* nonterminals, const float* weights, float kappa,
+                               float gamma_n, int B, float* loss, float* dz, float* theta_out, int64_t* astar_out, float eps,
+                               rb_stream_t stream) {
+  int rc = vt_check("rb_qr_dueling_vt_loss_grad", true, eps);
+  if (rc != RB_OK) return rc;
+  return qr_dueling_launch<true>("rb_qr_dueling_vt_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
+                                 nonterminals, weights, kappa, gamma_n, B, loss, dz, theta_out, astar_out, eps, stream);
+}
+
+extern "C++" {
+template <bool VT>
+static int qr_launch(const char* name, const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
+                     const int64_t* actions, const float* returns, const float* nonterminals, const float* weights, float kappa,
+                     float gamma_n, int B, int A, int N, float* loss, float* grad_q_online_s, float* theta_out,
+                     int64_t* astar_out, float eps, rb_stream_t stream) {
+  char msg[128];
+  if (!q_online_s || !q_online_ns || !q_target_ns || !actions || !returns || !nonterminals || !weights || !loss ||
+      !grad_q_online_s) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  int rc = qr_check(name, B, A, N, kappa);
+  if (rc != RB_OK) return rc;
+  const size_t smem = (size_t)(4 * N + A) * sizeof(float);
+  if (smem > 200 * 1024) {
+    snprintf(msg, sizeof msg, "%s: too many actions", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  rc = rbi::ensure_dynamic_smem(k_qr<2, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<4, VT>, smem, name);
+  if (rc != RB_OK) return rc;
+  { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
+    if (N <= 64)
+      k_qr<2, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
+                                                          nonterminals, weights, kappa, gamma_n, B, A, N, loss,
+                                                          grad_q_online_s, theta_out, astar_out, eps);
+    else
+      k_qr<4, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
+                                                          nonterminals, weights, kappa, gamma_n, B, A, N, loss,
+                                                          grad_q_online_s, theta_out, astar_out, eps); }
+  return check_launch(name);
+}
 }
 
 int rb_qr_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
                     const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n, int B,
                     int A, int N, float* loss, float* grad_q_online_s, float* theta_out, int64_t* astar_out,
                     rb_stream_t stream) {
-  if (!q_online_s || !q_online_ns || !q_target_ns || !actions || !returns || !nonterminals || !weights || !loss ||
-      !grad_q_online_s)
-    return fail(RB_ERR_INVAL, "rb_qr_loss_grad: null pointer");
-  int rc = qr_check("rb_qr_loss_grad", B, A, N, kappa);
+  return qr_launch<false>("rb_qr_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights,
+                          kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, 0.0f, stream);
+}
+
+int rb_qr_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                       const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
+                       int B, int A, int N, float* loss, float* grad_q_online_s, float* theta_out, int64_t* astar_out,
+                       float eps, rb_stream_t stream) {
+  int rc = vt_check("rb_qr_vt_loss_grad", true, eps);
   if (rc != RB_OK) return rc;
-  const size_t smem = (size_t)(4 * N + A) * sizeof(float);
-  if (smem > 200 * 1024) return fail(RB_ERR_RANGE, "rb_qr_loss_grad: too many actions");
-  rc = rbi::ensure_dynamic_smem(k_qr<2>, smem, "rb_qr_loss_grad");
-  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<4>, smem, "rb_qr_loss_grad");
-  if (rc != RB_OK) return rc;
-  { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
-    if (N <= 64)
-      k_qr<2><<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals,
-                                                      weights, kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out,
-                                                      astar_out);
-    else
-      k_qr<4><<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals,
-                                                      weights, kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out,
-                                                      astar_out); }
-  return check_launch("rb_qr_loss_grad");
+  return qr_launch<true>("rb_qr_vt_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights,
+                         kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, eps, stream);
+}
+
+extern "C++" {
+template <bool VT>
+static int qr_q_values_launch(const char* name, const float* z, int M, int actions, int atoms, float* q,
+                              int64_t* best_action, float* best_q, float eps, rb_stream_t stream) {
+  char msg[128];
+  if (!z) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (!q && !best_action && !best_q) {
+    snprintf(msg, sizeof msg, "%s: no output requested", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (M <= 0 || actions <= 0 || atoms <= 1) {
+    snprintf(msg, sizeof msg, "%s: M, actions > 0 and atoms > 1 are required", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (atoms > RB_MAX_ATOMS) {
+    snprintf(msg, sizeof msg, "%s: atoms exceeds RB_MAX_ATOMS", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  { ProfScope prof_(RB_K_Q_VALUES, (cudaStream_t)stream);
+    k_qr_select<VT><<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, q, best_action, best_q, eps); }
+  return check_launch(name);
+}
 }
 
 int rb_qr_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
                    rb_stream_t stream) {
-  if (!z) return fail(RB_ERR_INVAL, "rb_qr_q_values: null pointer");
-  if (!q && !best_action && !best_q) return fail(RB_ERR_INVAL, "rb_qr_q_values: no output requested");
-  if (M <= 0 || actions <= 0 || atoms <= 1)
-    return fail(RB_ERR_INVAL, "rb_qr_q_values: M, actions > 0 and atoms > 1 are required");
-  if (atoms > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_qr_q_values: atoms exceeds RB_MAX_ATOMS");
-  { ProfScope prof_(RB_K_Q_VALUES, (cudaStream_t)stream);
-    k_qr_select<<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, q, best_action, best_q); }
-  return check_launch("rb_qr_q_values");
+  return qr_q_values_launch<false>("rb_qr_q_values", z, M, actions, atoms, q, best_action, best_q, 0.0f, stream);
+}
+
+int rb_qr_vt_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
+                      float eps, rb_stream_t stream) {
+  int rc = vt_check("rb_qr_vt_q_values", true, eps);
+  if (rc != RB_OK) return rc;
+  return qr_q_values_launch<true>("rb_qr_vt_q_values", z, M, actions, atoms, q, best_action, best_q, eps, stream);
 }
 
 static int stats_batch_check(const float* loss, const float* weights, const int64_t* actions, const float* m,
@@ -3095,18 +3362,50 @@ int rb_learn_stats_batch(const float* loss, const float* weights, const int64_t*
   return check_launch("rb_learn_stats_batch");
 }
 
-int rb_learn_stats_batch_qr(const float* loss, const float* weights, const int64_t* actions, const float* theta, const float* z,
-                            const float* q, int B, int A, int N, double* scratch, rb_stream_t stream) {
-  if (!loss || !weights || !actions || !theta || !scratch) return fail(RB_ERR_INVAL, "rb_learn_stats_batch_qr: null pointer");
-  if ((z == nullptr) == (q == nullptr)) return fail(RB_ERR_INVAL, "rb_learn_stats_batch_qr: give exactly one of z and q");
-  if (B <= 0 || A <= 0 || N <= 1) return fail(RB_ERR_INVAL, "rb_learn_stats_batch_qr: B, A > 0 and N > 1 are required");
-  if (N > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_learn_stats_batch_qr: N exceeds RB_MAX_ATOMS");
+extern "C++" {
+template <bool VT>
+static int stats_batch_qr_launch(const char* name, const float* loss, const float* weights, const int64_t* actions,
+                                 const float* theta, const float* z, const float* q, int B, int A, int N, double* scratch,
+                                 float eps, rb_stream_t stream) {
+  char msg[128];
+  if (!loss || !weights || !actions || !theta || !scratch) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if ((z == nullptr) == (q == nullptr)) {
+    snprintf(msg, sizeof msg, "%s: give exactly one of z and q", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (B <= 0 || A <= 0 || N <= 1) {
+    snprintf(msg, sizeof msg, "%s: B, A > 0 and N > 1 are required", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (N > RB_MAX_ATOMS) {
+    snprintf(msg, sizeof msg, "%s: N exceeds RB_MAX_ATOMS", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
   int ctas = (B + STATS_WARPS - 1) / STATS_WARPS;
   if (ctas > STATS_MAX_CTAS) ctas = STATS_MAX_CTAS;
   { ProfScope prof_(RB_K_LEARN_STATS, (cudaStream_t)stream);
-    k_learn_stats_batch_qr<<<ctas, STATS_THREADS, 0, (cudaStream_t)stream>>>(loss, weights, actions, theta, z, q, B, A, N,
-                                                                             scratch); }
-  return check_launch("rb_learn_stats_batch_qr");
+    k_learn_stats_batch_qr<VT><<<ctas, STATS_THREADS, 0, (cudaStream_t)stream>>>(loss, weights, actions, theta, z, q, B, A,
+                                                                                 N, scratch, eps); }
+  return check_launch(name);
+}
+}
+
+int rb_learn_stats_batch_qr(const float* loss, const float* weights, const int64_t* actions, const float* theta, const float* z,
+                            const float* q, int B, int A, int N, double* scratch, rb_stream_t stream) {
+  return stats_batch_qr_launch<false>("rb_learn_stats_batch_qr", loss, weights, actions, theta, z, q, B, A, N, scratch, 0.0f,
+                                      stream);
+}
+
+int rb_learn_stats_batch_qr_vt(const float* loss, const float* weights, const int64_t* actions, const float* theta,
+                               const float* z, const float* q, int B, int A, int N, double* scratch, float eps,
+                               rb_stream_t stream) {
+  int rc = vt_check("rb_learn_stats_batch_qr_vt", true, eps);
+  if (rc != RB_OK) return rc;
+  return stats_batch_qr_launch<true>("rb_learn_stats_batch_qr_vt", loss, weights, actions, theta, z, q, B, A, N, scratch, eps,
+                                     stream);
 }
 
 int rb_learn_stats_write(const double* scratch, const float* grad_norm, const int32_t* gate, float max_norm,
