@@ -441,6 +441,33 @@ int rb_qr_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const 
 int rb_qr_vt_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
                       float eps, rb_stream_t stream);
 
+/* rb_qr_dueling_loss_grad with DrQ's averaging over K target copies and M online copies, rows as
+ * rb_c51_dueling_avg_loss_grad takes them: z_online has (M + K) B rows, copy j of s at row jB + i, then copy k of s' at
+ * row (M + k) B + i; z_target K B rows, copy k of s' at row kB + i.  For sample i:
+ *   a*_k = argmax_a (1/N) sum_n q_online(s'_k, a)_n (first maximum wins),
+ *   T_k,n = rb_qr_dueling_loss_grad's target row from target(s'_k) at a*_k,
+ *   Tbar_n = (sum_k T_k,n, fp32 in k order) / K, rounded once: the quantile-wise average of the K target quantile
+ *            functions (its mean is DrQ's averaged target value), not the mixture of their K N samples,
+ *   loss_j, g_j = rb_qr_dueling_loss_grad's loss and gradient row of online(s_j) at the taken action against Tbar, with
+ *            weight / (M B) in place of weight / B,
+ *   loss[i] = (sum_j loss_j, fp32 in j order) / M (also the priority).
+ * dz[M B][atoms*(1+actions)]: row jB + i is g_j through the dueling backward.  theta_out [B][atoms] (optional) receives
+ * Tbar, so rb_learn_stats_batch_qr takes it unchanged; astar_out [K][B] (optional) a*_k.  At M = K = 1 every output
+ * equals rb_qr_dueling_loss_grad's, bitwise.  RB_ERR_INVAL: a NULL required pointer, B, actions <= 0, atoms < 2 or a bad
+ * kappa; RB_ERR_RANGE: M or K outside [1, RB_MAX_AUG_COPIES], atoms > RB_MAX_ATOMS, or the M + 2K staged rows too large
+ * for shared memory.  A refused call writes nothing.  Profiled under RB_K_C51_DUELING_AVG. */
+int rb_qr_dueling_avg_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                                float kappa, float gamma_n, int B, int M, int K, float* loss, float* dz, float* theta_out,
+                                int64_t* astar_out, rb_stream_t stream);
+/* rb_qr_dueling_avg_loss_grad under value rescaling: a*_k and T_k as rb_qr_dueling_vt_loss_grad forms them, Tbar averaged
+ * in h units; also RB_ERR_INVAL for eps outside [0, 1] or NaN.  At M = K = 1 every output equals
+ * rb_qr_dueling_vt_loss_grad's, bitwise.  Profiled under RB_K_C51_DUELING_AVG. */
+int rb_qr_dueling_avg_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                   const int64_t* actions, const float* returns, const float* nonterminals,
+                                   const float* weights, float kappa, float gamma_n, int B, int M, int K, float* loss,
+                                   float* dz, float* theta_out, int64_t* astar_out, float eps, rb_stream_t stream);
+
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */
 int rb_noisy_compose(const float* mu, const float* sigma, const float* eps, int64_t count, float* out,

@@ -152,6 +152,11 @@ SIGNATURES = {
                                      _f32, _vp]),
     "rb_qr_vt_q_values": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _f32, _vp]),
     "rb_learn_stats_batch_qr_vt": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _f32, _vp]),
+    # DrQ's K / M averaging under the quantile loss: rb_qr_dueling(_vt)_loss_grad's signature with M, K after B
+    "rb_qr_dueling_avg_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _i32, _i32, _vp,
+                                              _vp, _vp, _vp, _vp]),
+    "rb_qr_dueling_avg_vt_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _i32, _i32,
+                                                 _vp, _vp, _vp, _vp, _f32, _vp]),
 }
 
 # rb_learn_stats_record of include/rainbow_b200.h (48 bytes): field name -> numpy dtype, in memory order

@@ -18,7 +18,9 @@ One `learn(mem)` (agent.py:61-100) is:
                                               [M or K > 1: rb_c51_dueling_avg_loss_grad -- DrQ's target averaged over
                                                the K copies of s', loss over the M copies of s;
                                                args.distribution = "quantile": rb_qr_dueling_loss_grad -- QR-DQN's
-                                               quantile Huber loss, no support or projection]
+                                               quantile Huber loss, no support or projection; with M or K > 1
+                                               (args.quantile_average_copies) rb_qr_dueling_avg_loss_grad -- the target
+                                               quantiles averaged over the K copies, the loss over the M copies]
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
@@ -141,6 +143,25 @@ def qr_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns,
     return loss, dz
 
 
+def qr_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, kappa, gamma_n,
+                             M, K, theta_out=None, astar_out=None, eps=None):
+    """DrQ's K / M averaging under the quantile loss (rb_qr_dueling_avg_loss_grad), rows as c51_dueling_avg_loss_grad takes
+    them; returns (loss[B], dz[M B, N(1+A)]): the loss averaged over the M online copies against the quantile-wise average
+    of the K target copies' quantiles, and its gradient for every online copy of s.  eps given: value rescaling
+    (rb_qr_dueling_avg_vt_loss_grad)."""
+    B = actions.shape[0]
+    loss = torch.empty(B, dtype=torch.float32, device=actions.device)
+    dz = torch.empty((M * B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
+    lib = _lib.load()
+    fn, vt = ((lib.rb_qr_dueling_avg_loss_grad, ()) if eps is None else
+              (lib.rb_qr_dueling_avg_vt_loss_grad, (float(eps),)))
+    _lib.check(fn(
+        _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+        _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, M, K, _lib.ptr(loss), _lib.ptr(dz),
+        _lib.ptr(theta_out), _lib.ptr(astar_out), *vt, _lib.stream()))
+    return loss, dz
+
+
 DISTRIBUTIONS = ("categorical", "quantile")
 
 
@@ -164,10 +185,24 @@ def distribution_options(args):
     if not 2 <= args.atoms <= 128:
         raise ValueError(f"distribution 'quantile' needs 2 <= atoms <= 128 quantiles, got {args.atoms}")
     copies = (getattr(args, "augment_m", 1), getattr(args, "augment_k", 1))
-    if copies != (1, 1):
+    if copies != (1, 1) and not quantile_average_switch(args):
         raise ValueError(f"augment_m / augment_k = {copies} average categorical targets; with distribution 'quantile' "
-                         f"both must be 1")
+                         f"both must be 1, or set args.quantile_average_copies = True to average the K copies' target "
+                         f"quantiles quantile by quantile")
     return dist, kappa
+
+
+def quantile_average_switch(args):
+    """args.quantile_average_copies (absent or None: False), checked to be a bool.  True lets distribution "quantile" take
+    DrQ's augment_m / augment_k copies: the target is the quantile-wise average of the K target copies' quantile rows,
+    the loss the mean over the M online copies (rb_qr_dueling_avg_loss_grad).  It is read only under the quantile
+    distribution with copies other than (1, 1); elsewhere it changes nothing."""
+    v = getattr(args, "quantile_average_copies", None)
+    if v is None:
+        return False
+    if not isinstance(v, (bool, np.bool_)):
+        raise ValueError(f"quantile_average_copies must be a bool, got {v!r}")
+    return bool(v)
 
 
 def value_transform_options(args):
@@ -535,6 +570,8 @@ class Agent:
         # the distributional loss: C51's categorical projection (default) or quantile regression (QR-DQN)
         self.distribution, self.quantile_kappa = distribution_options(args)
         self.quantile = self.distribution == "quantile"
+        # the quantile loss with DrQ's copies (opt-in, args.quantile_average_copies): True only where it is in effect
+        self.quantile_average_copies = self.quantile and self.augment_copies != (1, 1)
         # Polyak target updates (tau > 0: every applied optimiser step also moves the target, DrQ(eps) / SPR / BBF) and
         # periodic shrink-and-perturb resets of the online net (SR-SPR, BBF); both off by default
         self.target_tau, self.reset_interval, self.reset_shrink = target_reset_options(args)
@@ -946,15 +983,18 @@ class Agent:
         return torch.empty((B, self.atoms), dtype=torch.float32, device=self.device) if self._stats is not None else None
 
     def _fused_loss(self, z_online, z_target, batch, M, K):
-        """The loss on the fused heads' rows for M copies of s and K of s': rb_qr_dueling_loss_grad (quantile; M = K = 1,
-        the Agent refuses copies), rb_c51_dueling_loss_grad, or at M or K > 1 rb_c51_dueling_avg_loss_grad.  Returns
-        (loss[B], dz, stats rows)."""
+        """The loss on the fused heads' rows for M copies of s and K of s': rb_qr_dueling_loss_grad (quantile, M = K = 1)
+        or rb_qr_dueling_avg_loss_grad (quantile, M or K > 1: args.quantile_average_copies), rb_c51_dueling_loss_grad, or
+        at M or K > 1 rb_c51_dueling_avg_loss_grad.  Returns (loss[B], dz, stats rows)."""
         _, _, actions, returns, _, nonterminals, weights = batch
         m = self._stats_rows(actions.shape[0])
         rows = (z_online, z_target, self.action_space, self.atoms, actions, returns, nonterminals, weights)
         vt = self._vt_args()
-        if self.quantile:
+        if self.quantile and (M, K) == (1, 1):
             return (*qr_dueling_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"]), m)
+        if self.quantile:
+            return (*qr_dueling_avg_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), M, K, theta_out=m,
+                                              eps=vt["eps"]), m)
         c51 = (self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n())
         if (M, K) == (1, 1):
             return (*c51_dueling_loss_grad(*rows, *c51, m_out=m, **vt), m)

@@ -377,6 +377,8 @@ def _meta(agent, mem):
         hyper["distribution"], hyper["quantile_kappa"] = agent.distribution, agent.quantile_kappa
     if agent.value_transform is not None:   # absent: no value rescaling
         hyper["value_transform"], hyper["value_transform_eps"] = agent.value_transform, agent.value_transform_eps
+    if agent.quantile_average_copies:   # absent: the quantile loss does not average copies
+        hyper["quantile_average_copies"] = True
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
         learner["redo_count"] = agent.redo_count
     if opt.grouped:   # the group optimiser's bias-correction counts, [encoder, head]
@@ -522,6 +524,10 @@ def _validate(agent, mem, man):
     vt = (hyper.get("value_transform"), hyper.get("value_transform_eps"))
     if vt != (agent.value_transform, agent.value_transform_eps):
         raise _Error(f"value transform differs: checkpoint {vt}, live {(agent.value_transform, agent.value_transform_eps)}")
+    # and a net trained against the quantile-wise average of K target copies would resume under another loss
+    qavg = hyper.get("quantile_average_copies", False)
+    if qavg is not agent.quantile_average_copies:
+        raise _Error(f"quantile_average_copies differs: checkpoint {qavg!r}, live {agent.quantile_average_copies!r}")
     layout = agent.optimiser.state_dict(clone=False)["layout"]
     if man.get("optimiser") != layout:
         raise _Error(f"optimiser layout differs: checkpoint {man.get('optimiser')}, this learner {layout}")

@@ -1641,7 +1641,9 @@ __device__ __forceinline__ int qr_argmax(const float* s_mean, int A) {
 }
 
 // Phases 3 and 4 (without the gradient write) from the rows s_theta, s_T [N] in shared memory: s_g [N] receives the
-// gradient row of the taken action, loss[i_sample] the loss; s_l is N floats of scratch.  s_g is complete on return.
+// gradient row of the taken action, loss[i_sample] the loss (written by warp 0; loss may be global or shared: the
+// averaging kernel passes its per-copy slots); s_l is N floats of scratch.  s_g is complete on return; a caller that
+// runs it again on the same s_l synchronises first (warp 0 may still read it).
 template <int R>
 __device__ __forceinline__ void qr_core(const float* s_theta, const float* s_T, float* s_l, float* s_g, int N, float kappa,
                                         float wi, int i_sample, float* __restrict__ loss) {
@@ -1784,6 +1786,136 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
       } else {
         const int a = (idx - N) / N, c = (idx - N) - a * N;
         dzi[idx] = s_g[c] * ((a == act ? 1.0f : 0.0f) - inv_a);
+      }
+    }
+  }
+}
+
+// DrQ's K / M averaging under the quantile loss: z rows as k_c51_dueling_avg takes them (z_on (M + K) B rows, copy j of s
+// at row jB + i, copy k of s' at row (M + k) B + i; z_tg K B rows, copy k of s' at row kB + i).  ONE CTA PER SAMPLE with
+// the sample's M + 2K z rows staged in shared memory:
+//   phase 1  the mean quantile of every (target copy k, action a) of online(s'_k), one warp per pair (k_qr_dueling's
+//            phase 1 per pair, bitwise);
+//   phase 2  thread k: a*_k (first maximum wins); then per quantile n, T_k,n as k_qr_dueling forms it and
+//            Tbar_n = (sum_k T_k,n in k order) / K, rounded once -- the quantile-wise average of the K target quantile
+//            functions (in h units under VT), not the mixture of their K N samples; theta_j of every online copy;
+//   phase 3  qr_core once per online copy j against Tbar, with wi = w / (M B): loss_j and g_j;
+//   phase 4  loss = (sum_j loss_j in j order) / M; dz rows jB + i get k_qr_dueling's phase 4 of g_j.
+// At M = K = 1 every output is k_qr_dueling's, bitwise.
+template <int R, bool VT>
+__global__ void __launch_bounds__(QR_T)
+k_qr_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
+                 const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                 const float* __restrict__ weights, float kappa, float gamma_n, int B, int A, int N, int M, int K,
+                 float* __restrict__ loss, float* __restrict__ dz, float* __restrict__ theta_out,
+                 int64_t* __restrict__ astar_out, float eps) {
+  extern __shared__ __align__(16) float s_dyn[];
+  __shared__ int s_best[RB_MAX_AUG_COPIES];
+  const int N2 = N + A * N;
+  const int rows = M + 2 * K;
+  float* zs = s_dyn;                 // [M + 2K][N2]: online(s_j), online(s'_k), target(s'_k)
+  float* s_theta = zs + rows * N2;   // [M][N] online quantiles of the taken action, per copy
+  float* s_T = s_theta + M * N;      // [N] averaged target quantiles Tbar
+  float* s_g = s_T + N;              // [M][N] gradient rows
+  float* s_l = s_g + M * N;          // [N] qr_core's loss sums
+  float* s_mean = s_l + N;           // [K][A] mean quantile of every action of online(s'_k)
+  float* s_loss = s_mean + K * A;    // [M] loss_j
+  const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  {  // phase 0: k_c51_dueling_avg's staging
+    const int total = rows * N2;
+    for (int base = tid; base < total; base += QR_T * 8) {
+      float v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int idx = base + u * QR_T;
+        v[u] = 0.0f;
+        if (idx < total) {
+          const int t = idx / N2;
+          const float* src = (t < M + K) ? z_on + ((size_t)t * B + i) * N2 : z_tg + ((size_t)(t - M - K) * B + i) * N2;
+          v[u] = __ldg(src + (idx - t * N2));
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int idx = base + u * QR_T;
+        if (idx < total) zs[idx] = v[u];
+      }
+    }
+  }
+  __syncthreads();
+  const int act = (int)actions[i];
+  for (int t = warp; t < K * A; t += QR_WARPS) {  // phase 1
+    const int k = t / A, a = t - k * A;
+    const float* r1 = zs + (size_t)(M + k) * N2;
+    float x[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int c = lane + 32 * r;
+      float acc = 0.0f;
+      if (c < N)
+        for (int aa = 0; aa < A; ++aa) acc += r1[N + aa * N + c];
+      const float mean = acc / (float)A;
+      x[r] = (c < N) ? r1[c] + r1[N + a * N + c] - mean : 0.0f;
+      if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
+    }
+    const float q = qr_row_mean<R>(x, N);
+    if (lane == 0) s_mean[t] = q;
+  }
+  __syncthreads();
+  if (tid < K) {  // phase 2
+    const int best = qr_argmax(s_mean + tid * A, A);
+    s_best[tid] = best;
+    if (astar_out) astar_out[(size_t)tid * B + i] = best;
+  }
+  __syncthreads();
+  const float ret = __ldg(returns + i), scale = __fmul_rn(__ldg(nonterminals + i), gamma_n);
+  for (int c = tid; c < N; c += QR_T) {
+    float acc = 0.0f;
+    for (int k = 0; k < K; ++k) {
+      const float* r2 = zs + (size_t)(M + K + k) * N2;
+      const int best = s_best[k];
+      float m2 = 0.0f;
+      for (int a = 0; a < A; ++a) m2 += r2[N + a * N + c];
+      float T;
+      if constexpr (VT) {
+        const float x = vt_hinv(r2[c] + r2[N + best * N + c] - m2 / (float)A, eps);
+        T = vt_h(__fadd_rn(ret, __fmul_rn(scale, x)), eps);
+      } else {
+        T = __fadd_rn(ret, __fmul_rn(scale, r2[c] + r2[N + best * N + c] - m2 / (float)A));
+      }
+      acc = (k == 0) ? T : __fadd_rn(acc, T);
+    }
+    const float Tbar = __fdiv_rn(acc, (float)K);
+    s_T[c] = Tbar;
+    if (theta_out) theta_out[(size_t)i * N + c] = Tbar;
+    for (int j = 0; j < M; ++j) {
+      const float* r0 = zs + (size_t)j * N2;
+      float m0 = 0.0f;
+      for (int a = 0; a < A; ++a) m0 += r0[N + a * N + c];
+      s_theta[j * N + c] = r0[c] + r0[N + act * N + c] - m0 / (float)A;
+    }
+  }
+  __syncthreads();
+  const float wi = __fdiv_rn(__ldg(weights + i), (float)(M * B));
+  for (int j = 0; j < M; ++j) {  // phase 3
+    qr_core<R>(s_theta + j * N, s_T, s_l, s_g + j * N, N, kappa, wi, j, s_loss);
+    __syncthreads();   // warp 0 has read s_l and written s_loss[j]
+  }
+  if (tid == 0) {  // phase 4
+    float acc = s_loss[0];
+    for (int j = 1; j < M; ++j) acc = __fadd_rn(acc, s_loss[j]);
+    loss[i] = __fdiv_rn(acc, (float)M);
+  }
+  const float inv_a = 1.0f / (float)A;
+  for (int j = 0; j < M; ++j) {
+    float* dzi = dz + ((size_t)j * B + i) * N2;
+    const float* gj = s_g + j * N;
+    for (int idx = tid; idx < N2; idx += QR_T) {
+      if (idx < N) {
+        dzi[idx] = gj[idx];
+      } else {
+        const int a = (idx - N) / N, c = (idx - N) - a * N;
+        dzi[idx] = gj[c] * ((a == act ? 1.0f : 0.0f) - inv_a);
       }
     }
   }
@@ -3238,6 +3370,65 @@ int rb_qr_dueling_vt_loss_grad(const float* z_online, const float* z_target, int
   if (rc != RB_OK) return rc;
   return qr_dueling_launch<true>("rb_qr_dueling_vt_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
                                  nonterminals, weights, kappa, gamma_n, B, loss, dz, theta_out, astar_out, eps, stream);
+}
+
+extern "C++" {
+template <bool VT>
+static int qr_dueling_avg_launch(const char* name, const float* z_online, const float* z_target, int actions_n, int atoms,
+                                 const int64_t* actions, const float* returns, const float* nonterminals,
+                                 const float* weights, float kappa, float gamma_n, int B, int M, int K, float* loss,
+                                 float* dz, float* theta_out, int64_t* astar_out, float eps, rb_stream_t stream) {
+  char msg[128];
+  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !loss || !dz) {
+    snprintf(msg, sizeof msg, "%s: null pointer", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  const int N = atoms, A = actions_n;
+  int rc = qr_check(name, B, A, N, kappa);
+  if (rc != RB_OK) return rc;
+  if (M < 1 || M > RB_MAX_AUG_COPIES || K < 1 || K > RB_MAX_AUG_COPIES) {
+    snprintf(msg, sizeof msg, "%s: copies outside [1, RB_MAX_AUG_COPIES]", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  const size_t smem = (size_t)((M + 2 * K) * (N + A * N) + (2 * M + 2) * N + K * A + M) * sizeof(float);
+  if (smem > 200 * 1024) {
+    snprintf(msg, sizeof msg, "%s: (M + 2K) * actions * atoms too large", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  rc = rbi::ensure_dynamic_smem(k_qr_dueling_avg<2, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling_avg<4, VT>, smem, name);
+  if (rc != RB_OK) return rc;
+  { ProfScope prof_(RB_K_C51_DUELING_AVG, (cudaStream_t)stream);
+    if (N <= 64)
+      k_qr_dueling_avg<2, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                      weights, kappa, gamma_n, B, A, N, M, K, loss, dz,
+                                                                      theta_out, astar_out, eps);
+    else
+      k_qr_dueling_avg<4, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
+                                                                      weights, kappa, gamma_n, B, A, N, M, K, loss, dz,
+                                                                      theta_out, astar_out, eps); }
+  return check_launch(name);
+}
+}
+
+int rb_qr_dueling_avg_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                                float kappa, float gamma_n, int B, int M, int K, float* loss, float* dz, float* theta_out,
+                                int64_t* astar_out, rb_stream_t stream) {
+  return qr_dueling_avg_launch<false>("rb_qr_dueling_avg_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
+                                      nonterminals, weights, kappa, gamma_n, B, M, K, loss, dz, theta_out, astar_out, 0.0f,
+                                      stream);
+}
+
+int rb_qr_dueling_avg_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                   const int64_t* actions, const float* returns, const float* nonterminals,
+                                   const float* weights, float kappa, float gamma_n, int B, int M, int K, float* loss,
+                                   float* dz, float* theta_out, int64_t* astar_out, float eps, rb_stream_t stream) {
+  int rc = vt_check("rb_qr_dueling_avg_vt_loss_grad", true, eps);
+  if (rc != RB_OK) return rc;
+  return qr_dueling_avg_launch<true>("rb_qr_dueling_avg_vt_loss_grad", z_online, z_target, actions_n, atoms, actions,
+                                     returns, nonterminals, weights, kappa, gamma_n, B, M, K, loss, dz, theta_out, astar_out,
+                                     eps, stream);
 }
 
 extern "C++" {
