@@ -55,23 +55,32 @@ from .memory import ReplayMemory, _SampleWorkspace
 from .model import DQN, FusedHead, NoisyLinear
 
 
+def _loss_grad(entries, args, loss, grad, outs, vt):
+    """The body the loss wrappers share: launch entries[0], or under value rescaling (vt: its trailing arguments, None
+    when off) entries[1], on `args`, the outputs loss and grad, the optional outputs `outs` and the stream; returns
+    (loss, grad)."""
+    lib = _lib.load()
+    fn = getattr(lib, entries[0] if vt is None else entries[1])
+    _lib.check(fn(*args, _lib.ptr(loss), _lib.ptr(grad), *map(_lib.ptr, outs), *(vt or ()), _lib.stream()))
+    return loss, grad
+
+
+def _empty(*shape, like):
+    return torch.empty(shape, dtype=torch.float32, device=like.device)
+
+
 def c51_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax,
                   delta_z, gamma_n, loss=None, grad=None, m_out=None, astar_out=None, support_q=None, eps=None):
     """Launch K3 on pre-softmax logits [B,A,Z]; returns (loss[B], grad[B,A,Z]).  eps given: value rescaling
     (rb_c51_vt_loss_grad) with support_q = fl32(h^-1(support))."""
     B, A, Z = q_online_s.shape
-    dev = q_online_s.device
-    if loss is None:
-        loss = torch.empty(B, dtype=torch.float32, device=dev)
-    if grad is None:
-        grad = torch.empty((B, A, Z), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    fn, vt = (lib.rb_c51_loss_grad, ()) if eps is None else (lib.rb_c51_vt_loss_grad, (_lib.ptr(support_q), float(eps)))
-    _lib.check(fn(
-        _lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
-        _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
-        float(gamma_n), B, A, Z, _lib.ptr(loss), _lib.ptr(grad), _lib.ptr(m_out), _lib.ptr(astar_out), *vt, _lib.stream()))
-    return loss, grad
+    return _loss_grad(
+        ("rb_c51_loss_grad", "rb_c51_vt_loss_grad"),
+        (_lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
+         float(gamma_n), B, A, Z),
+        _empty(B, like=q_online_s) if loss is None else loss, _empty(B, A, Z, like=q_online_s) if grad is None else grad,
+        (m_out, astar_out), None if eps is None else (_lib.ptr(support_q), float(eps)))
 
 
 def c51_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin, vmax,
@@ -80,16 +89,13 @@ def c51_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns
     z_target [B, Z(1+A)]; returns (loss[B], dz[B, Z(1+A)]) with dz = d mean(w*loss) / d (z_value | z_advantage).
     eps given: value rescaling (rb_c51_dueling_vt_loss_grad) with support_q = fl32(h^-1(support))."""
     B = actions.shape[0]
-    loss = torch.empty(B, dtype=torch.float32, device=actions.device)
-    dz = torch.empty((B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
-    lib = _lib.load()
-    fn, vt = ((lib.rb_c51_dueling_loss_grad, ()) if eps is None else
-              (lib.rb_c51_dueling_vt_loss_grad, (_lib.ptr(support_q), float(eps))))
-    _lib.check(fn(
-        _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
-        _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
-        float(gamma_n), B, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), *vt, _lib.stream()))
-    return loss, dz
+    return _loss_grad(
+        ("rb_c51_dueling_loss_grad", "rb_c51_dueling_vt_loss_grad"),
+        (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
+         float(gamma_n), B),
+        _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (m_out, astar_out),
+        None if eps is None else (_lib.ptr(support_q), float(eps)))
 
 
 def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin,
@@ -99,16 +105,13 @@ def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, ret
     copies against the target averaged over the K target copies, and its gradient for every online copy of s.  eps
     given: value rescaling (rb_c51_dueling_avg_vt_loss_grad)."""
     B = actions.shape[0]
-    loss = torch.empty(B, dtype=torch.float32, device=actions.device)
-    dz = torch.empty((M * B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
-    lib = _lib.load()
-    fn, vt = ((lib.rb_c51_dueling_avg_loss_grad, ()) if eps is None else
-              (lib.rb_c51_dueling_avg_vt_loss_grad, (_lib.ptr(support_q), float(eps))))
-    _lib.check(fn(
-        _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
-        _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
-        float(gamma_n), B, M, K, _lib.ptr(loss), _lib.ptr(dz), _lib.ptr(m_out), _lib.ptr(astar_out), *vt, _lib.stream()))
-    return loss, dz
+    return _loss_grad(
+        ("rb_c51_dueling_avg_loss_grad", "rb_c51_dueling_avg_vt_loss_grad"),
+        (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
+         float(gamma_n), B, M, K),
+        _empty(B, like=actions), _empty(M * B, atoms * (1 + actions_n), like=actions), (m_out, astar_out),
+        None if eps is None else (_lib.ptr(support_q), float(eps)))
 
 
 def qr_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, kappa, gamma_n,
@@ -116,15 +119,12 @@ def qr_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterm
     """The quantile loss (rb_qr_loss_grad) on quantile rows [B,A,N]; returns (loss[B], grad[B,A,N]).  eps given: value
     rescaling (rb_qr_vt_loss_grad)."""
     B, A, N = q_online_s.shape
-    loss = torch.empty(B, dtype=torch.float32, device=q_online_s.device)
-    grad = torch.empty((B, A, N), dtype=torch.float32, device=q_online_s.device)
-    lib = _lib.load()
-    fn, vt = (lib.rb_qr_loss_grad, ()) if eps is None else (lib.rb_qr_vt_loss_grad, (float(eps),))
-    _lib.check(fn(
-        _lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
-        _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, A, N, _lib.ptr(loss), _lib.ptr(grad),
-        _lib.ptr(theta_out), _lib.ptr(astar_out), *vt, _lib.stream()))
-    return loss, grad
+    return _loss_grad(
+        ("rb_qr_loss_grad", "rb_qr_vt_loss_grad"),
+        (_lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, A, N),
+        _empty(B, like=q_online_s), _empty(B, A, N, like=q_online_s), (theta_out, astar_out),
+        None if eps is None else (float(eps),))
 
 
 def qr_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, kappa, gamma_n,
@@ -132,15 +132,12 @@ def qr_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns,
     """The quantile loss fed straight by the fused heads (rb_qr_dueling_loss_grad), rows as c51_dueling_loss_grad takes
     them; returns (loss[B], dz[B, N(1+A)]).  eps given: value rescaling (rb_qr_dueling_vt_loss_grad)."""
     B = actions.shape[0]
-    loss = torch.empty(B, dtype=torch.float32, device=actions.device)
-    dz = torch.empty((B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
-    lib = _lib.load()
-    fn, vt = (lib.rb_qr_dueling_loss_grad, ()) if eps is None else (lib.rb_qr_dueling_vt_loss_grad, (float(eps),))
-    _lib.check(fn(
-        _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
-        _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, _lib.ptr(loss), _lib.ptr(dz),
-        _lib.ptr(theta_out), _lib.ptr(astar_out), *vt, _lib.stream()))
-    return loss, dz
+    return _loss_grad(
+        ("rb_qr_dueling_loss_grad", "rb_qr_dueling_vt_loss_grad"),
+        (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B),
+        _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (theta_out, astar_out),
+        None if eps is None else (float(eps),))
 
 
 def qr_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, kappa, gamma_n,
@@ -150,16 +147,12 @@ def qr_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, retu
     of the K target copies' quantiles, and its gradient for every online copy of s.  eps given: value rescaling
     (rb_qr_dueling_avg_vt_loss_grad)."""
     B = actions.shape[0]
-    loss = torch.empty(B, dtype=torch.float32, device=actions.device)
-    dz = torch.empty((M * B, atoms * (1 + actions_n)), dtype=torch.float32, device=actions.device)
-    lib = _lib.load()
-    fn, vt = ((lib.rb_qr_dueling_avg_loss_grad, ()) if eps is None else
-              (lib.rb_qr_dueling_avg_vt_loss_grad, (float(eps),)))
-    _lib.check(fn(
-        _lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
-        _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, M, K, _lib.ptr(loss), _lib.ptr(dz),
-        _lib.ptr(theta_out), _lib.ptr(astar_out), *vt, _lib.stream()))
-    return loss, dz
+    return _loss_grad(
+        ("rb_qr_dueling_avg_loss_grad", "rb_qr_dueling_avg_vt_loss_grad"),
+        (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, M, K),
+        _empty(B, like=actions), _empty(M * B, atoms * (1 + actions_n), like=actions), (theta_out, astar_out),
+        None if eps is None else (float(eps),))
 
 
 DISTRIBUTIONS = ("categorical", "quantile")

@@ -1223,6 +1223,89 @@ k_c51(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const
   }
 }
 
+// ---- stages the dueling kernels share: a z row is (z_value [Z] | z_advantage [A][Z]), N2 = Z + A Z floats ----
+
+// Mean advantage at atom c of z row zr (model.py:75): summed over the actions in order from 0, divided once by A.  This
+// and dueling_q define the dueling combination for the quantile, select and statistics kernels, which agree bitwise with
+// the loss kernels because of it.  k_c51_dueling and k_c51_dueling_avg spell the same arithmetic out inline: through these
+// helpers ptxas gives them more registers, and a spill at R = 4.  LDG: the row is in global memory, read through the
+// read-only cache (else shared).
+template <bool LDG = false>
+__device__ __forceinline__ float dueling_mean(const float* zr, int A, int Z, int c) {
+  float acc = 0.0f;
+  for (int a = 0; a < A; ++a) acc += LDG ? __ldg(zr + Z + a * Z + c) : zr[Z + a * Z + c];
+  return acc / (float)A;
+}
+
+// q_a[c] = v[c] + adv_a[c] - mean[c], from values the caller loaded (sites that reuse v and the mean across actions)
+__device__ __forceinline__ float dueling_q(float v, float adv, float mean) { return v + adv - mean; }
+
+// q_a[c] of z row zr, the mean formed for this one atom and action
+template <bool LDG = false>
+__device__ __forceinline__ float dueling_q(const float* zr, int A, int Z, int c, int a) {
+  const float mean = dueling_mean<LDG>(zr, A, Z, c);
+  return dueling_q(LDG ? __ldg(zr + c) : zr[c], LDG ? __ldg(zr + Z + a * Z + c) : zr[Z + a * Z + c], mean);
+}
+
+// Stage sample i's M + 2K z rows into zs [M + 2K][N2] with all T threads: online(s_j) from z_on row jB + i, online(s'_k)
+// from z_on row (M + k)B + i, target(s'_k) from z_tg row kB + i.  Eight independent loads in flight per thread, then the
+// stores: the fused loss kernels are pure dependent latency, so every load is issued before any is waited on.
+template <int T>
+__device__ __forceinline__ void stage_z_rows(float* zs, const float* __restrict__ z_on, const float* __restrict__ z_tg,
+                                             int i, int B, int N2, int M, int K) {
+  const int total = (M + 2 * K) * N2;
+  const size_t BN2 = (size_t)B * N2;
+  z_on += (size_t)i * N2;
+  z_tg += (size_t)i * N2;
+  for (int base = threadIdx.x; base < total; base += T * 8) {
+    float v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int idx = base + u * T;
+      v[u] = 0.0f;
+      if (idx < total) {
+        const int t = idx / N2;
+        const float* src = t < M + K ? z_on + (size_t)t * BN2 : z_tg + (size_t)(t - M - K) * BN2;
+        v[u] = __ldg(src + (idx - t * N2));
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int idx = base + u * T;
+      if (idx < total) zs[idx] = v[u];
+    }
+  }
+}
+
+// dz row of one sample from the gradient row g [Z] of its taken action, with all T threads: the dueling combination's
+// backward, dzv[c] = g[c] and dza[a][c] = g[c] ([a == act] - 1/A).
+template <int T>
+__device__ __forceinline__ void dueling_dz(float* __restrict__ dzi, const float* g, int A, int Z, int act) {
+  const float inv_a = 1.0f / (float)A;
+  for (int idx = threadIdx.x; idx < Z + A * Z; idx += T) {
+    if (idx < Z) {
+      dzi[idx] = g[idx];
+    } else {
+      const int a = (idx - Z) / Z, c = (idx - Z) - a * Z;
+      dzi[idx] = g[c] * ((a == act ? 1.0f : 0.0f) - inv_a);
+    }
+  }
+}
+
+// arg-max of s[0, n): the first maximum wins, like torch.argmax
+__device__ __forceinline__ int first_argmax(const float* s, int n) {
+  int best = 0;
+  float best_v = -CUDART_INF_F;
+  for (int a = 0; a < n; ++a) {
+    const float v = s[a];
+    if (v > best_v) {
+      best_v = v;
+      best = a;
+    }
+  }
+  return best;
+}
+
 // Dueling entry point: fed by the fused heads' outputs z = (z_value | z_advantage) [rows][Z + A*Z]
 // (online net: 2B rows, s then s'; target net: B rows).  ONE CTA PER SAMPLE, 8 warps: the kernel is pure dependent latency
 // (184 KB in, 46 KB out), so the serial chain per sample is cut instead of packing samples into few CTAs:
@@ -1559,35 +1642,19 @@ k_q_select(const float* __restrict__ z, int M, int A, int Z, const float* __rest
     if (c < Z) {
       sup[r] = __ldg(support + c);
       zv[r] = __ldg(zr + c);
-      float acc = 0.0f;
-      for (int a = 0; a < A; ++a) acc += __ldg(zr + Z + a * Z + c);
-      mean[r] = acc / (float)A;
+      mean[r] = dueling_mean<true>(zr, A, Z, c);
     }
   }
   int best = 0;
   float best_ev = -CUDART_INF_F;
   for (int a = 0; a < A; ++a) {
-    float x[R], mx = -CUDART_INF_F;
+    float x[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       const int c = lane + 32 * r;
-      x[r] = (c < Z) ? zv[r] + __ldg(zr + Z + a * Z + c) - mean[r] : -CUDART_INF_F;
-      mx = fmaxf(mx, x[r]);
+      x[r] = (c < Z) ? dueling_q(zv[r], __ldg(zr + Z + a * Z + c), mean[r]) : -CUDART_INF_F;
     }
-    mx = warp_max(mx);
-    float se = 0.0f, sn = 0.0f;
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-      const float ee = (lane + 32 * r < Z) ? expf(x[r] - mx) : 0.0f;
-      se = __fadd_rn(se, ee);
-      sn = __fadd_rn(sn, __fmul_rn(sup[r], ee));
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      se = __fadd_rn(se, __shfl_xor_sync(0xffffffffu, se, o));
-      sn = __fadd_rn(sn, __shfl_xor_sync(0xffffffffu, sn, o));
-    }
-    const float ev = __fdiv_rn(sn, se);
+    const float ev = c51_expected_value<R>(x, sup, Z, lane);
     if (q_out && lane == 0) q_out[(size_t)m * A + a] = ev;
     if (ev > best_ev) {   // first maximum wins, like torch.argmax / max
       best_ev = ev;
@@ -1627,17 +1694,11 @@ __device__ __forceinline__ float qr_row_mean(const float (&x)[R], int N) {
   return __fdiv_rn(warp_sum(s), (float)N);
 }
 
-__device__ __forceinline__ int qr_argmax(const float* s_mean, int A) {
-  int best = 0;
-  float best_q = -CUDART_INF_F;
-  for (int a = 0; a < A; ++a) {
-    const float q = s_mean[a];
-    if (q > best_q) {  // first maximum wins, like torch.argmax
-      best_q = q;
-      best = a;
-    }
-  }
-  return best;
+// Target quantile T = r + scale q with scale = fl32(nt gamma_n); VT: h(r + scale h^-1(q)), q in h units
+template <bool VT>
+__device__ __forceinline__ float qr_target(float ret, float scale, float q, float eps) {
+  if constexpr (VT) return vt_h(__fadd_rn(ret, __fmul_rn(scale, vt_hinv(q, eps))), eps);
+  return __fadd_rn(ret, __fmul_rn(scale, q));
 }
 
 // Phases 3 and 4 (without the gradient write) from the rows s_theta, s_T [N] in shared memory: s_g [N] receives the
@@ -1706,27 +1767,7 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
   float* s_l = s_g + N;           // [N] loss sum of every online quantile
   float* s_mean = s_l + N;        // [A] mean quantile of every action of online(s')
   const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  {  // phase 0: k_c51_dueling's staging
-    const int total = 3 * N2;
-    const float* src[3] = {z_on + (size_t)i * N2, z_on + (size_t)(B + i) * N2, z_tg + (size_t)i * N2};
-    for (int base = tid; base < total; base += QR_T * 8) {
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int idx = base + u * QR_T;
-        v[u] = 0.0f;
-        if (idx < total) {
-          const int t = idx / N2;
-          v[u] = __ldg(src[t] + (idx - t * N2));
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int idx = base + u * QR_T;
-        if (idx < total) zs[idx] = v[u];
-      }
-    }
-  }
+  stage_z_rows<QR_T>(zs, z_on, z_tg, i, B, N2, 1, 1);  // phase 0
   __syncthreads();
   const int act = (int)actions[i];
   {  // phase 1
@@ -1735,17 +1776,14 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       const int c = lane + 32 * r;
-      float acc = 0.0f;
-      if (c < N)
-        for (int a = 0; a < A; ++a) acc += r1[N + a * N + c];
-      mean[r] = acc / (float)A;
+      mean[r] = (c < N) ? dueling_mean(r1, A, N, c) : 0.0f;
     }
     for (int a = warp; a < A; a += QR_WARPS) {
       float x[R];
 #pragma unroll
       for (int r = 0; r < R; ++r) {
         const int c = lane + 32 * r;
-        x[r] = (c < N) ? r1[c] + r1[N + a * N + c] - mean[r] : 0.0f;
+        x[r] = (c < N) ? dueling_q(r1[c], r1[N + a * N + c], mean[r]) : 0.0f;
         if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
       }
       const float q = qr_row_mean<R>(x, N);
@@ -1753,42 +1791,18 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
     }
   }
   __syncthreads();
-  const int best = qr_argmax(s_mean, A);  // phase 2
+  const int best = first_argmax(s_mean, A);  // phase 2
   if (astar_out && tid == 0) astar_out[i] = best;
   const float ret = __ldg(returns + i), scale = __fmul_rn(__ldg(nonterminals + i), gamma_n);
   for (int c = tid; c < N; c += QR_T) {
-    const float* r0 = zs;
-    const float* r2 = zs + 2 * N2;
-    float m0 = 0.0f, m2 = 0.0f;
-    for (int a = 0; a < A; ++a) {
-      m0 += r0[N + a * N + c];
-      m2 += r2[N + a * N + c];
-    }
-    s_theta[c] = r0[c] + r0[N + act * N + c] - m0 / (float)A;
-    float T;
-    if constexpr (VT) {
-      const float x = vt_hinv(r2[c] + r2[N + best * N + c] - m2 / (float)A, eps);
-      T = vt_h(__fadd_rn(ret, __fmul_rn(scale, x)), eps);
-    } else {
-      T = __fadd_rn(ret, __fmul_rn(scale, r2[c] + r2[N + best * N + c] - m2 / (float)A));
-    }
+    s_theta[c] = dueling_q(zs, A, N, c, act);
+    const float T = qr_target<VT>(ret, scale, dueling_q(zs + 2 * N2, A, N, c, best), eps);
     s_T[c] = T;
     if (theta_out) theta_out[(size_t)i * N + c] = T;
   }
   __syncthreads();
   qr_core<R>(s_theta, s_T, s_l, s_g, N, kappa, __fdiv_rn(__ldg(weights + i), (float)B), i, loss);
-  {  // phase 4: dzv[c] = g[c], dza[a][c] = g[c] ([a == act] - 1/A), as k_c51_dueling
-    float* dzi = dz + (size_t)i * N2;
-    const float inv_a = 1.0f / (float)A;
-    for (int idx = tid; idx < N2; idx += QR_T) {
-      if (idx < N) {
-        dzi[idx] = s_g[idx];
-      } else {
-        const int a = (idx - N) / N, c = (idx - N) - a * N;
-        dzi[idx] = s_g[c] * ((a == act ? 1.0f : 0.0f) - inv_a);
-      }
-    }
-  }
+  dueling_dz<QR_T>(dz + (size_t)i * N2, s_g, A, N, act);  // phase 4
 }
 
 // DrQ's K / M averaging under the quantile loss: z rows as k_c51_dueling_avg takes them (z_on (M + K) B rows, copy j of s
@@ -1796,11 +1810,11 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
 // the sample's M + 2K z rows staged in shared memory:
 //   phase 1  the mean quantile of every (target copy k, action a) of online(s'_k), one warp per pair (k_qr_dueling's
 //            phase 1 per pair, bitwise);
-//   phase 2  thread k: a*_k (first maximum wins); then per quantile n, T_k,n as k_qr_dueling forms it and
+//   phase 2  thread k: a*_k (first maximum wins); then per quantile n, T_k,n (qr_target) and
 //            Tbar_n = (sum_k T_k,n in k order) / K, rounded once -- the quantile-wise average of the K target quantile
 //            functions (in h units under VT), not the mixture of their K N samples; theta_j of every online copy;
 //   phase 3  qr_core once per online copy j against Tbar, with wi = w / (M B): loss_j and g_j;
-//   phase 4  loss = (sum_j loss_j in j order) / M; dz rows jB + i get k_qr_dueling's phase 4 of g_j.
+//   phase 4  loss = (sum_j loss_j in j order) / M; dz rows jB + i from g_j (dueling_dz).
 // At M = K = 1 every output is k_qr_dueling's, bitwise.
 template <int R, bool VT>
 __global__ void __launch_bounds__(QR_T)
@@ -1821,27 +1835,7 @@ k_qr_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg,
   float* s_mean = s_l + N;           // [K][A] mean quantile of every action of online(s'_k)
   float* s_loss = s_mean + K * A;    // [M] loss_j
   const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  {  // phase 0: k_c51_dueling_avg's staging
-    const int total = rows * N2;
-    for (int base = tid; base < total; base += QR_T * 8) {
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int idx = base + u * QR_T;
-        v[u] = 0.0f;
-        if (idx < total) {
-          const int t = idx / N2;
-          const float* src = (t < M + K) ? z_on + ((size_t)t * B + i) * N2 : z_tg + ((size_t)(t - M - K) * B + i) * N2;
-          v[u] = __ldg(src + (idx - t * N2));
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int idx = base + u * QR_T;
-        if (idx < total) zs[idx] = v[u];
-      }
-    }
-  }
+  stage_z_rows<QR_T>(zs, z_on, z_tg, i, B, N2, M, K);  // phase 0
   __syncthreads();
   const int act = (int)actions[i];
   for (int t = warp; t < K * A; t += QR_WARPS) {  // phase 1
@@ -1851,11 +1845,7 @@ k_qr_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg,
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       const int c = lane + 32 * r;
-      float acc = 0.0f;
-      if (c < N)
-        for (int aa = 0; aa < A; ++aa) acc += r1[N + aa * N + c];
-      const float mean = acc / (float)A;
-      x[r] = (c < N) ? r1[c] + r1[N + a * N + c] - mean : 0.0f;
+      x[r] = (c < N) ? dueling_q(r1, A, N, c, a) : 0.0f;
       if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
     }
     const float q = qr_row_mean<R>(x, N);
@@ -1863,7 +1853,7 @@ k_qr_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg,
   }
   __syncthreads();
   if (tid < K) {  // phase 2
-    const int best = qr_argmax(s_mean + tid * A, A);
+    const int best = first_argmax(s_mean + tid * A, A);
     s_best[tid] = best;
     if (astar_out) astar_out[(size_t)tid * B + i] = best;
   }
@@ -1872,28 +1862,13 @@ k_qr_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg,
   for (int c = tid; c < N; c += QR_T) {
     float acc = 0.0f;
     for (int k = 0; k < K; ++k) {
-      const float* r2 = zs + (size_t)(M + K + k) * N2;
-      const int best = s_best[k];
-      float m2 = 0.0f;
-      for (int a = 0; a < A; ++a) m2 += r2[N + a * N + c];
-      float T;
-      if constexpr (VT) {
-        const float x = vt_hinv(r2[c] + r2[N + best * N + c] - m2 / (float)A, eps);
-        T = vt_h(__fadd_rn(ret, __fmul_rn(scale, x)), eps);
-      } else {
-        T = __fadd_rn(ret, __fmul_rn(scale, r2[c] + r2[N + best * N + c] - m2 / (float)A));
-      }
+      const float T = qr_target<VT>(ret, scale, dueling_q(zs + (size_t)(M + K + k) * N2, A, N, c, s_best[k]), eps);
       acc = (k == 0) ? T : __fadd_rn(acc, T);
     }
     const float Tbar = __fdiv_rn(acc, (float)K);
     s_T[c] = Tbar;
     if (theta_out) theta_out[(size_t)i * N + c] = Tbar;
-    for (int j = 0; j < M; ++j) {
-      const float* r0 = zs + (size_t)j * N2;
-      float m0 = 0.0f;
-      for (int a = 0; a < A; ++a) m0 += r0[N + a * N + c];
-      s_theta[j * N + c] = r0[c] + r0[N + act * N + c] - m0 / (float)A;
-    }
+    for (int j = 0; j < M; ++j) s_theta[j * N + c] = dueling_q(zs + (size_t)j * N2, A, N, c, act);
   }
   __syncthreads();
   const float wi = __fdiv_rn(__ldg(weights + i), (float)(M * B));
@@ -1906,19 +1881,7 @@ k_qr_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg,
     for (int j = 1; j < M; ++j) acc = __fadd_rn(acc, s_loss[j]);
     loss[i] = __fdiv_rn(acc, (float)M);
   }
-  const float inv_a = 1.0f / (float)A;
-  for (int j = 0; j < M; ++j) {
-    float* dzi = dz + ((size_t)j * B + i) * N2;
-    const float* gj = s_g + j * N;
-    for (int idx = tid; idx < N2; idx += QR_T) {
-      if (idx < N) {
-        dzi[idx] = gj[idx];
-      } else {
-        const int a = (idx - N) / N, c = (idx - N) - a * N;
-        dzi[idx] = gj[c] * ((a == act ? 1.0f : 0.0f) - inv_a);
-      }
-    }
-  }
+  for (int j = 0; j < M; ++j) dueling_dz<QR_T>(dz + ((size_t)j * B + i) * N2, s_g + j * N, A, N, act);
 }
 
 // Plain entry point: quantile rows [B][A][N] of online(s), online(s') and target(s'); grad [B][A][N] is the gradient row
@@ -1950,16 +1913,12 @@ k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const 
   }
   __syncthreads();
   const int act = (int)actions[i];
-  const int best = qr_argmax(s_mean, A);  // phase 2
+  const int best = first_argmax(s_mean, A);  // phase 2
   if (astar_out && tid == 0) astar_out[i] = best;
   const float ret = __ldg(returns + i), scale = __fmul_rn(__ldg(nonterminals + i), gamma_n);
   for (int c = tid; c < N; c += QR_T) {
     s_theta[c] = __ldg(q_on_s + (row0 + act) * N + c);
-    float T;
-    if constexpr (VT)
-      T = vt_h(__fadd_rn(ret, __fmul_rn(scale, vt_hinv(__ldg(q_tg_ns + (row0 + best) * N + c), eps))), eps);
-    else
-      T = __fadd_rn(ret, __fmul_rn(scale, __ldg(q_tg_ns + (row0 + best) * N + c)));
+    const float T = qr_target<VT>(ret, scale, __ldg(q_tg_ns + (row0 + best) * N + c), eps);
     s_T[c] = T;
     if (theta_out) theta_out[(size_t)i * N + c] = T;
   }
@@ -1991,9 +1950,7 @@ k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict_
     zv[r] = mean[r] = 0.0f;
     if (c < N) {
       zv[r] = __ldg(zr + c);
-      float acc = 0.0f;
-      for (int a = 0; a < A; ++a) acc += __ldg(zr + N + a * N + c);
-      mean[r] = acc / (float)A;
+      mean[r] = dueling_mean<true>(zr, A, N, c);
     }
   }
   int best = 0;
@@ -2003,7 +1960,7 @@ k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict_
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       const int c = lane + 32 * r;
-      x[r] = (c < N) ? zv[r] + __ldg(zr + N + a * N + c) - mean[r] : 0.0f;
+      x[r] = (c < N) ? dueling_q(zv[r], __ldg(zr + N + a * N + c), mean[r]) : 0.0f;
       if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
     }
     const float q = qr_row_mean<R>(x, N);
@@ -2147,17 +2104,13 @@ k_learn_stats_batch(const float* __restrict__ loss, const float* __restrict__ we
       if (lane + 32 * r < Z) tv = __fadd_rn(tv, __fmul_rn(__ldg(mr + lane + 32 * r), sup[r]));
     const float edge = __fadd_rn(__ldg(mr), __ldg(mr + Z - 1));
     float x[R];
-    if (z) {   // dueling combination of the taken action, as k_c51_dueling forms it
+    if (z) {
       const float* zr = z + (size_t)i * (Z + A * Z);
 #pragma unroll
       for (int r = 0; r < R; ++r) {
         const int c = lane + 32 * r;
         x[r] = -CUDART_INF_F;
-        if (c < Z) {
-          float mean = 0.0f;
-          for (int a = 0; a < A; ++a) mean += __ldg(zr + Z + a * Z + c);
-          x[r] = __ldg(zr + c) + __ldg(zr + Z + act * Z + c) - mean / (float)A;
-        }
+        if (c < Z) x[r] = dueling_q<true>(zr, A, Z, c, act);
       }
     } else {
       const float* qr = q + ((size_t)i * A + act) * Z;
@@ -2178,7 +2131,7 @@ k_learn_stats_batch(const float* __restrict__ loss, const float* __restrict__ we
 }
 
 // k_learn_stats_batch for the quantile loss: theta = the T rows [B][N] of the loss kernel (theta_out); per sample
-// q(s, a) = mean_i theta_i of the online quantiles of the taken action (dueling combination as k_qr_dueling forms it) and
+// q(s, a) = mean_i theta_i of the online quantiles of the taken action (dueling_q from z, or the row of q) and
 // the target value mean_j T_j; edge_mass is NaN (there is no support to clamp to).  VT: both means are of h^-1 of the
 // quantiles (return units).
 template <bool VT>
@@ -2203,14 +2156,7 @@ k_learn_stats_batch_qr(const float* __restrict__ loss, const float* __restrict__
       t[r] = (c < N) ? __ldg(tr + c) : 0.0f;
       x[r] = 0.0f;
       if (c < N) {
-        if (z) {
-          const float* zr = z + (size_t)i * (N + A * N);
-          float mean = 0.0f;
-          for (int a = 0; a < A; ++a) mean += __ldg(zr + N + a * N + c);
-          x[r] = __ldg(zr + c) + __ldg(zr + N + act * N + c) - mean / (float)A;
-        } else {
-          x[r] = __ldg(q + ((size_t)i * A + act) * N + c);
-        }
+        x[r] = z ? dueling_q<true>(z + (size_t)i * (N + A * N), A, N, c, act) : __ldg(q + ((size_t)i * A + act) * N + c);
         if constexpr (VT) {
           t[r] = vt_hinv(t[r], eps);
           x[r] = vt_hinv(x[r], eps);
@@ -3042,6 +2988,48 @@ static int vt_check(const char* name, bool support_q_ok, float eps) {
   return RB_OK;
 }
 
+static int null_pointer(const char* name) {
+  char msg[128];
+  snprintf(msg, sizeof msg, "%s: null pointer", name);
+  return fail(RB_ERR_INVAL, msg);
+}
+
+// The C51 launchers' shared refusals; a_name / z_name: what the entry calls A and Z in its messages.
+static int c51_check(const char* name, bool pointers_ok, int B, int A, int Z, const char* a_name, const char* z_name) {
+  if (!pointers_ok) return null_pointer(name);
+  char msg[128];
+  if (B <= 0 || A <= 0 || Z <= 1) {
+    snprintf(msg, sizeof msg, "%s: B, %s > 0 and %s > 1 are required", name, a_name, z_name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (Z > RB_MAX_ATOMS) {
+    snprintf(msg, sizeof msg, "%s: %s exceeds RB_MAX_ATOMS", name, z_name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  return RB_OK;
+}
+
+// The averaging launchers' copies range and the fused loss launchers' shared-memory limit.  Those launchers grant the
+// dynamic shared memory to both R instantiations: ensure_dynamic_smem skips requests of at most 48 KB without counting the
+// kernel's static shared memory, so a launch can depend on a grant a larger request of the other R already made.
+static int copies_check(const char* name, int M, int K) {
+  if (M < 1 || M > RB_MAX_AUG_COPIES || K < 1 || K > RB_MAX_AUG_COPIES) {
+    char msg[128];
+    snprintf(msg, sizeof msg, "%s: copies outside [1, RB_MAX_AUG_COPIES]", name);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  return RB_OK;
+}
+
+static int smem_check(const char* name, size_t smem, const char* what) {
+  if (smem > 200 * 1024) {
+    char msg[128];
+    snprintf(msg, sizeof msg, "%s: %s", name, what);
+    return fail(RB_ERR_RANGE, msg);
+  }
+  return RB_OK;
+}
+
 extern "C++" {   // the shared launchers are templates, which cannot have C linkage
 template <bool VT>
 static int c51_launch(const char* name, const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
@@ -3049,32 +3037,16 @@ static int c51_launch(const char* name, const float* q_online_s, const float* q_
                       const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z,
                       float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, const float* support_q, float eps,
                       rb_stream_t stream) {
-  char msg[128];
-  if (!q_online_s || !q_online_ns || !q_target_ns || !actions || !returns || !nonterminals || !weights || !support ||
-      !loss || !grad_q_online_s) {
-    snprintf(msg, sizeof msg, "%s: null pointer", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
-  if (B <= 0 || A <= 0 || Z <= 1) {
-    snprintf(msg, sizeof msg, "%s: B, A > 0 and Z > 1 are required", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
-  if (Z > RB_MAX_ATOMS) {
-    snprintf(msg, sizeof msg, "%s: Z exceeds RB_MAX_ATOMS", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
-  const int ctas = (B + C51_WARPS - 1) / C51_WARPS;
+  int rc = VT ? vt_check(name, support_q != nullptr, eps) : RB_OK;
+  if (rc == RB_OK)
+    rc = c51_check(name, q_online_s && q_online_ns && q_target_ns && actions && returns && nonterminals && weights &&
+                   support && loss && grad_q_online_s, B, A, Z, "A", "Z");
+  if (rc != RB_OK) return rc;
+  const auto k = Z <= 64 ? k_c51<2, VT> : k_c51<4, VT>;
   { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
-    if (Z <= 64)
-      k_c51<2, VT><<<ctas, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
-                                                                   nonterminals, weights, support, vmin, vmax, delta_z,
-                                                                   gamma_n, B, A, Z, loss, grad_q_online_s, m_out,
-                                                                   astar_out, support_q, eps);
-    else
-      k_c51<4, VT><<<ctas, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
-                                                                   nonterminals, weights, support, vmin, vmax, delta_z,
-                                                                   gamma_n, B, A, Z, loss, grad_q_online_s, m_out,
-                                                                   astar_out, support_q, eps); }
+    k<<<(B + C51_WARPS - 1) / C51_WARPS, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n,
+        B, A, Z, loss, grad_q_online_s, m_out, astar_out, support_q, eps); }
   return check_launch(name);
 }
 }
@@ -3093,8 +3065,6 @@ int rb_c51_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const
                         float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z, float* loss,
                         float* grad_q_online_s, float* m_out, int64_t* astar_out, const float* support_q, float eps,
                         rb_stream_t stream) {
-  int rc = vt_check("rb_c51_vt_loss_grad", support_q != nullptr, eps);
-  if (rc != RB_OK) return rc;
   return c51_launch<true>("rb_c51_vt_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals,
                           weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss, grad_q_online_s, m_out, astar_out,
                           support_q, eps, stream);
@@ -3168,37 +3138,21 @@ static int c51_dueling_launch(const char* name, const float* z_online, const flo
                               const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss,
                               float* dz, float* m_out, int64_t* astar_out, const float* support_q, float eps,
                               rb_stream_t stream) {
-  char msg[128];
-  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !support || !loss || !dz) {
-    snprintf(msg, sizeof msg, "%s: null pointer", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
   const int Z = atoms, A = actions_n;
-  if (B <= 0 || A <= 0 || Z <= 1) {
-    snprintf(msg, sizeof msg, "%s: B, actions > 0 and atoms > 1 are required", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
-  if (Z > RB_MAX_ATOMS) {
-    snprintf(msg, sizeof msg, "%s: atoms exceeds RB_MAX_ATOMS", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
+  int rc = VT ? vt_check(name, support_q != nullptr, eps) : RB_OK;
+  if (rc == RB_OK)
+    rc = c51_check(name, z_online && z_target && actions && returns && nonterminals && weights && support && loss && dz, B,
+                   A, Z, "actions", "atoms");
+  if (rc != RB_OK) return rc;
   const size_t smem = (size_t)(3 * (Z + A * Z) + 3 * Z + A) * sizeof(float);
-  if (smem > 200 * 1024) {
-    snprintf(msg, sizeof msg, "%s: actions * atoms too large", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
-  int rc_s = rbi::ensure_dynamic_smem(k_c51_dueling<2, VT>, smem, name);
-  if (rc_s == RB_OK) rc_s = rbi::ensure_dynamic_smem(k_c51_dueling<4, VT>, smem, name);
-  if (rc_s != RB_OK) return rc_s;
+  rc = smem_check(name, smem, "actions * atoms too large");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling<2, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling<4, VT>, smem, name);
+  if (rc != RB_OK) return rc;
+  const auto k = Z <= 64 ? k_c51_dueling<2, VT> : k_c51_dueling<4, VT>;
   { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
-    if (Z <= 64)
-      k_c51_dueling<2, VT><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                      weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z,
-                                                                      loss, dz, m_out, astar_out, support_q, eps);
-    else
-      k_c51_dueling<4, VT><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                      weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z,
-                                                                      loss, dz, m_out, astar_out, support_q, eps); }
+    k<<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, support, vmin,
+                                                 vmax, delta_z, gamma_n, B, A, Z, loss, dz, m_out, astar_out, support_q, eps); }
   return check_launch(name);
 }
 }
@@ -3216,8 +3170,6 @@ int rb_c51_dueling_vt_loss_grad(const float* z_online, const float* z_target, in
                                 const float* returns, const float* nonterminals, const float* weights, const float* support,
                                 float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss, float* dz,
                                 float* m_out, int64_t* astar_out, const float* support_q, float eps, rb_stream_t stream) {
-  int rc = vt_check("rb_c51_dueling_vt_loss_grad", support_q != nullptr, eps);
-  if (rc != RB_OK) return rc;
   return c51_dueling_launch<true>("rb_c51_dueling_vt_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
                                   nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, loss, dz, m_out, astar_out,
                                   support_q, eps, stream);
@@ -3230,43 +3182,23 @@ static int c51_dueling_avg_launch(const char* name, const float* z_online, const
                                   const float* weights, const float* support, float vmin, float vmax, float delta_z,
                                   float gamma_n, int B, int M, int K, float* loss, float* dz, float* m_out, int64_t* astar_out,
                                   const float* support_q, float eps, rb_stream_t stream) {
-  char msg[128];
-  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !support || !loss || !dz) {
-    snprintf(msg, sizeof msg, "%s: null pointer", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
   const int Z = atoms, A = actions_n;
-  if (B <= 0 || A <= 0 || Z <= 1) {
-    snprintf(msg, sizeof msg, "%s: B, actions > 0 and atoms > 1 are required", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
-  if (Z > RB_MAX_ATOMS) {
-    snprintf(msg, sizeof msg, "%s: atoms exceeds RB_MAX_ATOMS", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
-  if (M < 1 || M > RB_MAX_AUG_COPIES || K < 1 || K > RB_MAX_AUG_COPIES) {
-    snprintf(msg, sizeof msg, "%s: copies outside [1, RB_MAX_AUG_COPIES]", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
+  int rc = VT ? vt_check(name, support_q != nullptr, eps) : RB_OK;
+  if (rc == RB_OK)
+    rc = c51_check(name, z_online && z_target && actions && returns && nonterminals && weights && support && loss && dz, B,
+                   A, Z, "actions", "atoms");
+  if (rc == RB_OK) rc = copies_check(name, M, K);
+  if (rc != RB_OK) return rc;
   const size_t smem = (size_t)((M + 2 * K) * (Z + A * Z) + (2 * M + 2 * K + 1) * Z + K * A + M) * sizeof(float);
-  if (smem > 200 * 1024) {
-    snprintf(msg, sizeof msg, "%s: (M + 2K) * actions * atoms too large", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
-  int rc_s = rbi::ensure_dynamic_smem(k_c51_dueling_avg<2, VT>, smem, name);
-  if (rc_s == RB_OK) rc_s = rbi::ensure_dynamic_smem(k_c51_dueling_avg<4, VT>, smem, name);
-  if (rc_s != RB_OK) return rc_s;
+  rc = smem_check(name, smem, "(M + 2K) * actions * atoms too large");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling_avg<2, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling_avg<4, VT>, smem, name);
+  if (rc != RB_OK) return rc;
+  const auto k = Z <= 64 ? k_c51_dueling_avg<2, VT> : k_c51_dueling_avg<4, VT>;
   { ProfScope prof_(RB_K_C51_DUELING_AVG, (cudaStream_t)stream);
-    if (Z <= 64)
-      k_c51_dueling_avg<2, VT><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                          weights, support, vmin, vmax, delta_z, gamma_n, B,
-                                                                          A, Z, M, K, loss, dz, m_out, astar_out, support_q,
-                                                                          eps);
-    else
-      k_c51_dueling_avg<4, VT><<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                          weights, support, vmin, vmax, delta_z, gamma_n, B,
-                                                                          A, Z, M, K, loss, dz, m_out, astar_out, support_q,
-                                                                          eps); }
+    k<<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, support, vmin,
+                                                 vmax, delta_z, gamma_n, B, A, Z, M, K, loss, dz, m_out, astar_out, support_q,
+                                                 eps); }
   return check_launch(name);
 }
 }
@@ -3285,8 +3217,6 @@ int rb_c51_dueling_avg_vt_loss_grad(const float* z_online, const float* z_target
                                     const float* weights, const float* support, float vmin, float vmax, float delta_z,
                                     float gamma_n, int B, int M, int K, float* loss, float* dz, float* m_out,
                                     int64_t* astar_out, const float* support_q, float eps, rb_stream_t stream) {
-  int rc = vt_check("rb_c51_dueling_avg_vt_loss_grad", support_q != nullptr, eps);
-  if (rc != RB_OK) return rc;
   return c51_dueling_avg_launch<true>("rb_c51_dueling_avg_vt_loss_grad", z_online, z_target, actions_n, atoms, actions,
                                       returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, M, K, loss,
                                       dz, m_out, astar_out, support_q, eps, stream);
@@ -3326,31 +3256,21 @@ static int qr_dueling_launch(const char* name, const float* z_online, const floa
                              const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
                              float kappa, float gamma_n, int B, float* loss, float* dz, float* theta_out, int64_t* astar_out,
                              float eps, rb_stream_t stream) {
-  char msg[128];
-  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !loss || !dz) {
-    snprintf(msg, sizeof msg, "%s: null pointer", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
   const int N = atoms, A = actions_n;
-  int rc = qr_check(name, B, A, N, kappa);
+  int rc = VT ? vt_check(name, true, eps) : RB_OK;
+  if (rc == RB_OK && !(z_online && z_target && actions && returns && nonterminals && weights && loss && dz))
+    rc = null_pointer(name);
+  if (rc == RB_OK) rc = qr_check(name, B, A, N, kappa);
   if (rc != RB_OK) return rc;
   const size_t smem = (size_t)(3 * (N + A * N) + 4 * N + A) * sizeof(float);
-  if (smem > 200 * 1024) {
-    snprintf(msg, sizeof msg, "%s: actions * atoms too large", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
-  rc = rbi::ensure_dynamic_smem(k_qr_dueling<2, VT>, smem, name);
+  rc = smem_check(name, smem, "actions * atoms too large");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<2, VT>, smem, name);
   if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<4, VT>, smem, name);
   if (rc != RB_OK) return rc;
+  const auto k = N <= 64 ? k_qr_dueling<2, VT> : k_qr_dueling<4, VT>;
   { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
-    if (N <= 64)
-      k_qr_dueling<2, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                  weights, kappa, gamma_n, B, A, N, loss, dz, theta_out,
-                                                                  astar_out, eps);
-    else
-      k_qr_dueling<4, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                  weights, kappa, gamma_n, B, A, N, loss, dz, theta_out,
-                                                                  astar_out, eps); }
+    k<<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, kappa, gamma_n, B,
+                                               A, N, loss, dz, theta_out, astar_out, eps); }
   return check_launch(name);
 }
 }
@@ -3366,8 +3286,6 @@ int rb_qr_dueling_vt_loss_grad(const float* z_online, const float* z_target, int
                                const float* returns, const float* nonterminals, const float* weights, float kappa,
                                float gamma_n, int B, float* loss, float* dz, float* theta_out, int64_t* astar_out, float eps,
                                rb_stream_t stream) {
-  int rc = vt_check("rb_qr_dueling_vt_loss_grad", true, eps);
-  if (rc != RB_OK) return rc;
   return qr_dueling_launch<true>("rb_qr_dueling_vt_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
                                  nonterminals, weights, kappa, gamma_n, B, loss, dz, theta_out, astar_out, eps, stream);
 }
@@ -3378,35 +3296,22 @@ static int qr_dueling_avg_launch(const char* name, const float* z_online, const 
                                  const int64_t* actions, const float* returns, const float* nonterminals,
                                  const float* weights, float kappa, float gamma_n, int B, int M, int K, float* loss,
                                  float* dz, float* theta_out, int64_t* astar_out, float eps, rb_stream_t stream) {
-  char msg[128];
-  if (!z_online || !z_target || !actions || !returns || !nonterminals || !weights || !loss || !dz) {
-    snprintf(msg, sizeof msg, "%s: null pointer", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
   const int N = atoms, A = actions_n;
-  int rc = qr_check(name, B, A, N, kappa);
+  int rc = VT ? vt_check(name, true, eps) : RB_OK;
+  if (rc == RB_OK && !(z_online && z_target && actions && returns && nonterminals && weights && loss && dz))
+    rc = null_pointer(name);
+  if (rc == RB_OK) rc = qr_check(name, B, A, N, kappa);
+  if (rc == RB_OK) rc = copies_check(name, M, K);
   if (rc != RB_OK) return rc;
-  if (M < 1 || M > RB_MAX_AUG_COPIES || K < 1 || K > RB_MAX_AUG_COPIES) {
-    snprintf(msg, sizeof msg, "%s: copies outside [1, RB_MAX_AUG_COPIES]", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
   const size_t smem = (size_t)((M + 2 * K) * (N + A * N) + (2 * M + 2) * N + K * A + M) * sizeof(float);
-  if (smem > 200 * 1024) {
-    snprintf(msg, sizeof msg, "%s: (M + 2K) * actions * atoms too large", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
-  rc = rbi::ensure_dynamic_smem(k_qr_dueling_avg<2, VT>, smem, name);
+  rc = smem_check(name, smem, "(M + 2K) * actions * atoms too large");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling_avg<2, VT>, smem, name);
   if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling_avg<4, VT>, smem, name);
   if (rc != RB_OK) return rc;
+  const auto k = N <= 64 ? k_qr_dueling_avg<2, VT> : k_qr_dueling_avg<4, VT>;
   { ProfScope prof_(RB_K_C51_DUELING_AVG, (cudaStream_t)stream);
-    if (N <= 64)
-      k_qr_dueling_avg<2, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                      weights, kappa, gamma_n, B, A, N, M, K, loss, dz,
-                                                                      theta_out, astar_out, eps);
-    else
-      k_qr_dueling_avg<4, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals,
-                                                                      weights, kappa, gamma_n, B, A, N, M, K, loss, dz,
-                                                                      theta_out, astar_out, eps); }
+    k<<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, kappa, gamma_n, B,
+                                               A, N, M, K, loss, dz, theta_out, astar_out, eps); }
   return check_launch(name);
 }
 }
@@ -3424,8 +3329,6 @@ int rb_qr_dueling_avg_vt_loss_grad(const float* z_online, const float* z_target,
                                    const int64_t* actions, const float* returns, const float* nonterminals,
                                    const float* weights, float kappa, float gamma_n, int B, int M, int K, float* loss,
                                    float* dz, float* theta_out, int64_t* astar_out, float eps, rb_stream_t stream) {
-  int rc = vt_check("rb_qr_dueling_avg_vt_loss_grad", true, eps);
-  if (rc != RB_OK) return rc;
   return qr_dueling_avg_launch<true>("rb_qr_dueling_avg_vt_loss_grad", z_online, z_target, actions_n, atoms, actions,
                                      returns, nonterminals, weights, kappa, gamma_n, B, M, K, loss, dz, theta_out, astar_out,
                                      eps, stream);
@@ -3437,31 +3340,21 @@ static int qr_launch(const char* name, const float* q_online_s, const float* q_o
                      const int64_t* actions, const float* returns, const float* nonterminals, const float* weights, float kappa,
                      float gamma_n, int B, int A, int N, float* loss, float* grad_q_online_s, float* theta_out,
                      int64_t* astar_out, float eps, rb_stream_t stream) {
-  char msg[128];
-  if (!q_online_s || !q_online_ns || !q_target_ns || !actions || !returns || !nonterminals || !weights || !loss ||
-      !grad_q_online_s) {
-    snprintf(msg, sizeof msg, "%s: null pointer", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
-  int rc = qr_check(name, B, A, N, kappa);
+  int rc = VT ? vt_check(name, true, eps) : RB_OK;
+  if (rc == RB_OK && !(q_online_s && q_online_ns && q_target_ns && actions && returns && nonterminals && weights && loss &&
+                       grad_q_online_s))
+    rc = null_pointer(name);
+  if (rc == RB_OK) rc = qr_check(name, B, A, N, kappa);
   if (rc != RB_OK) return rc;
   const size_t smem = (size_t)(4 * N + A) * sizeof(float);
-  if (smem > 200 * 1024) {
-    snprintf(msg, sizeof msg, "%s: too many actions", name);
-    return fail(RB_ERR_RANGE, msg);
-  }
-  rc = rbi::ensure_dynamic_smem(k_qr<2, VT>, smem, name);
+  rc = smem_check(name, smem, "too many actions");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<2, VT>, smem, name);
   if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<4, VT>, smem, name);
   if (rc != RB_OK) return rc;
+  const auto k = N <= 64 ? k_qr<2, VT> : k_qr<4, VT>;
   { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
-    if (N <= 64)
-      k_qr<2, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
-                                                          nonterminals, weights, kappa, gamma_n, B, A, N, loss,
-                                                          grad_q_online_s, theta_out, astar_out, eps);
-    else
-      k_qr<4, VT><<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns,
-                                                          nonterminals, weights, kappa, gamma_n, B, A, N, loss,
-                                                          grad_q_online_s, theta_out, astar_out, eps); }
+    k<<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights,
+                                               kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, eps); }
   return check_launch(name);
 }
 }
@@ -3478,8 +3371,6 @@ int rb_qr_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const 
                        const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
                        int B, int A, int N, float* loss, float* grad_q_online_s, float* theta_out, int64_t* astar_out,
                        float eps, rb_stream_t stream) {
-  int rc = vt_check("rb_qr_vt_loss_grad", true, eps);
-  if (rc != RB_OK) return rc;
   return qr_launch<true>("rb_qr_vt_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights,
                          kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, eps, stream);
 }
@@ -3488,11 +3379,10 @@ extern "C++" {
 template <bool VT>
 static int qr_q_values_launch(const char* name, const float* z, int M, int actions, int atoms, float* q,
                               int64_t* best_action, float* best_q, float eps, rb_stream_t stream) {
+  int rc = VT ? vt_check(name, true, eps) : RB_OK;
+  if (rc != RB_OK) return rc;
+  if (!z) return null_pointer(name);
   char msg[128];
-  if (!z) {
-    snprintf(msg, sizeof msg, "%s: null pointer", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
   if (!q && !best_action && !best_q) {
     snprintf(msg, sizeof msg, "%s: no output requested", name);
     return fail(RB_ERR_INVAL, msg);
@@ -3518,8 +3408,6 @@ int rb_qr_q_values(const float* z, int M, int actions, int atoms, float* q, int6
 
 int rb_qr_vt_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
                       float eps, rb_stream_t stream) {
-  int rc = vt_check("rb_qr_vt_q_values", true, eps);
-  if (rc != RB_OK) return rc;
   return qr_q_values_launch<true>("rb_qr_vt_q_values", z, M, actions, atoms, q, best_action, best_q, eps, stream);
 }
 
@@ -3558,11 +3446,10 @@ template <bool VT>
 static int stats_batch_qr_launch(const char* name, const float* loss, const float* weights, const int64_t* actions,
                                  const float* theta, const float* z, const float* q, int B, int A, int N, double* scratch,
                                  float eps, rb_stream_t stream) {
+  int rc = VT ? vt_check(name, true, eps) : RB_OK;
+  if (rc != RB_OK) return rc;
+  if (!loss || !weights || !actions || !theta || !scratch) return null_pointer(name);
   char msg[128];
-  if (!loss || !weights || !actions || !theta || !scratch) {
-    snprintf(msg, sizeof msg, "%s: null pointer", name);
-    return fail(RB_ERR_INVAL, msg);
-  }
   if ((z == nullptr) == (q == nullptr)) {
     snprintf(msg, sizeof msg, "%s: give exactly one of z and q", name);
     return fail(RB_ERR_INVAL, msg);
@@ -3593,8 +3480,6 @@ int rb_learn_stats_batch_qr(const float* loss, const float* weights, const int64
 int rb_learn_stats_batch_qr_vt(const float* loss, const float* weights, const int64_t* actions, const float* theta,
                                const float* z, const float* q, int B, int A, int N, double* scratch, float eps,
                                rb_stream_t stream) {
-  int rc = vt_check("rb_learn_stats_batch_qr_vt", true, eps);
-  if (rc != RB_OK) return rc;
   return stats_batch_qr_launch<true>("rb_learn_stats_batch_qr_vt", loss, weights, actions, theta, z, q, B, A, N, scratch, eps,
                                      stream);
 }
