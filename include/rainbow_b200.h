@@ -468,6 +468,35 @@ int rb_qr_dueling_avg_vt_loss_grad(const float* z_online, const float* z_target,
                                    const float* weights, float kappa, float gamma_n, int B, int M, int K, float* loss,
                                    float* dz, float* theta_out, int64_t* astar_out, float eps, rb_stream_t stream);
 
+/* Munchausen targets for the quantile loss (M-RL, Vieillard, Pietquin & Geist 2020; DESIGN.md §17): the target net's
+ * softmax policy replaces the double-DQN arg-max, and a clipped log-policy bonus joins the return.  With
+ * q(x, a) = (1/N) sum_j q_target(x, a)_j (the dueling combination, then the mean over quantiles) and, per row q[A],
+ *   m = max_a q_a,  S = sum_a exp((q_a - m) / temperature) (in action order),  pi_a = exp((q_a - m) / temperature) / S,
+ *   l_a = (q_a - m) - temperature log S   (temperature ln pi_a, <= 0),
+ * sample i with taken action a has
+ *   b   = alpha max(l_a(s), clip)                                                (target row of s),
+ *   c_j = sum_a' pi_a'(s') (q_target(s', a')_j - l_a'(s'))  (in action order),
+ *   T_j = fl32(r + b) + fl32(fl32(nonterminal * gamma_n) c_j),
+ * and theta, the loss (also the priority) and the gradient are rb_qr_dueling_loss_grad's against T.  There is no arg-max.
+ * expf / logf run at full precision.
+ * rb_qr_dueling_munchausen_loss_grad: z_online has B rows (s only; the online s' rows feed nothing), z_target 2B rows,
+ * s at row i then s' at row B + i; writes loss[B] and dz[B][atoms*(1+actions)].  rb_qr_munchausen_loss_grad: plain
+ * quantile rows [B][A][N] of online(s), target(s) and target(s'); writes grad[B][A][N] (g at the taken action, 0
+ * elsewhere).  Optional outputs: theta_out [B][N] receives T (rb_learn_stats_batch_qr takes it unchanged), bonus_out [B]
+ * receives b.  RB_ERR_INVAL: rb_qr_dueling_loss_grad's, plus alpha outside [0, 1], temperature not finite or below
+ * FLT_MIN, clip not finite or >= 0 (NaN refused); RB_ERR_RANGE: atoms > RB_MAX_ATOMS or rows too large for shared memory.
+ * A refused call writes nothing.  Sums run in a fixed order (eager launches and graph replays agree bitwise).  Profiled
+ * under RB_K_C51_DUELING / RB_K_C51. */
+int rb_qr_dueling_munchausen_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                       const int64_t* actions, const float* returns, const float* nonterminals,
+                                       const float* weights, float kappa, float gamma_n, float alpha, float temperature,
+                                       float clip, int B, float* loss, float* dz, float* theta_out, float* bonus_out,
+                                       rb_stream_t stream);
+int rb_qr_munchausen_loss_grad(const float* q_online_s, const float* q_target_s, const float* q_target_ns,
+                               const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                               float kappa, float gamma_n, float alpha, float temperature, float clip, int B, int A, int N,
+                               float* loss, float* grad_q_online_s, float* theta_out, float* bonus_out, rb_stream_t stream);
+
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */
 int rb_noisy_compose(const float* mu, const float* sigma, const float* eps, int64_t count, float* out,

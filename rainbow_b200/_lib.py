@@ -157,6 +157,11 @@ SIGNATURES = {
                                               _vp, _vp, _vp, _vp]),
     "rb_qr_dueling_avg_vt_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _i32, _i32,
                                                  _vp, _vp, _vp, _vp, _f32, _vp]),
+    # Munchausen targets under the quantile loss: alpha, temperature, clip after gamma_n; bonus_out in astar_out's place
+    "rb_qr_dueling_munchausen_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32,
+                                                     _f32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "rb_qr_munchausen_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32, _i32, _i32,
+                                             _i32, _vp, _vp, _vp, _vp, _vp]),
 }
 
 # rb_learn_stats_record of include/rainbow_b200.h (48 bytes): field name -> numpy dtype, in memory order

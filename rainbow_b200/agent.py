@@ -14,13 +14,16 @@ One `learn(mem)` (agent.py:61-100) is:
     3 x conv body (torch: cuDNN)              (agent.py:66,71,75 -> model.py:70-71)
     K6 rb_noisy_resample (target net)         (agent.py:74)
     fused noisy dueling heads (rb_head_forward) on the conv features -- online net on [s; s'], target on s'
+                                              [args.munchausen: online net on s, target on [s; s']]
     K3 rb_c51_dueling_loss_grad               (agent.py:67,72-73,76-96 + softmax halves of model.py:76-79 + model.py:75)
                                               [M or K > 1: rb_c51_dueling_avg_loss_grad -- DrQ's target averaged over
                                                the K copies of s', loss over the M copies of s;
                                                args.distribution = "quantile": rb_qr_dueling_loss_grad -- QR-DQN's
                                                quantile Huber loss, no support or projection; with M or K > 1
                                                (args.quantile_average_copies) rb_qr_dueling_avg_loss_grad -- the target
-                                               quantiles averaged over the K copies, the loss over the M copies]
+                                               quantiles averaged over the K copies, the loss over the M copies;
+                                               args.munchausen: rb_qr_dueling_munchausen_loss_grad -- the target net's
+                                               softmax policy in place of the arg-max, and a clipped log-policy bonus]
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
@@ -155,6 +158,32 @@ def qr_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, retu
         None if eps is None else (float(eps),))
 
 
+def qr_munchausen_loss_grad(q_online_s, q_target_s, q_target_ns, actions, returns, nonterminals, weights, kappa, gamma_n,
+                            alpha, temperature, clip, theta_out=None, bonus_out=None):
+    """The quantile loss against Munchausen targets (rb_qr_munchausen_loss_grad) on quantile rows [B,A,N] of online(s),
+    target(s) and target(s'); returns (loss[B], grad[B,A,N])."""
+    B, A, N = q_online_s.shape
+    return _loss_grad(
+        ("rb_qr_munchausen_loss_grad",),
+        (_lib.ptr(q_online_s), _lib.ptr(q_target_s), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), float(alpha), float(temperature),
+         float(clip), B, A, N),
+        _empty(B, like=q_online_s), _empty(B, A, N, like=q_online_s), (theta_out, bonus_out), None)
+
+
+def qr_dueling_munchausen_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, kappa,
+                                    gamma_n, alpha, temperature, clip, theta_out=None, bonus_out=None):
+    """The quantile loss against Munchausen targets fed straight by the fused heads (rb_qr_dueling_munchausen_loss_grad):
+    z_online [B, N(1+A)] (s only), z_target [2B, N(1+A)] (s rows, then s'); returns (loss[B], dz[B, N(1+A)])."""
+    B = actions.shape[0]
+    return _loss_grad(
+        ("rb_qr_dueling_munchausen_loss_grad",),
+        (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), float(alpha), float(temperature),
+         float(clip), B),
+        _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (theta_out, bonus_out), None)
+
+
 DISTRIBUTIONS = ("categorical", "quantile")
 
 
@@ -220,6 +249,47 @@ def value_transform_options(args):
         raise ValueError(f"value_transform_eps must be 0 or in [{np.finfo(np.float32).tiny:g}, 1] (a normal fp32), "
                          f"got {eps}")
     return vt, float(np.float32(eps))   # the fp32 the kernels take: the host's float64 h^-1 uses the same eps
+
+
+def munchausen_options(args):
+    """(alpha, temperature, clip) of Munchausen targets (Vieillard et al. 2020, DESIGN.md §17) from `args`, or None when
+    args.munchausen is absent, None or False.  args.munchausen must be a bool.  When it is True:
+    munchausen_alpha (absent or None: 0.9) in [0, 1] (0: the soft target without the bonus), munchausen_temperature (0.03)
+    finite and > 0 as a normal fp32, munchausen_clip (l0, -1) finite and < 0; each returned rounded to the fp32 the
+    kernels take.  Refused with it: distribution "categorical", value_transform "rescale" and augment_m / augment_k other
+    than (1, 1)."""
+    on = getattr(args, "munchausen", None)
+    if on is None:
+        return None
+    if not isinstance(on, (bool, np.bool_)):
+        raise ValueError(f"munchausen must be a bool, got {on!r}")
+    if not on:
+        return None
+    dist = getattr(args, "distribution", None)
+    if dist != "quantile":
+        raise ValueError(f"munchausen needs distribution 'quantile', got {dist!r}: the categorical projection of the "
+                         f"policy-weighted mixture of shifted distributions is not implemented")
+    if getattr(args, "value_transform", None) not in (None, "none"):
+        raise ValueError("munchausen does not compose with value_transform 'rescale'")
+    copies = (getattr(args, "augment_m", 1), getattr(args, "augment_k", 1))
+    if copies != (1, 1):
+        raise ValueError(f"munchausen needs augment_m = augment_k = 1, got {copies}")
+    tiny = float(np.finfo(np.float32).tiny)
+    out = []
+    for key, default, ok, want in (("munchausen_alpha", 0.9, lambda v: 0.0 <= v <= 1.0, "in [0, 1]"),
+                                   ("munchausen_temperature", 0.03, lambda v: tiny <= v < math.inf,
+                                    "finite and > 0 as a normal fp32"),
+                                   ("munchausen_clip", -1.0, lambda v: -math.inf < v < 0.0, "finite and < 0")):
+        v = getattr(args, key, None)
+        v = default if v is None else v
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.floating, np.integer)):
+            raise ValueError(f"{key} must be a number, got {v!r}")
+        with np.errstate(over="ignore"):
+            v32 = float(np.float32(v))
+        if not (ok(float(v)) and ok(v32)):
+            raise ValueError(f"{key} must be {want}, got {v}")
+        out.append(v32)
+    return tuple(out)
 
 
 def vt_hinv(y, eps):
@@ -520,6 +590,9 @@ class Agent:
         self.device = torch.device(args.device)
         if self.device.type != "cuda":
             raise _lib.RainbowB200Error(f"rainbow_b200.Agent needs a CUDA device, got '{self.device}' (no CPU fallback)")
+        # Munchausen targets under the quantile loss (off by default): (alpha, temperature, clip) or None; the online net
+        # then runs on s only and the target net on [s; s']
+        self.munchausen = munchausen_options(args)
         # value rescaling (off by default): the network learns in h units, V_min / V_max included; acting, evaluation and
         # the statistics report return units
         self.value_transform, self.value_transform_eps = value_transform_options(args)
@@ -809,8 +882,18 @@ class Agent:
         agent's augment_m / augment_k copies (1 / 1: [s; s'] and s)."""
         on = self.online_net
         M, K = self.augment_copies
+        if self.munchausen is not None:   # online on s, target on [s; s']
+            return (self.use_fused_head and on.training and on.fused_ok(B, backward_batch=B) and
+                    self.target_net.fused_ok(2 * B))
         return (self.use_fused_head and on.training and on.fused_ok((M + K) * B, backward_batch=M * B) and
                 self.target_net.fused_ok(K * B))
+
+    def _target_rows(self, states, next_states):
+        """The target net's input: s' alone, or under Munchausen [s; s'] (the adjacent blocks' view, else a copy)."""
+        if self.munchausen is None:
+            return next_states
+        both = self._adjacent(states, next_states)
+        return both if both is not None else torch.cat([states, next_states])
 
     @staticmethod
     def _adjacent(states, next_states):
@@ -843,7 +926,9 @@ class Agent:
         two state blocks out back to back, else with online(s') on a second side stream.
         DrQ's K / M: `states` may hold M copies of the B sampled states and `next_states` K copies of the next states
         (copy-major); the online pass then runs over all (M + K) B rows, the target pass over K B rows, and the backward
-        over the M B rows of s."""
+        over the M B rows of s.
+        Munchausen: the online s' rows feed nothing, so the online pass runs on s alone (B rows) and the target pass, with
+        one noise draw, on [s; s'] (2B rows): 3B conv rows in all, as without it."""
         states, next_states = batch[1], batch[4]
         on, tg = self.online_net, self.target_net
         B, Bs, Bn = batch[2].shape[0], states.shape[0], next_states.shape[0]      # Bs = M B rows of s, Bn = K B of s'
@@ -852,16 +937,17 @@ class Agent:
         noise_done = None
         if on._noise_pending:   # the online net's deferred reset_noise(): beside the sampling / conv work, not in front of it
             noise_done = _lib.side_branch(s_ns, on.flush_noise)[1]
+        munch = self.munchausen is not None
 
         def target_pass():
             tg.reset_noise(*(target_noise or ()))                          # agent.py:74
-            return tg.head().forward(tg.features_nograd(next_states))[0]
+            return tg.head().forward(tg.features_nograd(self._target_rows(states, next_states)))[0]
         with torch.no_grad():
             z_t, done_tg = _lib.side_branch(s_tg, target_pass)
         manual = on.manual_conv_ok(states)
         # [s; s'] in ONE conv pass when the sampler laid both state blocks out back to back (ReplayMemory's workspaces do):
         # the online net's weights stream once, and two concurrent conv chains (online, target) share the SMs instead of three
-        both = self._adjacent(states, next_states) if manual else None
+        both = self._adjacent(states, next_states) if manual and not munch else None
         if both is not None:
             with torch.no_grad():
                 acts2 = on.conv_forward_saving(both)
@@ -871,14 +957,18 @@ class Agent:
             head_in = (x_both,)
         else:
             with torch.no_grad():
-                x_ns, done_ns = _lib.side_branch(s_ns, lambda: on.features_nograd(next_states))
+                if not munch:
+                    x_ns, done_ns = _lib.side_branch(s_ns, lambda: on.features_nograd(next_states))
                 if manual:
                     acts = on.conv_forward_saving(states)  # library kernels, backward scheduled by hand below
             x_s = acts[-1].view(Bs, -1) if manual else on.features(states)    # else an autograd graph: convs only
             xs_d = x_s.detach()
-            main.wait_event(done_ns)
-            x_ns.record_stream(main)
-            head_in = (xs_d, x_ns)
+            if munch:
+                head_in = (xs_d,)
+            else:
+                main.wait_event(done_ns)
+                x_ns.record_stream(main)
+                head_in = (xs_d, x_ns)
         with torch.no_grad():
             if noise_done is not None:
                 main.wait_event(noise_done)
@@ -946,9 +1036,12 @@ class Agent:
             self.online_net._eps_stale = True    # the graph composes them from whatever draw precedes a replay
         q_s = self.online_net.logits(states)
         with torch.no_grad():
-            q_ns = self.online_net.logits(next_states)
+            # Munchausen: no online s' rows; the target's rows of s and s' from one noise draw, as q_ns and q_t
+            q_ns = self.online_net.logits(next_states) if self.munchausen is None else None
             self.target_net.reset_noise(*(target_noise or ()))
-            q_t = self.target_net.logits(next_states)
+            q_t = self.target_net.logits(self._target_rows(states, next_states))
+            if self.munchausen is not None:
+                q_ns, q_t = q_t[:B], q_t[B:]
             loss, grad, m = self._library_loss(q_s.detach(), q_ns, q_t, batch)
             stats_done = self._stats_batch(batch, loss, m, q=q_s.detach())
         self.optimiser.zero_grad()
@@ -978,10 +1071,14 @@ class Agent:
     def _fused_loss(self, z_online, z_target, batch, M, K):
         """The loss on the fused heads' rows for M copies of s and K of s': rb_qr_dueling_loss_grad (quantile, M = K = 1)
         or rb_qr_dueling_avg_loss_grad (quantile, M or K > 1: args.quantile_average_copies), rb_c51_dueling_loss_grad, or
-        at M or K > 1 rb_c51_dueling_avg_loss_grad.  Returns (loss[B], dz, stats rows)."""
+        at M or K > 1 rb_c51_dueling_avg_loss_grad; under Munchausen rb_qr_dueling_munchausen_loss_grad (z_online: s rows,
+        z_target: [s; s'] rows).  Returns (loss[B], dz, stats rows)."""
         _, _, actions, returns, _, nonterminals, weights = batch
         m = self._stats_rows(actions.shape[0])
         rows = (z_online, z_target, self.action_space, self.atoms, actions, returns, nonterminals, weights)
+        if self.munchausen is not None:
+            return (*qr_dueling_munchausen_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), *self.munchausen,
+                                                     theta_out=m), m)
         vt = self._vt_args()
         if self.quantile and (M, K) == (1, 1):
             return (*qr_dueling_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"]), m)
@@ -994,11 +1091,14 @@ class Agent:
         return (*c51_dueling_avg_loss_grad(*rows, *c51, M, K, m_out=m, **vt), m)
 
     def _library_loss(self, q_s, q_ns, q_t, batch):
-        """The loss on the library head's logits [B, A, Z]: rb_qr_loss_grad (quantile) or rb_c51_loss_grad.  Returns
-        (loss[B], grad[B, A, Z], stats rows)."""
+        """The loss on the library head's logits [B, A, Z]: rb_qr_loss_grad (quantile) or rb_c51_loss_grad; under
+        Munchausen rb_qr_munchausen_loss_grad, q_ns then being the target's rows of s.  Returns (loss[B], grad[B, A, Z],
+        stats rows)."""
         _, _, actions, returns, _, nonterminals, weights = batch
         m = self._stats_rows(actions.shape[0])
         rows = (q_s, q_ns, q_t, actions, returns, nonterminals, weights)
+        if self.munchausen is not None:
+            return (*qr_munchausen_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), *self.munchausen, theta_out=m), m)
         vt = self._vt_args()
         if self.quantile:
             return (*qr_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"]), m)

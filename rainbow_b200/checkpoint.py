@@ -379,6 +379,8 @@ def _meta(agent, mem):
         hyper["value_transform"], hyper["value_transform_eps"] = agent.value_transform, agent.value_transform_eps
     if agent.quantile_average_copies:   # absent: the quantile loss does not average copies
         hyper["quantile_average_copies"] = True
+    if agent.munchausen is not None:   # absent: no Munchausen targets
+        hyper["munchausen_alpha"], hyper["munchausen_temperature"], hyper["munchausen_clip"] = agent.munchausen
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
         learner["redo_count"] = agent.redo_count
     if opt.grouped:   # the group optimiser's bias-correction counts, [encoder, head]
@@ -528,6 +530,11 @@ def _validate(agent, mem, man):
     qavg = hyper.get("quantile_average_copies", False)
     if qavg is not agent.quantile_average_copies:
         raise _Error(f"quantile_average_copies differs: checkpoint {qavg!r}, live {agent.quantile_average_copies!r}")
+    # and one trained against Munchausen targets, or under other (alpha, temperature, clip)
+    munch = tuple(hyper.get(k) for k in ("munchausen_alpha", "munchausen_temperature", "munchausen_clip"))
+    live = agent.munchausen or (None, None, None)
+    if munch != live:
+        raise _Error(f"munchausen (alpha, temperature, clip) differs: checkpoint {munch}, live {live}")
     layout = agent.optimiser.state_dict(clone=False)["layout"]
     if man.get("optimiser") != layout:
         raise _Error(f"optimiser layout differs: checkpoint {man.get('optimiser')}, this learner {layout}")

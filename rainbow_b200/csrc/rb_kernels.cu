@@ -1931,6 +1931,194 @@ k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const 
   }
 }
 
+// ---- Munchausen targets under the quantile loss (M-RL, Vieillard et al. 2020; DESIGN.md §17) ----
+// q(x, a) = (1/N) sum_j theta_j(x, a) of the TARGET net (qr_row_mean of the dueling combination, k_qr_dueling's phase 1).
+// Per row q[A]: m = max_a q_a, e_a = exp((q_a - m) / tau), S = sum_a e_a in action order, pi_a = e_a / S and
+// l_a = (q_a - m) - tau log S = tau ln pi_a in the stable form (<= 0 exactly: S >= 1).  For sample i, taken action a:
+//   b   = alpha max(l_a(s), l0)                                          (target row of s)
+//   c_j = sum_a' pi_a'(s') (theta_j(s', a') - l_a'(s')) in action order   (target row of s')
+//   T_j = fl32(r + b) + fl32(fl32(nt gamma_n) c_j)
+// then qr_core against T.  expf / logf at full precision; every other step rounded explicitly.
+
+// One row's policy from its A mean quantiles q: pi [A] and l [A] (either may be NULL); returns l_act (act in [0, A)) or 0.
+__device__ __forceinline__ float munchausen_policy(const float* q, int A, float tau, float* pi, float* ell, int act) {
+  float m = q[0];
+  for (int a = 1; a < A; ++a) m = fmaxf(m, q[a]);
+  float S = 0.0f;
+  for (int a = 0; a < A; ++a) S = __fadd_rn(S, expf(__fdiv_rn(__fsub_rn(q[a], m), tau)));
+  const float tlog = __fmul_rn(tau, logf(S));
+  float l_act = 0.0f;
+  for (int a = 0; a < A; ++a) {
+    const float d = __fsub_rn(q[a], m);
+    const float l = __fsub_rn(d, tlog);
+    if (pi) pi[a] = __fdiv_rn(expf(__fdiv_rn(d, tau)), S);
+    if (ell) ell[a] = l;
+    if (a == act) l_act = l;
+  }
+  return l_act;
+}
+
+// The scalar stage both Munchausen kernels share, after phase 1 has left the target mean quantiles in s_q [2][A] (row 0:
+// s, row 1: s'): warp 0 lane 0 forms b from row 0 into *s_b (and bonus_out), warp 1 lane 0 pi and l of row 1 into s_pi,
+// s_ell.  The caller synchronises afterwards.
+__device__ __forceinline__ void munchausen_stage(const float* s_q, float* s_pi, float* s_ell, float* s_b, int A, int act,
+                                                 float alpha, float tau, float l0, int i, float* __restrict__ bonus_out) {
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    const float b = __fmul_rn(alpha, fmaxf(munchausen_policy(s_q, A, tau, nullptr, nullptr, act), l0));
+    *s_b = b;
+    if (bonus_out) bonus_out[i] = b;
+  } else if (tid == 32) {
+    munchausen_policy(s_q + A, A, tau, s_pi, s_ell, -1);
+  }
+}
+
+// c_j of one quantile from the s' quantiles theta_j(s', a') = q(a'), summed over a' in action order
+template <typename Q>
+__device__ __forceinline__ float munchausen_soft_value(const Q& q, const float* s_pi, const float* s_ell, int A) {
+  float acc = 0.0f;
+  for (int a = 0; a < A; ++a) acc = __fadd_rn(acc, __fmul_rn(s_pi[a], __fsub_rn(q(a), s_ell[a])));
+  return acc;
+}
+
+// Stage sample i's three z rows into zs [3][N2] with all T threads: online(s) from z_on row i, target(s) from z_tg row i,
+// target(s') from z_tg row B + i (stage_z_rows' pattern: every load issued before any is waited on).
+template <int T>
+__device__ __forceinline__ void stage_munchausen_rows(float* zs, const float* __restrict__ z_on,
+                                                      const float* __restrict__ z_tg, int i, int B, int N2) {
+  const int total = 3 * N2;
+  for (int base = threadIdx.x; base < total; base += T * 8) {
+    float v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int idx = base + u * T;
+      v[u] = 0.0f;
+      if (idx < total) {
+        const int t = idx / N2;
+        const float* src = t == 0 ? z_on + (size_t)i * N2 : z_tg + (size_t)(t == 1 ? i : B + i) * N2;
+        v[u] = __ldg(src + (idx - t * N2));
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int idx = base + u * T;
+      if (idx < total) zs[idx] = v[u];
+    }
+  }
+}
+
+// Dueling entry point: z_on B rows (s), z_tg 2B rows (s, then s').  One CTA of QR_T threads per sample:
+//   phase 0  stage online(s), target(s), target(s');
+//   phase 1  the 2A target mean quantiles, one warp per (row, action), into s_q;
+//   phase 2  m, S, pi, l of both rows (munchausen_stage), then b and T_j per quantile, theta of the taken action;
+//   phase 3  qr_core; phase 4 dueling_dz.
+template <int R>
+__global__ void __launch_bounds__(QR_T)
+k_qr_dueling_munchausen(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
+                        const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                        const float* __restrict__ weights, float kappa, float gamma_n, float alpha, float tau, float l0,
+                        int B, int A, int N, float* __restrict__ loss, float* __restrict__ dz,
+                        float* __restrict__ theta_out, float* __restrict__ bonus_out) {
+  extern __shared__ __align__(16) float s_dyn[];
+  __shared__ float s_b;
+  const int N2 = N + A * N;
+  float* zs = s_dyn;              // [3][N2]: online(s), target(s), target(s')
+  float* s_theta = zs + 3 * N2;   // [N] online quantiles of the taken action
+  float* s_T = s_theta + N;       // [N] target quantiles T_j
+  float* s_g = s_T + N;           // [N] gradient row
+  float* s_l = s_g + N;           // [N] loss sum of every online quantile
+  float* s_q = s_l + N;           // [2][A] target mean quantiles of s and s'
+  float* s_pi = s_q + 2 * A;      // [A] pi(s')
+  float* s_ell = s_pi + A;        // [A] l(s')
+  const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  stage_munchausen_rows<QR_T>(zs, z_on, z_tg, i, B, N2);  // phase 0
+  __syncthreads();
+  const int act = (int)actions[i];
+  for (int t = warp; t < 2 * A; t += QR_WARPS) {  // phase 1
+    const int row = t / A, a = t - row * A;
+    const float* r1 = zs + (size_t)(1 + row) * N2;
+    float x[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int c = lane + 32 * r;
+      x[r] = (c < N) ? dueling_q(r1, A, N, c, a) : 0.0f;
+    }
+    const float q = qr_row_mean<R>(x, N);
+    if (lane == 0) s_q[t] = q;
+  }
+  __syncthreads();
+  munchausen_stage(s_q, s_pi, s_ell, &s_b, A, act, alpha, tau, l0, i, bonus_out);  // phase 2
+  __syncthreads();
+  const float ret = __ldg(returns + i), scale = __fmul_rn(__ldg(nonterminals + i), gamma_n);
+  const float rb = __fadd_rn(ret, s_b);
+  const float* r2 = zs + 2 * N2;
+  for (int c = tid; c < N; c += QR_T) {
+    s_theta[c] = dueling_q(zs, A, N, c, act);
+    const float v = r2[c], mean = dueling_mean(r2, A, N, c);
+    const float cj = munchausen_soft_value([&](int a) { return dueling_q(v, r2[N + a * N + c], mean); }, s_pi, s_ell, A);
+    const float T = __fadd_rn(rb, __fmul_rn(scale, cj));
+    s_T[c] = T;
+    if (theta_out) theta_out[(size_t)i * N + c] = T;
+  }
+  __syncthreads();
+  qr_core<R>(s_theta, s_T, s_l, s_g, N, kappa, __fdiv_rn(__ldg(weights + i), (float)B), i, loss);  // phase 3
+  dueling_dz<QR_T>(dz + (size_t)i * N2, s_g, A, N, act);  // phase 4
+}
+
+// Plain entry point: quantile rows [B][A][N] of online(s), target(s) and target(s'); grad [B][A][N] as k_qr writes it.
+template <int R>
+__global__ void __launch_bounds__(QR_T)
+k_qr_munchausen(const float* __restrict__ q_on_s, const float* __restrict__ q_tg_s, const float* __restrict__ q_tg_ns,
+                const int64_t* __restrict__ actions, const float* __restrict__ returns,
+                const float* __restrict__ nonterminals, const float* __restrict__ weights, float kappa, float gamma_n,
+                float alpha, float tau, float l0, int B, int A, int N, float* __restrict__ loss, float* __restrict__ grad,
+                float* __restrict__ theta_out, float* __restrict__ bonus_out) {
+  extern __shared__ __align__(16) float s_dyn[];
+  __shared__ float s_b;
+  float* s_theta = s_dyn;
+  float* s_T = s_theta + N;
+  float* s_g = s_T + N;
+  float* s_l = s_g + N;
+  float* s_q = s_l + N;           // [2][A]
+  float* s_pi = s_q + 2 * A;      // [A]
+  float* s_ell = s_pi + A;        // [A]
+  const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const size_t row0 = (size_t)i * A;
+  for (int t = warp; t < 2 * A; t += QR_WARPS) {  // phase 1
+    const int row = t / A, a = t - row * A;
+    const float* src = (row == 0 ? q_tg_s : q_tg_ns) + (row0 + a) * N;
+    float x[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const int c = lane + 32 * r;
+      x[r] = (c < N) ? __ldg(src + c) : 0.0f;
+    }
+    const float q = qr_row_mean<R>(x, N);
+    if (lane == 0) s_q[t] = q;
+  }
+  __syncthreads();
+  const int act = (int)actions[i];
+  munchausen_stage(s_q, s_pi, s_ell, &s_b, A, act, alpha, tau, l0, i, bonus_out);  // phase 2
+  __syncthreads();
+  const float ret = __ldg(returns + i), scale = __fmul_rn(__ldg(nonterminals + i), gamma_n);
+  const float rb = __fadd_rn(ret, s_b);
+  const float* tn = q_tg_ns + row0 * N;
+  for (int c = tid; c < N; c += QR_T) {
+    s_theta[c] = __ldg(q_on_s + (row0 + act) * N + c);
+    const float cj = munchausen_soft_value([&](int a) { return __ldg(tn + (size_t)a * N + c); }, s_pi, s_ell, A);
+    const float T = __fadd_rn(rb, __fmul_rn(scale, cj));
+    s_T[c] = T;
+    if (theta_out) theta_out[(size_t)i * N + c] = T;
+  }
+  __syncthreads();
+  qr_core<R>(s_theta, s_T, s_l, s_g, N, kappa, __fdiv_rn(__ldg(weights + i), (float)B), i, loss);
+  float* gq = grad + row0 * N;
+  for (int idx = tid; idx < A * N; idx += QR_T) {
+    const int a = idx / N;
+    gq[idx] = (a == act) ? s_g[idx - a * N] : 0.0f;
+  }
+}
+
 // Greedy values for acting / evaluation under quantiles: k_q_select with the mean over quantiles in place of
 // softmax . support.  One warp per state; the dueling combination and the mean are k_qr_dueling's phase 1, bitwise.
 // VT: the mean of h^-1 of the quantiles (return units).
@@ -3373,6 +3561,73 @@ int rb_qr_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const 
                        float eps, rb_stream_t stream) {
   return qr_launch<true>("rb_qr_vt_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights,
                          kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, eps, stream);
+}
+
+// The Munchausen entries' own refusals: alpha in [0, 1], tau finite and >= FLT_MIN (a normal fp32), l0 finite and < 0;
+// NaN fails every comparison.
+static int munchausen_check(const char* name, float alpha, float tau, float l0) {
+  char msg[128];
+  if (!(alpha >= 0.0f && alpha <= 1.0f)) {
+    snprintf(msg, sizeof msg, "%s: alpha must be in [0, 1]", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (!(tau >= FLT_MIN) || !isfinite(tau)) {
+    snprintf(msg, sizeof msg, "%s: temperature must be finite and a normal fp32 > 0", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (!(l0 < 0.0f) || !isfinite(l0)) {
+    snprintf(msg, sizeof msg, "%s: clip must be finite and < 0", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  return RB_OK;
+}
+
+int rb_qr_dueling_munchausen_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                       const int64_t* actions, const float* returns, const float* nonterminals,
+                                       const float* weights, float kappa, float gamma_n, float alpha, float temperature,
+                                       float clip, int B, float* loss, float* dz, float* theta_out, float* bonus_out,
+                                       rb_stream_t stream) {
+  const char* name = "rb_qr_dueling_munchausen_loss_grad";
+  const int N = atoms, A = actions_n;
+  int rc = RB_OK;
+  if (!(z_online && z_target && actions && returns && nonterminals && weights && loss && dz)) rc = null_pointer(name);
+  if (rc == RB_OK) rc = qr_check(name, B, A, N, kappa);
+  if (rc == RB_OK) rc = munchausen_check(name, alpha, temperature, clip);
+  if (rc != RB_OK) return rc;
+  const size_t smem = (size_t)(3 * (N + A * N) + 4 * N + 4 * A) * sizeof(float);
+  rc = smem_check(name, smem, "actions * atoms too large");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling_munchausen<2>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling_munchausen<4>, smem, name);
+  if (rc != RB_OK) return rc;
+  const auto k = N <= 64 ? k_qr_dueling_munchausen<2> : k_qr_dueling_munchausen<4>;
+  { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
+    k<<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, kappa, gamma_n,
+                                               alpha, temperature, clip, B, A, N, loss, dz, theta_out, bonus_out); }
+  return check_launch(name);
+}
+
+int rb_qr_munchausen_loss_grad(const float* q_online_s, const float* q_target_s, const float* q_target_ns,
+                               const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                               float kappa, float gamma_n, float alpha, float temperature, float clip, int B, int A, int N,
+                               float* loss, float* grad_q_online_s, float* theta_out, float* bonus_out, rb_stream_t stream) {
+  const char* name = "rb_qr_munchausen_loss_grad";
+  int rc = RB_OK;
+  if (!(q_online_s && q_target_s && q_target_ns && actions && returns && nonterminals && weights && loss && grad_q_online_s))
+    rc = null_pointer(name);
+  if (rc == RB_OK) rc = qr_check(name, B, A, N, kappa);
+  if (rc == RB_OK) rc = munchausen_check(name, alpha, temperature, clip);
+  if (rc != RB_OK) return rc;
+  const size_t smem = (size_t)(4 * N + 4 * A) * sizeof(float);
+  rc = smem_check(name, smem, "too many actions");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_munchausen<2>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_munchausen<4>, smem, name);
+  if (rc != RB_OK) return rc;
+  const auto k = N <= 64 ? k_qr_munchausen<2> : k_qr_munchausen<4>;
+  { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
+    k<<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_target_s, q_target_ns, actions, returns, nonterminals, weights,
+                                               kappa, gamma_n, alpha, temperature, clip, B, A, N, loss, grad_q_online_s,
+                                               theta_out, bonus_out); }
+  return check_launch(name);
 }
 
 extern "C++" {
