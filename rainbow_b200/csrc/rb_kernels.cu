@@ -419,6 +419,7 @@ k_tree_sample(const float* __restrict__ tree, int64_t tree_start, int64_t size, 
 constexpr int GATHER_THREADS = 256;
 constexpr int FRAME_VEC = RB_FRAME_BYTES / 16;  // 441 uint4 per frame
 
+// bit k: record idx - (history - 1) + k starts an episode, for k < W
 __device__ __forceinline__ uint64_t window_first_bits(const int32_t* __restrict__ timestep, int64_t size, int64_t idx,
                                                       int history, int W) {
   // lane s (and s+32) looks at window record s; ballot -> 64-bit "timestep == 0" mask (memory.py:114)
@@ -447,72 +448,111 @@ __device__ __forceinline__ float4 u8x4_to_unit(uint32_t w) {
                      __fdiv_rn((float)((w >> 16) & 0xffu), 255.0f), __fdiv_rn((float)(w >> 24), 255.0f));
 }
 
+// rb_gather_horizon: every gather body takes n (the n_max the grid and the blanking window are sized for) and gamma_pow
+// from its arguments when HZ is false, and n_t = clamp(hz->n, 1, n_max), gamma_pow and gamma_n from the schedule's
+// current row when it is true.  Window slots the grid holds for n_max but n_t does not use -- used slots
+// >= H + min(n_t, H) -- exit at once; the rest map as for a launch with n = n_t.  A slot's blanking depends only on the
+// slots between it and slot H - 1, so the wider ballot changes nothing.
+//
+// What a gather CTA knows of its sample and window slot.  gather_slot fills it, or returns false for a slot the current n
+// does not use.
+struct GatherSlot {
+  int n, W, s, b, part;          // horizon in use; ballot width history + n_max; window slot; sample; part of the split
+  const float* gamma_pow;
+  float gamma_n;                 // 1 unless HZ
+  int64_t idx, rec0, pos;        // the sample's data index; that of window slot 0; that of slot s, wrapped
+  const uint4* src;              // the stored frame of slot s
+
+  // where slot s appears in output row `row` (copy * B + b) of `states` / `next_states`, nullptr where it does not
+  __device__ __forceinline__ float4* state_dst(float* __restrict__ states, size_t row, int history) const {
+    return s < history ? reinterpret_cast<float4*>(states + (row * history + s) * RB_FRAME_BYTES) : nullptr;
+  }
+  __device__ __forceinline__ float4* next_state_dst(float* __restrict__ next_states, size_t row, int history) const {
+    const int s = this->s, n = this->n;   // as values: through `this` the compares compile in another order
+    return (s >= n && s < n + history)
+               ? reinterpret_cast<float4*>(next_states + (row * history + (s - n)) * RB_FRAME_BYTES)
+               : nullptr;
+  }
+};
+
+template <bool HZ>
+__device__ __forceinline__ bool gather_slot(GatherSlot& g, int64_t size, const int64_t* __restrict__ data_idx, int history,
+                                            int n, const float* __restrict__ gamma_pow, int split,
+                                            const rb_horizon* __restrict__ hz) {
+  g.b = blockIdx.y;
+  g.W = history + n;
+  g.n = n; g.gamma_pow = gamma_pow; g.gamma_n = 1.0f;
+  if constexpr (HZ) { g.n = min(max(__ldg(&hz->n), 1), n); g.gamma_pow = hz->gamma_pow; g.gamma_n = __ldg(&hz->gamma_n); }
+  const int used = blockIdx.x / split;
+  g.part = blockIdx.x % split;
+  if (HZ && used >= history + min(g.n, history)) return false;
+  // used-slot -> window slot: slots [0,H) feed `states`, [n,n+H) feed `next_states`
+  g.s = (g.n >= history && used >= history) ? g.n + (used - history) : used;
+  g.idx = data_idx[g.b];
+  g.rec0 = g.idx - (history - 1);
+  g.pos = pymod(g.rec0 + g.s, size);
+  return true;
+}
+
+// Loads this thread's first vector of the caller's range [v0, v1) of the frame, and has warp 0 ballot the window's
+// episode starts into s_first; the caller syncs before reading it.  Issue the (rarely discarded) frame load first so it
+// overlaps the timestep loads that decide the blanking.
+__device__ __forceinline__ uint4 gather_prefetch(GatherSlot& g, const uint8_t* __restrict__ frames,
+                                                 const int32_t* __restrict__ timestep, int64_t size, int history, int v0,
+                                                 int v1, uint64_t& s_first) {
+  g.src = reinterpret_cast<const uint4*>(frames + (size_t)g.pos * RB_FRAME_BYTES);
+  uint4 pre = make_uint4(0, 0, 0, 0);
+  if (v0 + (int)threadIdx.x < v1) pre = __ldg(g.src + v0 + threadIdx.x);
+  if (threadIdx.x < 32) {
+    uint64_t f = window_first_bits(timestep, size, g.rec0, 1, g.W);   // the W records from slot 0's
+    if (threadIdx.x == 0) s_first = f;
+  }
+  return pre;
+}
+
 // per-sample scalars, once per sample (memory.py:140-145).  HZ (rb_gather_horizon): the nonterminal is written in discount
 // form, fl32(nonterminal * gamma_n), i.e. gamma_n or +0.
 template <bool HZ>
-__device__ __forceinline__ void gather_scalars(uint64_t first, const int32_t* __restrict__ action, const float* __restrict__ reward,
-                                               const uint8_t* __restrict__ nonterminal, int64_t size, int64_t idx, int b,
-                                               int history, int n, const float* __restrict__ gamma_pow,
-                                               int64_t* __restrict__ actions, float* __restrict__ returns,
-                                               float* __restrict__ nonterminals, float gamma_n) {
+__device__ __forceinline__ void gather_scalars(const GatherSlot& g, uint64_t first, const int32_t* __restrict__ action,
+                                               const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal,
+                                               int64_t size, int history, int64_t* __restrict__ actions,
+                                               float* __restrict__ returns, float* __restrict__ nonterminals) {
   const int sa = history - 1;
-  actions[b] = (int64_t)__ldg(action + pymod(idx, size));  // slot H-1 is never blanked
+  actions[g.b] = (int64_t)__ldg(action + pymod(g.idx, size));  // slot H-1 is never blanked
   float acc = 0.0f;
-  for (int k = 0; k < n; ++k) {
+  for (int k = 0; k < g.n; ++k) {
     int sk = sa + k;
-    float r = slot_blank(first, sk, history) ? 0.0f : __ldg(reward + pymod(idx + k, size));
-    acc = __fadd_rn(acc, __fmul_rn(r, __ldg(gamma_pow + k)));
+    float r = slot_blank(first, sk, history) ? 0.0f : __ldg(reward + pymod(g.idx + k, size));
+    acc = __fadd_rn(acc, __fmul_rn(r, __ldg(g.gamma_pow + k)));
   }
-  returns[b] = acc;
-  const int sl = history + n - 1;
-  const float nt = slot_blank(first, sl, history) ? 0.0f : (__ldg(nonterminal + pymod(idx + n, size)) ? 1.0f : 0.0f);
-  if constexpr (HZ) nonterminals[b] = __fmul_rn(nt, gamma_n);
-  else nonterminals[b] = nt;
+  returns[g.b] = acc;
+  const int sl = history + g.n - 1;
+  const float nt = slot_blank(first, sl, history) ? 0.0f : (__ldg(nonterminal + pymod(g.idx + g.n, size)) ? 1.0f : 0.0f);
+  if constexpr (HZ) nonterminals[g.b] = __fmul_rn(nt, g.gamma_n);
+  else nonterminals[g.b] = nt;
 }
 
-// rb_gather_horizon: the three gather bodies below take n (the n_max the grid and the blanking window are sized for) and
-// gamma_pow from their arguments when HZ is false, and n_t = clamp(hz->n, 1, n_max), gamma_pow and gamma_n from the
-// schedule's current row when it is true.  Window slots the grid holds for n_max but n_t does not use -- used slots
-// >= H + min(n_t, H) -- exit at once; the rest map as for a launch with n = n_t.  A slot's blanking depends only on the
-// slots between it and slot H - 1, so the wider ballot changes nothing.
 template <bool HZ>
 __device__ __forceinline__ void
 gather_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
             const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
-            const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+            const int64_t* __restrict__ data_idx, int history, int n, const float* __restrict__ gamma_pow,
             float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
             float* __restrict__ returns, float* __restrict__ nonterminals, int split, const rb_horizon* __restrict__ hz) {
   __shared__ uint64_t s_first;
-  const int b = blockIdx.y;
-  const int W = history + n;
-  float gamma_n = 1.0f;
-  if constexpr (HZ) { n = min(max(__ldg(&hz->n), 1), n); gamma_pow = hz->gamma_pow; gamma_n = __ldg(&hz->gamma_n); }
-  const int used = blockIdx.x / split, part = blockIdx.x % split;
-  if (HZ && used >= history + min(n, history)) return;
-  // used-slot -> window slot: slots [0,H) feed `states`, [n,n+H) feed `next_states`
-  const int s = (n >= history && used >= history) ? n + (used - history) : used;
-  const int64_t idx = data_idx[b];
-  const int64_t pos = pymod(idx - (history - 1) + s, size);
+  GatherSlot g;
+  if (!gather_slot<HZ>(g, size, data_idx, history, n, gamma_pow, split, hz)) return;
   const int per = (FRAME_VEC + split - 1) / split;
-  const int v0 = part * per, v1 = min(FRAME_VEC, v0 + per);
-  // issue the (rarely discarded) frame load first so it overlaps the timestep loads that decide the blanking
-  const uint4* src = reinterpret_cast<const uint4*>(frames + (size_t)pos * RB_FRAME_BYTES);
-  uint4 pre = make_uint4(0, 0, 0, 0);
-  if (v0 + (int)threadIdx.x < v1) pre = __ldg(src + v0 + threadIdx.x);
-  if (threadIdx.x < 32) {
-    uint64_t f = window_first_bits(timestep, size, idx, history, W);
-    if (threadIdx.x == 0) s_first = f;
-  }
+  const int v0 = g.part * per, v1 = min(FRAME_VEC, v0 + per);
+  const uint4 pre = gather_prefetch(g, frames, timestep, size, history, v0, v1, s_first);
   __syncthreads();
   const uint64_t first = s_first;
-  const bool blank = slot_blank(first, s, history);
+  const bool blank = slot_blank(first, g.s, history);
 
-  float4* dst_s = (s < history) ? reinterpret_cast<float4*>(states + ((size_t)b * history + s) * RB_FRAME_BYTES) : nullptr;
-  float4* dst_n = (s >= n && s < n + history)
-                      ? reinterpret_cast<float4*>(next_states + ((size_t)b * history + (s - n)) * RB_FRAME_BYTES)
-                      : nullptr;
+  float4* dst_s = g.state_dst(states, (size_t)g.b, history);
+  float4* dst_n = g.next_state_dst(next_states, (size_t)g.b, history);
   for (int v = v0 + threadIdx.x; v < v1; v += GATHER_THREADS) {
-    uint4 q = blank ? make_uint4(0, 0, 0, 0) : (v == v0 + (int)threadIdx.x ? pre : __ldg(src + v));
+    uint4 q = blank ? make_uint4(0, 0, 0, 0) : (v == v0 + (int)threadIdx.x ? pre : __ldg(g.src + v));
     float4 a = u8x4_to_unit(q.x), bq = u8x4_to_unit(q.y), c = u8x4_to_unit(q.z), d = u8x4_to_unit(q.w);
     if (dst_s) {
       __stcs(dst_s + 4 * v + 0, a); __stcs(dst_s + 4 * v + 1, bq); __stcs(dst_s + 4 * v + 2, c); __stcs(dst_s + 4 * v + 3, d);
@@ -522,8 +562,7 @@ gather_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ time
     }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0)
-    gather_scalars<HZ>(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns,
-                       nonterminals, gamma_n);
+    gather_scalars<HZ>(g, first, action, reward, nonterminal, size, history, actions, returns, nonterminals);
 }
 
 __global__ void __launch_bounds__(GATHER_THREADS)
@@ -532,7 +571,7 @@ k_gather(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timeste
          const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
          float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
          float* __restrict__ returns, float* __restrict__ nonterminals, int split) {
-  gather_body<false>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states,
+  gather_body<false>(frames, timestep, action, reward, nonterminal, size, data_idx, history, n, gamma_pow, states,
                      next_states, actions, returns, nonterminals, split, nullptr);
 }
 
@@ -542,7 +581,7 @@ k_gather_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ time
             const int64_t* __restrict__ data_idx, int B, int history, int n_max, const rb_horizon* __restrict__ hz,
             float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
             float* __restrict__ returns, float* __restrict__ nonterminals, int split) {
-  gather_body<true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, nullptr, states,
+  gather_body<true>(frames, timestep, action, reward, nonterminal, size, data_idx, history, n_max, nullptr, states,
                     next_states, actions, returns, nonterminals, split, hz);
 }
 
@@ -557,7 +596,7 @@ k_gather_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ time
 // float4 store lies inside one row.
 // Offsets: one Philox4x32-10 call per sample b, counter (c_lo, c_hi, b, SHIFT_STREAM) with c = *rng_counter (advanced by
 // rb_tree_sample just before), key = seed; words x, y -> the state's (oy, ox), z, w -> the next state's;
-// offset = (word * (2 pad + 1)) >> 32.
+// offset = (word * (2 pad + 1)) >> 32.  The kernels are k_gather_aug's body with one copy of each side and no intensity.
 constexpr int FRAME_SIDE = 84;
 constexpr int ROW_VEC = FRAME_SIDE / 4;              // float4 per output row
 constexpr uint32_t SHIFT_STREAM = 0x53484654u;       // "SHFT": apart from sampling (0x5A4D504C) and noise (0x4E4F4953 + i)
@@ -573,96 +612,6 @@ __device__ __forceinline__ float4 shifted4(const uint8_t* s_frame, int y, int x,
   const uint8_t* row = s_frame + clamp_px(y + dy) * FRAME_SIDE;
   return make_float4(__fdiv_rn((float)row[clamp_px(x + dx)], 255.0f), __fdiv_rn((float)row[clamp_px(x + 1 + dx)], 255.0f),
                      __fdiv_rn((float)row[clamp_px(x + 2 + dx)], 255.0f), __fdiv_rn((float)row[clamp_px(x + 3 + dx)], 255.0f));
-}
-
-template <bool HZ>
-__device__ __forceinline__ void
-gather_shift_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep,
-                  const int32_t* __restrict__ action, const float* __restrict__ reward,
-                  const uint8_t* __restrict__ nonterminal, int64_t size, const int64_t* __restrict__ data_idx, int B,
-                  int history, int n, const float* __restrict__ gamma_pow, float* __restrict__ states,
-                  float* __restrict__ next_states, int64_t* __restrict__ actions, float* __restrict__ returns,
-                  float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
-                  const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts,
-                  const rb_horizon* __restrict__ hz) {
-  __shared__ uint64_t s_first;
-  __shared__ __align__(16) uint8_t s_frame[RB_FRAME_BYTES];
-  const int b = blockIdx.y;
-  const int W = history + n;
-  float gamma_n = 1.0f;
-  if constexpr (HZ) { n = min(max(__ldg(&hz->n), 1), n); gamma_pow = hz->gamma_pow; gamma_n = __ldg(&hz->gamma_n); }
-  const int used = blockIdx.x / split, part = blockIdx.x % split;
-  if (HZ && used >= history + min(n, history)) return;
-  const int s = (n >= history && used >= history) ? n + (used - history) : used;
-  const int64_t idx = data_idx[b];
-  const int64_t pos = pymod(idx - (history - 1) + s, size);
-  const int rows = (FRAME_SIDE + split - 1) / split;
-  const int r0 = part * rows, r1 = min(FRAME_SIDE, r0 + rows);
-  // the 16-byte vectors covering input rows [r0 - pad, r1 + pad) (a frame starts on a 16-byte boundary: 7056 = 441 x 16)
-  const int v0 = max(r0 - pad, 0) * FRAME_SIDE / 16;
-  const int v1 = min(FRAME_VEC, (min(r1 + pad, FRAME_SIDE) * FRAME_SIDE + 15) / 16);
-  const uint4* src = reinterpret_cast<const uint4*>(frames + (size_t)pos * RB_FRAME_BYTES);
-  uint4 pre = make_uint4(0, 0, 0, 0);
-  if (v0 + (int)threadIdx.x < v1) pre = __ldg(src + v0 + threadIdx.x);
-  const unsigned long long c = *rng_counter;
-  if (threadIdx.x < 32) {
-    uint64_t f = window_first_bits(timestep, size, idx, history, W);
-    if (threadIdx.x == 0) s_first = f;
-  }
-  const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), (uint32_t)b, SHIFT_STREAM),
-                                make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-  const int oy_s = shift_offset(r.x, pad), ox_s = shift_offset(r.y, pad);
-  const int oy_n = shift_offset(r.z, pad), ox_n = shift_offset(r.w, pad);
-  __syncthreads();
-  const uint64_t first = s_first;
-  const bool blank = slot_blank(first, s, history);
-  if (!blank) {
-    uint4* dst = reinterpret_cast<uint4*>(s_frame);
-    for (int v = v0 + threadIdx.x; v < v1; v += GATHER_THREADS) dst[v] = (v == v0 + (int)threadIdx.x) ? pre : __ldg(src + v);
-  }
-  __syncthreads();
-
-  float4* dst_s = (s < history) ? reinterpret_cast<float4*>(states + ((size_t)b * history + s) * RB_FRAME_BYTES) : nullptr;
-  float4* dst_n = (s >= n && s < n + history)
-                      ? reinterpret_cast<float4*>(next_states + ((size_t)b * history + (s - n)) * RB_FRAME_BYTES)
-                      : nullptr;
-  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int i = r0 * ROW_VEC + threadIdx.x; i < r1 * ROW_VEC; i += GATHER_THREADS) {
-    const int y = i / ROW_VEC, x = (i - y * ROW_VEC) * 4;
-    if (dst_s) __stcs(dst_s + i, blank ? zero : shifted4(s_frame, y, x, oy_s - pad, ox_s - pad));
-    if (dst_n) __stcs(dst_n + i, blank ? zero : shifted4(s_frame, y, x, oy_n - pad, ox_n - pad));
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    gather_scalars<HZ>(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns,
-                       nonterminals, gamma_n);
-    int32_t* sh_s = shifts + 2 * (size_t)b;          // int32 [2][B][2]: (side, sample, (oy, ox))
-    int32_t* sh_n = shifts + 2 * ((size_t)B + b);
-    sh_s[0] = oy_s; sh_s[1] = ox_s;
-    sh_n[0] = oy_n; sh_n[1] = ox_n;
-  }
-}
-
-__global__ void __launch_bounds__(GATHER_THREADS)
-k_gather_shift(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
-               const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
-               const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
-               float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
-               float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
-               const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
-  gather_shift_body<false>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states,
-                           next_states, actions, returns, nonterminals, split, pad, seed, rng_counter, shifts, nullptr);
-}
-
-__global__ void __launch_bounds__(GATHER_THREADS)
-k_gather_shift_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep,
-                  const int32_t* __restrict__ action, const float* __restrict__ reward,
-                  const uint8_t* __restrict__ nonterminal, int64_t size, const int64_t* __restrict__ data_idx, int B,
-                  int history, int n_max, const rb_horizon* __restrict__ hz, float* __restrict__ states,
-                  float* __restrict__ next_states, int64_t* __restrict__ actions, float* __restrict__ returns,
-                  float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
-                  const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
-  gather_shift_body<true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, nullptr, states,
-                          next_states, actions, returns, nonterminals, split, pad, seed, rng_counter, shifts, hz);
 }
 
 // ================================================================================================
@@ -694,7 +643,10 @@ __device__ __forceinline__ float intensity_mult(float s, float normal) {
   return __fmaf_rn(s, fminf(fmaxf(normal, -2.0f), 2.0f), 1.0f);
 }
 
-template <bool HZ>
+// SHIFT (k_gather_shift*): one copy of each side and no intensity, fixed at compile time; `scales` is neither read nor
+// written.  Copy 0 draws from SHIFT_STREAM + 0 and [2][1][B][2] is the [2][B][2] offsets layout, so the draws and
+// `shifts` are those documented for k_gather_shift above.
+template <bool HZ, bool SHIFT>
 __device__ __forceinline__ void
 gather_aug_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
                 const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
@@ -703,32 +655,22 @@ gather_aug_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ 
                 float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, float intensity,
                 int m_copies, int k_copies, uint64_t seed, const unsigned long long* __restrict__ rng_counter,
                 int32_t* __restrict__ shifts, float* __restrict__ scales, const rb_horizon* __restrict__ hz) {
+  constexpr int MAX_COPIES = SHIFT ? 1 : RB_MAX_AUG_COPIES;
   __shared__ uint64_t s_first;
-  __shared__ int s_off[2][RB_MAX_AUG_COPIES][2];   // (side, copy, (dy, dx)) = offset - pad
-  __shared__ float s_mult[2][RB_MAX_AUG_COPIES];
+  __shared__ int s_off[2][MAX_COPIES][2];   // (side, copy, (dy, dx)) = offset - pad
+  __shared__ float s_mult[2][MAX_COPIES];
   __shared__ __align__(16) uint8_t s_frame[RB_FRAME_BYTES];
-  const int b = blockIdx.y;
-  const int W = history + n;
-  float gamma_n = 1.0f;
-  if constexpr (HZ) { n = min(max(__ldg(&hz->n), 1), n); gamma_pow = hz->gamma_pow; gamma_n = __ldg(&hz->gamma_n); }
-  const int copies = max(m_copies, k_copies);
-  const int used = blockIdx.x / split, part = blockIdx.x % split;
-  if (HZ && used >= history + min(n, history)) return;
-  const int s = (n >= history && used >= history) ? n + (used - history) : used;
-  const int64_t idx = data_idx[b];
-  const int64_t pos = pymod(idx - (history - 1) + s, size);
+  GatherSlot g;
+  if (!gather_slot<HZ>(g, size, data_idx, history, n, gamma_pow, split, hz)) return;
+  const int b = g.b, s = g.s;
+  const int copies = SHIFT ? 1 : max(m_copies, k_copies);
+  const bool scaled = !SHIFT && intensity > 0.0f;
   const int rows = (FRAME_SIDE + split - 1) / split;
-  const int r0 = part * rows, r1 = min(FRAME_SIDE, r0 + rows);
+  const int r0 = g.part * rows, r1 = min(FRAME_SIDE, r0 + rows);
+  // the 16-byte vectors covering input rows [r0 - pad, r1 + pad) (a frame starts on a 16-byte boundary: 7056 = 441 x 16)
   const int v0 = max(r0 - pad, 0) * FRAME_SIDE / 16;
   const int v1 = min(FRAME_VEC, (min(r1 + pad, FRAME_SIDE) * FRAME_SIDE + 15) / 16);
-  const uint4* src = reinterpret_cast<const uint4*>(frames + (size_t)pos * RB_FRAME_BYTES);
-  uint4 pre = make_uint4(0, 0, 0, 0);
-  if (v0 + (int)threadIdx.x < v1) pre = __ldg(src + v0 + threadIdx.x);
-  if (threadIdx.x < 32) {
-    uint64_t f = window_first_bits(timestep, size, idx, history, W);
-    if (threadIdx.x == 0) s_first = f;
-  }
-  const bool scaled = intensity > 0.0f;
+  const uint4 pre = gather_prefetch(g, frames, timestep, size, history, v0, v1, s_first);
   if (threadIdx.x >= 32 && threadIdx.x < 32 + copies) {   // one thread per copy draws its offsets and multipliers
     const int j = threadIdx.x - 32;
     const unsigned long long c = *rng_counter;
@@ -753,8 +695,10 @@ gather_aug_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ 
       int32_t* sh_n = shifts + 2 * ((size_t)(copies + j) * B + b);
       sh_s[0] = oy_s; sh_s[1] = ox_s;
       sh_n[0] = oy_n; sh_n[1] = ox_n;
-      scales[(size_t)j * B + b] = m_s;
-      scales[(size_t)(copies + j) * B + b] = m_n;
+      if constexpr (!SHIFT) {
+        scales[(size_t)j * B + b] = m_s;
+        scales[(size_t)(copies + j) * B + b] = m_n;
+      }
     }
   }
   __syncthreads();
@@ -762,19 +706,14 @@ gather_aug_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ 
   const bool blank = slot_blank(first, s, history);
   if (!blank) {
     uint4* dst = reinterpret_cast<uint4*>(s_frame);
-    for (int v = v0 + threadIdx.x; v < v1; v += GATHER_THREADS) dst[v] = (v == v0 + (int)threadIdx.x) ? pre : __ldg(src + v);
+    for (int v = v0 + threadIdx.x; v < v1; v += GATHER_THREADS) dst[v] = (v == v0 + (int)threadIdx.x) ? pre : __ldg(g.src + v);
   }
   __syncthreads();
 
-  const bool app_s = s < history, app_n = s >= n && s < n + history;
   const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
   for (int j = 0; j < copies; ++j) {
-    float4* dst_s = (app_s && j < m_copies)
-                        ? reinterpret_cast<float4*>(states + (((size_t)j * B + b) * history + s) * RB_FRAME_BYTES)
-                        : nullptr;
-    float4* dst_n = (app_n && j < k_copies)
-                        ? reinterpret_cast<float4*>(next_states + (((size_t)j * B + b) * history + (s - n)) * RB_FRAME_BYTES)
-                        : nullptr;
+    float4* dst_s = j < m_copies ? g.state_dst(states, (size_t)j * B + b, history) : nullptr;
+    float4* dst_n = j < k_copies ? g.next_state_dst(next_states, (size_t)j * B + b, history) : nullptr;
     const int dy_s = s_off[0][j][0], dx_s = s_off[0][j][1], dy_n = s_off[1][j][0], dx_n = s_off[1][j][1];
     const float m_s = s_mult[0][j], m_n = s_mult[1][j];
     for (int i = r0 * ROW_VEC + threadIdx.x; i < r1 * ROW_VEC; i += GATHER_THREADS) {
@@ -784,8 +723,32 @@ gather_aug_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ 
     }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0)
-    gather_scalars<HZ>(first, action, reward, nonterminal, size, idx, b, history, n, gamma_pow, actions, returns,
-                       nonterminals, gamma_n);
+    gather_scalars<HZ>(g, first, action, reward, nonterminal, size, history, actions, returns, nonterminals);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_shift(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
+               const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
+               const int64_t* __restrict__ data_idx, int B, int history, int n, const float* __restrict__ gamma_pow,
+               float* __restrict__ states, float* __restrict__ next_states, int64_t* __restrict__ actions,
+               float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
+               const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
+  gather_aug_body<false, true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow,
+                               states, next_states, actions, returns, nonterminals, split, pad, 0.0f, 1, 1, seed,
+                               rng_counter, shifts, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_shift_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep,
+                  const int32_t* __restrict__ action, const float* __restrict__ reward,
+                  const uint8_t* __restrict__ nonterminal, int64_t size, const int64_t* __restrict__ data_idx, int B,
+                  int history, int n_max, const rb_horizon* __restrict__ hz, float* __restrict__ states,
+                  float* __restrict__ next_states, int64_t* __restrict__ actions, float* __restrict__ returns,
+                  float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
+                  const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
+  gather_aug_body<true, true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, nullptr,
+                              states, next_states, actions, returns, nonterminals, split, pad, 0.0f, 1, 1, seed,
+                              rng_counter, shifts, nullptr, hz);
 }
 
 __global__ void __launch_bounds__(GATHER_THREADS)
@@ -796,9 +759,9 @@ k_gather_aug(const uint8_t* __restrict__ frames, const int32_t* __restrict__ tim
              float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, float intensity, int m_copies,
              int k_copies, uint64_t seed, const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts,
              float* __restrict__ scales) {
-  gather_aug_body<false>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states,
-                         next_states, actions, returns, nonterminals, split, pad, intensity, m_copies, k_copies, seed,
-                         rng_counter, shifts, scales, nullptr);
+  gather_aug_body<false, false>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow,
+                                states, next_states, actions, returns, nonterminals, split, pad, intensity, m_copies,
+                                k_copies, seed, rng_counter, shifts, scales, nullptr);
 }
 
 __global__ void __launch_bounds__(GATHER_THREADS)
@@ -809,9 +772,9 @@ k_gather_aug_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ 
                 float* __restrict__ returns, float* __restrict__ nonterminals, int split, int pad, float intensity,
                 int m_copies, int k_copies, uint64_t seed, const unsigned long long* __restrict__ rng_counter,
                 int32_t* __restrict__ shifts, float* __restrict__ scales) {
-  gather_aug_body<true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, nullptr, states,
-                        next_states, actions, returns, nonterminals, split, pad, intensity, m_copies, k_copies, seed,
-                        rng_counter, shifts, scales, hz);
+  gather_aug_body<true, false>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, nullptr,
+                               states, next_states, actions, returns, nonterminals, split, pad, intensity, m_copies,
+                               k_copies, seed, rng_counter, shifts, scales, hz);
 }
 
 // One thread: current <- table[min(*counter, T)] (a negative counter reads row 0), then ++*counter.  The first node of an
@@ -2962,14 +2925,17 @@ int rb_tree_sample(const float* tree, int64_t tree_start, int64_t size, const in
   return check_launch("rb_tree_sample");
 }
 
-static int gather_split(int ctas_without_split) {
+// The grid of a gather over a window of history + n (the k_*_hz kernels take n = n_max and retire the slots the current
+// n does not use): (used slots * split, B), each used slot split into `split` parts.
+static dim3 gather_grid(int history, int n, int B, int* split) {
+  const int used = (history + n < 2 * history) ? history + n : 2 * history;
   // aim for >= 4 CTAs per SM so small batches still cover the machine; a frame is 441 x 16 B
-  int split = 1;
-  while (split < 2 && ctas_without_split * split < rbi::SM_COUNT * 2) split *= 2;  // 221 of 256 threads busy per CTA at split 2
-  return split;
+  *split = 1;
+  while (*split < 2 && used * B * *split < rbi::SM_COUNT * 2) *split *= 2;  // 221 of 256 threads busy per CTA at split 2
+  return dim3(used * *split, B);
 }
 
-// the argument checks of rb_gather, shared with rb_gather_shift
+// the argument checks every gather entry point shares
 static int gather_check(const char* who, const uint8_t* frames, const int32_t* timestep, const int32_t* action,
                         const float* reward, const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B,
                         int history, int n, const float* gamma_pow, const float* states, const float* next_states,
@@ -2995,6 +2961,24 @@ static int gather_check(const char* who, const uint8_t* frames, const int32_t* t
   return RB_OK;
 }
 
+// the augmentation arguments of rb_gather_shift (pad_min 1, intensity 0, one copy), rb_gather_aug and rb_gather_horizon
+static int aug_check(const char* who, int pad, int pad_min, float intensity, int m_copies, int k_copies) {
+  char what[96];
+  if (pad < pad_min || pad > RB_MAX_SHIFT_PAD) {
+    snprintf(what, sizeof what, "%s: pad outside [%d, RB_MAX_SHIFT_PAD]", who, pad_min);
+    return fail(RB_ERR_RANGE, what);
+  }
+  if (!(intensity >= 0.0f && intensity <= 0.5f)) {
+    snprintf(what, sizeof what, "%s: intensity outside [0, 0.5]", who);
+    return fail(RB_ERR_RANGE, what);
+  }
+  if (m_copies < 1 || m_copies > RB_MAX_AUG_COPIES || k_copies < 1 || k_copies > RB_MAX_AUG_COPIES) {
+    snprintf(what, sizeof what, "%s: copies outside [1, RB_MAX_AUG_COPIES]", who);
+    return fail(RB_ERR_RANGE, what);
+  }
+  return RB_OK;
+}
+
 int rb_gather(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
               const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n,
               const float* gamma_pow, float* states, float* next_states, int64_t* actions, float* returns,
@@ -3002,9 +2986,8 @@ int rb_gather(const uint8_t* frames, const int32_t* timestep, const int32_t* act
   const int rc = gather_check("rb_gather", frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n,
                               gamma_pow, states, next_states, actions, returns, nonterminals);
   if (rc != RB_OK) return rc;
-  const int used = (history + n < 2 * history) ? history + n : 2 * history;
-  const int split = gather_split(used * B);
-  dim3 grid(used * split, B);
+  int split;
+  const dim3 grid = gather_grid(history, n, B, &split);
   { ProfScope prof_(RB_K_GATHER, (cudaStream_t)stream);
     k_gather<<<grid, GATHER_THREADS, 0, (cudaStream_t)stream>>>(frames, timestep, action, reward, nonterminal, size, data_idx,
                                                               B, history, n, gamma_pow, states, next_states, actions,
@@ -3021,10 +3004,10 @@ int rb_gather_shift(const uint8_t* frames, const int32_t* timestep, const int32_
                               n, gamma_pow, states, next_states, actions, returns, nonterminals);
   if (rc != RB_OK) return rc;
   if (!rng_counter || !shifts) return fail(RB_ERR_INVAL, "rb_gather_shift: null pointer");
-  if (pad < 1 || pad > RB_MAX_SHIFT_PAD) return fail(RB_ERR_RANGE, "rb_gather_shift: pad outside [1, RB_MAX_SHIFT_PAD]");
-  const int used = (history + n < 2 * history) ? history + n : 2 * history;
-  const int split = gather_split(used * B);
-  dim3 grid(used * split, B);
+  const int arc = aug_check("rb_gather_shift", pad, 1, 0.0f, 1, 1);
+  if (arc != RB_OK) return arc;
+  int split;
+  const dim3 grid = gather_grid(history, n, B, &split);
   { ProfScope prof_(RB_K_GATHER_SHIFT, (cudaStream_t)stream);
     k_gather_shift<<<grid, GATHER_THREADS, 0, (cudaStream_t)stream>>>(
       frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states, next_states, actions,
@@ -3041,15 +3024,12 @@ int rb_gather_aug(const uint8_t* frames, const int32_t* timestep, const int32_t*
                               gamma_pow, states, next_states, actions, returns, nonterminals);
   if (rc != RB_OK) return rc;
   if (!rng_counter || !shifts || !scales) return fail(RB_ERR_INVAL, "rb_gather_aug: null pointer");
-  if (pad < 0 || pad > RB_MAX_SHIFT_PAD) return fail(RB_ERR_RANGE, "rb_gather_aug: pad outside [0, RB_MAX_SHIFT_PAD]");
-  if (!(intensity >= 0.0f && intensity <= 0.5f)) return fail(RB_ERR_RANGE, "rb_gather_aug: intensity outside [0, 0.5]");
-  if (m_copies < 1 || m_copies > RB_MAX_AUG_COPIES || k_copies < 1 || k_copies > RB_MAX_AUG_COPIES)
-    return fail(RB_ERR_RANGE, "rb_gather_aug: copies outside [1, RB_MAX_AUG_COPIES]");
+  const int arc = aug_check("rb_gather_aug", pad, 0, intensity, m_copies, k_copies);
+  if (arc != RB_OK) return arc;
   if (pad == 0 && intensity == 0.0f && m_copies == 1 && k_copies == 1)
     return fail(RB_ERR_INVAL, "rb_gather_aug: no augmentation requested (that is rb_gather)");
-  const int used = (history + n < 2 * history) ? history + n : 2 * history;
-  const int split = gather_split(used * B);
-  dim3 grid(used * split, B);
+  int split;
+  const dim3 grid = gather_grid(history, n, B, &split);
   { ProfScope prof_(RB_K_GATHER_AUG, (cudaStream_t)stream);
     k_gather_aug<<<grid, GATHER_THREADS, 0, (cudaStream_t)stream>>>(
       frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n, gamma_pow, states, next_states, actions,
@@ -3075,18 +3055,14 @@ int rb_gather_horizon(const uint8_t* frames, const int32_t* timestep, const int3
                               n_max, reinterpret_cast<const float*>(current), states, next_states, actions, returns,
                               nonterminals);
   if (rc != RB_OK) return rc;
-  if (pad < 0 || pad > RB_MAX_SHIFT_PAD) return fail(RB_ERR_RANGE, "rb_gather_horizon: pad outside [0, RB_MAX_SHIFT_PAD]");
-  if (!(intensity >= 0.0f && intensity <= 0.5f)) return fail(RB_ERR_RANGE, "rb_gather_horizon: intensity outside [0, 0.5]");
-  if (m_copies < 1 || m_copies > RB_MAX_AUG_COPIES || k_copies < 1 || k_copies > RB_MAX_AUG_COPIES)
-    return fail(RB_ERR_RANGE, "rb_gather_horizon: copies outside [1, RB_MAX_AUG_COPIES]");
+  const int arc = aug_check("rb_gather_horizon", pad, 0, intensity, m_copies, k_copies);
+  if (arc != RB_OK) return arc;
   const bool plain = pad == 0 && intensity == 0.0f && m_copies == 1 && k_copies == 1;
   const bool shift = !plain && intensity == 0.0f && m_copies == 1 && k_copies == 1;
   if (!plain && (!rng_counter || !shifts || (!shift && !scales)))
     return fail(RB_ERR_INVAL, "rb_gather_horizon: null pointer");
-  // the grid of a launch with n = n_max; k_*_hz retire the slots the current n does not use
-  const int used = (history + n_max < 2 * history) ? history + n_max : 2 * history;
-  const int split = gather_split(used * B);
-  dim3 grid(used * split, B);
+  int split;
+  const dim3 grid = gather_grid(history, n_max, B, &split);
   const unsigned long long* ctr = (const unsigned long long*)rng_counter;
   cudaStream_t s = (cudaStream_t)stream;
   // profiled under the id of the gather this launch stands for
