@@ -497,6 +497,46 @@ int rb_qr_munchausen_loss_grad(const float* q_online_s, const float* q_target_s,
                                float kappa, float gamma_n, float alpha, float temperature, float clip, int B, int A, int N,
                                float* loss, float* grad_q_online_s, float* theta_out, float* bonus_out, rb_stream_t stream);
 
+/* Risk-sensitive selection (distortion risk measures, Dabney et al. 2018 §5; DESIGN.md §18): the double-DQN arg-max and
+ * the greedy values read the return distribution through a distortion beta: [0, 1] -> [0, 1] in place of its mean,
+ *   RB_RISK_CVAR  beta(t) = min(t / eta, 1),          eta in (0, 1]  (1: the mean);
+ *   RB_RISK_WANG  beta(t) = Phi(Phi^-1(t) - eta),     eta finite     (< 0 risk-averse, 0 the mean, > 0 risk-seeking),
+ * beta(t) being the weight of the levels [0, t]: the inverses of IQN's level maps eta tau and Phi(Phi^-1(tau) + eta).
+ * Quantile rows: Q_beta = sum_j (beta((j+1)/N) - beta(j/N)) theta_j, quantile j standing for the levels [j/N, (j+1)/N]
+ * in index order.  Categorical rows: p = softmax over atoms, F_k = sum_{k' <= k} p_k' (F_{Z-1} = 1),
+ * Q_beta = sum_k (beta(F_k) - beta(F_{k-1})) support_k with F_{-1} = 0; the support must be non-decreasing (the agent's
+ * linspace is).  DESIGN.md §18 states the fp32 operation order.
+ * Each entry below is its parent's (the name without _risk) with Q_beta in place of the mean, and the parent's arguments
+ * plus risk_kind and risk_eta: in the loss entries Q_beta of online(s') picks a* (the first maximum wins), and everything
+ * after it -- the projection or the quantile loss, the loss, the gradient, m_out / theta_out and astar_out -- is the
+ * parent's for that a*; rb_q_values_risk / rb_qr_q_values_risk write Q_beta per action, its arg-max and its max.
+ * RB_ERR_INVAL: the parent's refusals, plus a kind other than RB_RISK_CVAR / RB_RISK_WANG, a CVaR eta outside (0, 1] or a
+ * Wang eta that is not finite (NaN refused).  A refused call writes nothing.  Profiled under the parent's kernel id. */
+#define RB_RISK_CVAR 1
+#define RB_RISK_WANG 2
+int rb_c51_risk_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                          const float* returns, const float* nonterminals, const float* weights, const float* support,
+                          float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z, float* loss,
+                          float* grad_q_online_s, float* m_out, int64_t* astar_out, int risk_kind, float risk_eta,
+                          rb_stream_t stream);
+int rb_c51_dueling_risk_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                  const int64_t* actions, const float* returns, const float* nonterminals,
+                                  const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                  float gamma_n, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                  int risk_kind, float risk_eta, rb_stream_t stream);
+int rb_qr_dueling_risk_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                 const int64_t* actions, const float* returns, const float* nonterminals,
+                                 const float* weights, float kappa, float gamma_n, int B, float* loss, float* dz,
+                                 float* theta_out, int64_t* astar_out, int risk_kind, float risk_eta, rb_stream_t stream);
+int rb_qr_risk_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                         const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
+                         int B, int A, int N, float* loss, float* grad_q_online_s, float* theta_out, int64_t* astar_out,
+                         int risk_kind, float risk_eta, rb_stream_t stream);
+int rb_q_values_risk(const float* z, int M, int actions, int atoms, const float* support, float* q, int64_t* best_action,
+                     float* best_q, int risk_kind, float risk_eta, rb_stream_t stream);
+int rb_qr_q_values_risk(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
+                        int risk_kind, float risk_eta, rb_stream_t stream);
+
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */
 int rb_noisy_compose(const float* mu, const float* sigma, const float* eps, int64_t count, float* out,

@@ -162,6 +162,17 @@ SIGNATURES = {
                                                      _f32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "rb_qr_munchausen_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32, _i32, _i32,
                                              _i32, _vp, _vp, _vp, _vp, _vp]),
+    # risk-sensitive selection: each is its parent's signature with risk_kind, risk_eta inserted before the stream
+    "rb_c51_risk_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i32, _i32, _i32,
+                                        _vp, _vp, _vp, _vp, _i32, _f32, _vp]),
+    "rb_c51_dueling_risk_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32,
+                                                _i32, _vp, _vp, _vp, _vp, _i32, _f32, _vp]),
+    "rb_qr_dueling_risk_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _vp, _vp, _vp,
+                                               _vp, _i32, _f32, _vp]),
+    "rb_qr_risk_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _i32, _i32, _vp, _vp, _vp, _vp,
+                                       _i32, _f32, _vp]),
+    "rb_q_values_risk": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _vp]),
+    "rb_qr_q_values_risk": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _f32, _vp]),
 }
 
 # rb_learn_stats_record of include/rainbow_b200.h (48 bytes): field name -> numpy dtype, in memory order

@@ -23,7 +23,9 @@ One `learn(mem)` (agent.py:61-100) is:
                                                (args.quantile_average_copies) rb_qr_dueling_avg_loss_grad -- the target
                                                quantiles averaged over the K copies, the loss over the M copies;
                                                args.munchausen: rb_qr_dueling_munchausen_loss_grad -- the target net's
-                                               softmax policy in place of the arg-max, and a clipped log-policy bonus]
+                                               softmax policy in place of the arg-max, and a clipped log-policy bonus;
+                                               args.risk_measure: the _risk twin of the loss entry -- the arg-max on a
+                                               distorted expectation (CVaR / Wang) in place of the mean]
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
@@ -58,13 +60,18 @@ from .memory import ReplayMemory, _SampleWorkspace
 from .model import DQN, FusedHead, NoisyLinear
 
 
-def _loss_grad(entries, args, loss, grad, outs, vt):
+def _loss_grad(entries, args, loss, grad, outs, vt, risk=None):
     """The body the loss wrappers share: launch entries[0], or under value rescaling (vt: its trailing arguments, None
-    when off) entries[1], on `args`, the outputs loss and grad, the optional outputs `outs` and the stream; returns
-    (loss, grad)."""
+    when off) entries[1], or under a risk measure (risk: (kind, eta), None when off) entries[2], on `args`, the outputs
+    loss and grad, the optional outputs `outs` and the stream; returns (loss, grad)."""
     lib = _lib.load()
-    fn = getattr(lib, entries[0] if vt is None else entries[1])
-    _lib.check(fn(*args, _lib.ptr(loss), _lib.ptr(grad), *map(_lib.ptr, outs), *(vt or ()), _lib.stream()))
+    if risk is not None:
+        if vt is not None:
+            raise ValueError("a risk measure does not compose with value rescaling")
+        fn, tail = getattr(lib, entries[2]), (int(risk[0]), float(risk[1]))
+    else:
+        fn, tail = getattr(lib, entries[0] if vt is None else entries[1]), vt or ()
+    _lib.check(fn(*args, _lib.ptr(loss), _lib.ptr(grad), *map(_lib.ptr, outs), *tail, _lib.stream()))
     return loss, grad
 
 
@@ -73,32 +80,34 @@ def _empty(*shape, like):
 
 
 def c51_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax,
-                  delta_z, gamma_n, loss=None, grad=None, m_out=None, astar_out=None, support_q=None, eps=None):
+                  delta_z, gamma_n, loss=None, grad=None, m_out=None, astar_out=None, support_q=None, eps=None, risk=None):
     """Launch K3 on pre-softmax logits [B,A,Z]; returns (loss[B], grad[B,A,Z]).  eps given: value rescaling
-    (rb_c51_vt_loss_grad) with support_q = fl32(h^-1(support))."""
+    (rb_c51_vt_loss_grad) with support_q = fl32(h^-1(support)).  risk = (kind, eta) given: the distorted arg-max
+    (rb_c51_risk_loss_grad, DESIGN.md §18)."""
     B, A, Z = q_online_s.shape
     return _loss_grad(
-        ("rb_c51_loss_grad", "rb_c51_vt_loss_grad"),
+        ("rb_c51_loss_grad", "rb_c51_vt_loss_grad", "rb_c51_risk_loss_grad"),
         (_lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
          _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
          float(gamma_n), B, A, Z),
         _empty(B, like=q_online_s) if loss is None else loss, _empty(B, A, Z, like=q_online_s) if grad is None else grad,
-        (m_out, astar_out), None if eps is None else (_lib.ptr(support_q), float(eps)))
+        (m_out, astar_out), None if eps is None else (_lib.ptr(support_q), float(eps)), risk)
 
 
 def c51_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin, vmax,
-                          delta_z, gamma_n, m_out=None, astar_out=None, support_q=None, eps=None):
+                          delta_z, gamma_n, m_out=None, astar_out=None, support_q=None, eps=None, risk=None):
     """K3 fed straight by the fused heads (rb_c51_dueling_loss_grad): z_online [2B, Z(1+A)] (s rows, then s' rows),
     z_target [B, Z(1+A)]; returns (loss[B], dz[B, Z(1+A)]) with dz = d mean(w*loss) / d (z_value | z_advantage).
-    eps given: value rescaling (rb_c51_dueling_vt_loss_grad) with support_q = fl32(h^-1(support))."""
+    eps given: value rescaling (rb_c51_dueling_vt_loss_grad) with support_q = fl32(h^-1(support)).  risk = (kind, eta)
+    given: the distorted arg-max (rb_c51_dueling_risk_loss_grad)."""
     B = actions.shape[0]
     return _loss_grad(
-        ("rb_c51_dueling_loss_grad", "rb_c51_dueling_vt_loss_grad"),
+        ("rb_c51_dueling_loss_grad", "rb_c51_dueling_vt_loss_grad", "rb_c51_dueling_risk_loss_grad"),
         (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
          _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
          float(gamma_n), B),
         _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (m_out, astar_out),
-        None if eps is None else (_lib.ptr(support_q), float(eps)))
+        None if eps is None else (_lib.ptr(support_q), float(eps)), risk)
 
 
 def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin,
@@ -118,29 +127,30 @@ def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, ret
 
 
 def qr_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, kappa, gamma_n,
-                 theta_out=None, astar_out=None, eps=None):
+                 theta_out=None, astar_out=None, eps=None, risk=None):
     """The quantile loss (rb_qr_loss_grad) on quantile rows [B,A,N]; returns (loss[B], grad[B,A,N]).  eps given: value
-    rescaling (rb_qr_vt_loss_grad)."""
+    rescaling (rb_qr_vt_loss_grad).  risk = (kind, eta) given: the distorted arg-max (rb_qr_risk_loss_grad)."""
     B, A, N = q_online_s.shape
     return _loss_grad(
-        ("rb_qr_loss_grad", "rb_qr_vt_loss_grad"),
+        ("rb_qr_loss_grad", "rb_qr_vt_loss_grad", "rb_qr_risk_loss_grad"),
         (_lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
          _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B, A, N),
         _empty(B, like=q_online_s), _empty(B, A, N, like=q_online_s), (theta_out, astar_out),
-        None if eps is None else (float(eps),))
+        None if eps is None else (float(eps),), risk)
 
 
 def qr_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, kappa, gamma_n,
-                         theta_out=None, astar_out=None, eps=None):
+                         theta_out=None, astar_out=None, eps=None, risk=None):
     """The quantile loss fed straight by the fused heads (rb_qr_dueling_loss_grad), rows as c51_dueling_loss_grad takes
-    them; returns (loss[B], dz[B, N(1+A)]).  eps given: value rescaling (rb_qr_dueling_vt_loss_grad)."""
+    them; returns (loss[B], dz[B, N(1+A)]).  eps given: value rescaling (rb_qr_dueling_vt_loss_grad).  risk = (kind, eta)
+    given: the distorted arg-max (rb_qr_dueling_risk_loss_grad)."""
     B = actions.shape[0]
     return _loss_grad(
-        ("rb_qr_dueling_loss_grad", "rb_qr_dueling_vt_loss_grad"),
+        ("rb_qr_dueling_loss_grad", "rb_qr_dueling_vt_loss_grad", "rb_qr_dueling_risk_loss_grad"),
         (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
          _lib.ptr(nonterminals), _lib.ptr(weights), float(kappa), float(gamma_n), B),
         _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (theta_out, astar_out),
-        None if eps is None else (float(eps),))
+        None if eps is None else (float(eps),), risk)
 
 
 def qr_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, kappa, gamma_n,
@@ -290,6 +300,68 @@ def munchausen_options(args):
             raise ValueError(f"{key} must be {want}, got {v}")
         out.append(v32)
     return tuple(out)
+
+
+RISK_KINDS = {"cvar": 1, "wang": 2}          # RB_RISK_CVAR, RB_RISK_WANG
+RISK_ETA_DEFAULTS = {"cvar": 0.25, "wang": -0.75}   # IQN's settings (Dabney et al. 2018, §5)
+
+
+def risk_options(args):
+    """(measure, eta) of risk-sensitive selection (a distortion risk measure, DESIGN.md §18) from `args`, or None when
+    args.risk_measure is absent, None or "neutral".  risk_measure "cvar" (beta(t) = min(t / eta, 1), eta in (0, 1],
+    default 0.25) or "wang" (beta(t) = Phi(Phi^-1(t) - eta), eta finite, default -0.75: eta < 0 is risk-averse, as in
+    IQN, whose level map Phi(Phi^-1(tau) + eta) is beta's inverse); args.risk_eta (absent or None:
+    the default) is returned rounded to the fp32 the kernels take, and checked both before and after the rounding.  The
+    distorted value Q_beta replaces the mean in acting, evaluation and the double-DQN arg-max.  Refused with it:
+    value_transform "rescale", args.munchausen (its target has no arg-max) and augment_m / augment_k other than (1, 1)."""
+    measure = getattr(args, "risk_measure", None)
+    if measure is None or measure == "neutral":
+        return None
+    if measure not in RISK_KINDS:
+        raise ValueError(f"risk_measure must be 'cvar', 'wang', 'neutral' or None, got {measure!r}")
+    if getattr(args, "value_transform", None) not in (None, "none"):
+        raise ValueError("risk_measure does not compose with value_transform 'rescale'")
+    if getattr(args, "munchausen", None):
+        raise ValueError("risk_measure does not compose with munchausen: the Munchausen target has no arg-max")
+    copies = (getattr(args, "augment_m", 1), getattr(args, "augment_k", 1))
+    if copies != (1, 1):
+        raise ValueError(f"risk_measure needs augment_m = augment_k = 1, got {copies}")
+    eta = getattr(args, "risk_eta", None)
+    eta = RISK_ETA_DEFAULTS[measure] if eta is None else eta
+    if isinstance(eta, bool) or not isinstance(eta, (int, float, np.floating, np.integer)):
+        raise ValueError(f"risk_eta must be a number, got {eta!r}")
+    with np.errstate(over="ignore"):
+        eta32 = float(np.float32(eta))
+    if measure == "cvar":
+        ok, want = (lambda v: 0.0 < v <= 1.0), "in (0, 1] for 'cvar'"
+    else:
+        ok, want = (lambda v: -math.inf < v < math.inf), "finite (as an fp32) for 'wang'"
+    if not (ok(float(eta)) and ok(eta32)):
+        raise ValueError(f"risk_eta must be {want}, got {eta}")
+    return measure, eta32
+
+
+def risk_beta(t, measure, eta):
+    """The distortion beta(t) of DESIGN.md §18 elementwise in t's dtype: "cvar" min(t / eta, 1), "wang"
+    Phi(Phi^-1(t) - eta) (torch.special.ndtri / ndtr)."""
+    if measure == "cvar":
+        return (t / eta).clamp(max=1.0)
+    return torch.special.ndtr(torch.special.ndtri(t) - eta)
+
+
+def risk_values(x, measure, eta, support=None):
+    """Q_beta over the last dim with torch ops: quantile rows x (support None) weighted by beta((j+1)/N) - beta(j/N) in
+    index order, or probability rows x over a non-decreasing support weighted by beta(F_k) - beta(F_{k-1}) with F the
+    cumulative sum in atom order (F_{Z-1} = 1, F_{-1} = 0)."""
+    n = x.shape[-1]
+    if support is None:
+        b = risk_beta(torch.arange(n + 1, dtype=x.dtype, device=x.device) / n, measure, eta)
+        return (x * (b[1:] - b[:-1])).sum(-1)
+    F = x.cumsum(-1).clamp(max=1.0)
+    F[..., -1] = 1.0
+    b = risk_beta(F, measure, eta)
+    w = b - torch.nn.functional.pad(b[..., :-1], (1, 0))
+    return (w * support).sum(-1)
 
 
 def vt_hinv(y, eps):
@@ -593,6 +665,9 @@ class Agent:
         # Munchausen targets under the quantile loss (off by default): (alpha, temperature, clip) or None; the online net
         # then runs on s only and the target net on [s; s']
         self.munchausen = munchausen_options(args)
+        # risk-sensitive selection (off by default): (measure, eta) or None; Q_beta replaces the mean in acting, evaluation
+        # and the double-DQN arg-max
+        self.risk = risk_options(args)
         # value rescaling (off by default): the network learns in h units, V_min / V_max included; acting, evaluation and
         # the statistics report return units
         self.value_transform, self.value_transform_eps = value_transform_options(args)
@@ -754,6 +829,8 @@ class Agent:
         noisy dueling head, then rb_q_values -- softmax over atoms, expectation over the support (agent.py:55) and the
         arg-max / max over actions in one launch; under the quantile distribution rb_qr_q_values, the mean over quantiles.
         Under value rescaling the values are in return units: the expectation over q_support, or rb_qr_vt_q_values.
+        Under a risk measure (args.risk_measure) the values are the distorted Q_beta of DESIGN.md §18: rb_q_values_risk or
+        rb_qr_q_values_risk, and evaluation reports max_a Q_beta.
         Returns device tensors (actions int64[N], values float32[N]); nothing synchronises.  Falls back to plain torch ops
         for head shapes the fused kernels do not cover."""
         on = self.online_net
@@ -765,7 +842,13 @@ class Agent:
                 best_a = torch.empty(N, dtype=torch.int64, device=self.device)
                 best_q = torch.empty(N, dtype=torch.float32, device=self.device)
                 lib, outs = _lib.load(), (_lib.ptr(q_out), _lib.ptr(best_a), _lib.ptr(best_q))
-                if self.quantile and self.value_transform is not None:
+                if self.risk is not None and self.quantile:
+                    _lib.check(lib.rb_qr_q_values_risk(_lib.ptr(z), N, self.action_space, self.atoms, *outs,
+                                                       *self._risk_args(), _lib.stream()))
+                elif self.risk is not None:
+                    _lib.check(lib.rb_q_values_risk(_lib.ptr(z), N, self.action_space, self.atoms, _lib.ptr(self.q_support),
+                                                    *outs, *self._risk_args(), _lib.stream()))
+                elif self.quantile and self.value_transform is not None:
                     _lib.check(lib.rb_qr_vt_q_values(_lib.ptr(z), N, self.action_space, self.atoms, *outs,
                                                      self.value_transform_eps, _lib.stream()))
                 elif self.quantile:
@@ -774,7 +857,10 @@ class Agent:
                     _lib.check(lib.rb_q_values(_lib.ptr(z), N, self.action_space, self.atoms, _lib.ptr(self.q_support),
                                                *outs, _lib.stream()))
                 return best_a, best_q
-            if self.quantile:
+            if self.risk is not None:
+                x = on.logits(states) if self.quantile else on(states)
+                q = risk_values(x, *self.risk, support=None if self.quantile else self.q_support)
+            elif self.quantile:
                 q = on.logits(states)
                 q = (q if self.value_transform is None else vt_hinv(q, self.value_transform_eps)).mean(2)
             else:
@@ -1072,7 +1158,7 @@ class Agent:
         """The loss on the fused heads' rows for M copies of s and K of s': rb_qr_dueling_loss_grad (quantile, M = K = 1)
         or rb_qr_dueling_avg_loss_grad (quantile, M or K > 1: args.quantile_average_copies), rb_c51_dueling_loss_grad, or
         at M or K > 1 rb_c51_dueling_avg_loss_grad; under Munchausen rb_qr_dueling_munchausen_loss_grad (z_online: s rows,
-        z_target: [s; s'] rows).  Returns (loss[B], dz, stats rows)."""
+        z_target: [s; s'] rows).  Under a risk measure the (1, 1) entries' _risk twins.  Returns (loss[B], dz, stats rows)."""
         _, _, actions, returns, _, nonterminals, weights = batch
         m = self._stats_rows(actions.shape[0])
         rows = (z_online, z_target, self.action_space, self.atoms, actions, returns, nonterminals, weights)
@@ -1081,28 +1167,35 @@ class Agent:
                                                      theta_out=m), m)
         vt = self._vt_args()
         if self.quantile and (M, K) == (1, 1):
-            return (*qr_dueling_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"]), m)
+            return (*qr_dueling_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"],
+                                          risk=self._risk_args()), m)
         if self.quantile:
             return (*qr_dueling_avg_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), M, K, theta_out=m,
                                               eps=vt["eps"]), m)
         c51 = (self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n())
         if (M, K) == (1, 1):
-            return (*c51_dueling_loss_grad(*rows, *c51, m_out=m, **vt), m)
+            return (*c51_dueling_loss_grad(*rows, *c51, m_out=m, **vt, risk=self._risk_args()), m)
         return (*c51_dueling_avg_loss_grad(*rows, *c51, M, K, m_out=m, **vt), m)
 
     def _library_loss(self, q_s, q_ns, q_t, batch):
         """The loss on the library head's logits [B, A, Z]: rb_qr_loss_grad (quantile) or rb_c51_loss_grad; under
-        Munchausen rb_qr_munchausen_loss_grad, q_ns then being the target's rows of s.  Returns (loss[B], grad[B, A, Z],
-        stats rows)."""
+        Munchausen rb_qr_munchausen_loss_grad, q_ns then being the target's rows of s; under a risk measure their _risk
+        twins.  Returns (loss[B], grad[B, A, Z], stats rows)."""
         _, _, actions, returns, _, nonterminals, weights = batch
         m = self._stats_rows(actions.shape[0])
         rows = (q_s, q_ns, q_t, actions, returns, nonterminals, weights)
         if self.munchausen is not None:
             return (*qr_munchausen_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), *self.munchausen, theta_out=m), m)
         vt = self._vt_args()
+        risk = self._risk_args()
         if self.quantile:
-            return (*qr_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"]), m)
-        return (*c51_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m, **vt), m)
+            return (*qr_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"], risk=risk), m)
+        return (*c51_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m, **vt,
+                               risk=risk), m)
+
+    def _risk_args(self):
+        """(kind, eta) of the _risk entries (RB_RISK_CVAR / RB_RISK_WANG), or None when no risk measure is set."""
+        return None if self.risk is None else (RISK_KINDS[self.risk[0]], self.risk[1])
 
     def _vt_args(self):
         """The loss wrappers' value-rescaling arguments: eps None (the plain entries) when the transform is off."""

@@ -381,6 +381,8 @@ def _meta(agent, mem):
         hyper["quantile_average_copies"] = True
     if agent.munchausen is not None:   # absent: no Munchausen targets
         hyper["munchausen_alpha"], hyper["munchausen_temperature"], hyper["munchausen_clip"] = agent.munchausen
+    if agent.risk is not None:   # absent: the mean selects (no risk measure)
+        hyper["risk_measure"], hyper["risk_eta"] = agent.risk
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
         learner["redo_count"] = agent.redo_count
     if opt.grouped:   # the group optimiser's bias-correction counts, [encoder, head]
@@ -535,6 +537,11 @@ def _validate(agent, mem, man):
     live = agent.munchausen or (None, None, None)
     if munch != live:
         raise _Error(f"munchausen (alpha, temperature, clip) differs: checkpoint {munch}, live {live}")
+    # and one whose policy read its distribution through another risk measure, or through none
+    risk = (hyper.get("risk_measure"), hyper.get("risk_eta"))
+    live = agent.risk or (None, None)
+    if risk != live:
+        raise _Error(f"risk measure (measure, eta) differs: checkpoint {risk}, live {live}")
     layout = agent.optimiser.state_dict(clone=False)["layout"]
     if man.get("optimiser") != layout:
         raise _Error(f"optimiser layout differs: checkpoint {man.get('optimiser')}, this learner {layout}")

@@ -1022,6 +1022,88 @@ __device__ __forceinline__ float c51_expected_value(const float (&x)[C51_R], con
   return __fdiv_rn(sn, se);
 }
 
+// ---- Risk-sensitive values: distortion risk measures of the return distribution (DESIGN.md §18) ----
+// The loss kernels' risk instantiations carry this bit in their atoms-per-lane parameter R (k_qr_dueling<2 | RISK_INST,
+// false> is k_qr_dueling<2, false> with the distorted arg-max): their template argument lists, and so the names graph
+// dumps and profiles show for the parent instantiations, stay as they were.
+constexpr int RISK_INST = 16;
+// beta(t) of the distortion `kind`, the weight of the levels [0, t]: RB_RISK_CVAR min(t / eta, 1), RB_RISK_WANG
+// Phi(Phi^-1(t) - eta) -- the inverses of IQN's level maps eta tau and Phi(Phi^-1(tau) + eta), so eta keeps IQN's sign
+// (normcdfinvf gives -inf / +inf at t = 0 / 1, so beta(0) = 0 and beta(1) = 1 exactly for both).
+__device__ __forceinline__ float risk_beta(float t, int kind, float eta) {
+  if (kind == RB_RISK_CVAR) return fminf(__fdiv_rn(t, eta), 1.0f);
+  return normcdff(__fsub_rn(normcdfinvf(t), eta));
+}
+
+// Distorted value Q_beta = sum_k w_k support_k of one logit row held as c51_expected_value takes it (support
+// non-decreasing), w_k = beta(F_k) - beta(F_{k-1}).  With e = expf(x - max x) and se = sum e (c51_expected_value's lane
+// sums and butterfly): S_k is the inclusive scan of e in atom order (per 32-atom segment a Hillis-Steele scan over the
+// lanes, offsets 1, 2, 4, 8, 16, then the previous segment's total added in front), F_k = min(S_k / se, 1) and
+// F_{Z-1} = 1.  Each lane sums w_k support_k over its atoms in r order, then the butterfly.  All lanes return the value.
+template <int C51_R>
+__device__ __forceinline__ float c51_risk_value(const float (&x)[C51_R], const float (&sup)[C51_R], int Z, int lane,
+                                                int kind, float eta) {
+  float mx = -CUDART_INF_F;
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) mx = fmaxf(mx, x[r]);
+  mx = warp_max(mx);
+  float e[C51_R], se = 0.0f;
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) {
+    e[r] = (lane + 32 * r < Z) ? expf(x[r] - mx) : 0.0f;
+    se = __fadd_rn(se, e[r]);
+  }
+  se = warp_sum(se);
+  float carry = 0.0f, b_carry = 0.0f, s = 0.0f;
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) {
+    const int k = lane + 32 * r;
+    float v = e[r];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const float y = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v = __fadd_rn(v, y);
+    }
+    v = __fadd_rn(carry, v);
+    carry = __shfl_sync(0xffffffffu, v, 31);
+    const float F = k >= Z - 1 ? 1.0f : fminf(__fdiv_rn(v, se), 1.0f);
+    const float b = risk_beta(F, kind, eta);
+    float bp = __shfl_up_sync(0xffffffffu, b, 1);
+    if (lane == 0) bp = b_carry;
+    b_carry = __shfl_sync(0xffffffffu, b, 31);
+    if (k < Z) s = __fadd_rn(s, __fmul_rn(__fsub_rn(b, bp), sup[r]));
+  }
+  return warp_sum(s);
+}
+
+// Level weights of the quantiles a lane owns (j = lane + 32 r): quantile j stands for the levels [j/N, (j+1)/N] in index
+// order (not value order: quantiles can cross), w_j = beta(fl32((j+1)/N)) - beta(fl32(j/N)), 0 past N.  They depend on
+// no row, so a warp forms them once for all the actions it takes.
+template <int R>
+__device__ __forceinline__ void qr_risk_weights(int N, int lane, int kind, float eta, float (&w)[R]) {
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const int j = lane + 32 * r;
+    w[r] = 0.0f;
+    if (j < N) {
+      const float lo = risk_beta(__fdiv_rn((float)j, (float)N), kind, eta);
+      const float hi = risk_beta(__fdiv_rn((float)(j + 1), (float)N), kind, eta);
+      w[r] = __fsub_rn(hi, lo);
+    }
+  }
+}
+
+// Distorted value of one quantile row held as qr_row_mean takes it, with qr_risk_weights' w: each lane sums w_j theta_j
+// over its quantiles in r order, then the butterfly.  All lanes return the value.
+template <int R>
+__device__ __forceinline__ float qr_risk_value(const float (&x)[R], const float (&w)[R], int N, int lane) {
+  float s = 0.0f;
+#pragma unroll
+  for (int r = 0; r < R; ++r)
+    if (lane + 32 * r < N) s = __fadd_rn(s, __fmul_rn(w[r], x[r]));
+  return warp_sum(s);
+}
+
 // q_on_ns / q_tg_ns: A rows of Z (row stride Z); q_on_s_act: the row of the taken action.
 // best_known >= 0: a* was already determined by the caller (q_on_ns is then not read, q_tg_ns points at the row of a*).
 // VT (value rescaling): support_q = fl32(h^-1(support)) replaces the support in the arg-max and in Tz, and the target atoms
@@ -1160,22 +1242,49 @@ __device__ __forceinline__ void c51_core(C51Scratch& sc, int lane, int i, int B,
 }
 
 // VT: the value-rescaled instantiation (c51_core's VT); support_q / eps are read only there.
-template <int C51_R, bool VT>
+// RISK (R with RISK_INST set): a* = argmax_a c51_risk_value of online(s') (first maximum wins), found here and handed to
+// c51_core as best_known; risk_kind / risk_eta are read only there.
+template <int C51_R_RISK, bool VT>
 __global__ void __launch_bounds__(C51_WARPS * 32)
 k_c51(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
       const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
       const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax, float delta_z,
-      float gamma_n, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ grad, float* __restrict__ m_out,
-      int64_t* __restrict__ astar_out, const float* __restrict__ support_q, float eps) {
+      float gamma_n, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ grad,
+      float* __restrict__ m_out, int64_t* __restrict__ astar_out, const float* __restrict__ support_q, float eps,
+      int risk_kind, float risk_eta) {
+  constexpr int C51_R = C51_R_RISK & ~RISK_INST;
+  constexpr bool RISK = (C51_R_RISK & RISK_INST) != 0;
   __shared__ C51Scratch s_sc[C51_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i = blockIdx.x * C51_WARPS + warp;
   if (i >= B) return;
   const int act = (int)actions[i];
   float g[C51_R];
-  c51_core<C51_R, VT>(s_sc[warp], lane, i, B, A, Z, q_on_ns + (size_t)i * A * Z, q_tg_ns + (size_t)i * A * Z,
+  const float* q_tg = q_tg_ns + (size_t)i * A * Z;
+  int best_known = -1;
+  if constexpr (RISK) {
+    float best_v = -CUDART_INF_F;
+    best_known = 0;
+    for (int a = 0; a < A; ++a) {
+      const float* row = q_on_ns + ((size_t)i * A + a) * Z;
+      float sup[C51_R], x[C51_R];
+#pragma unroll
+      for (int r = 0; r < C51_R; ++r) {
+        const int z = lane + 32 * r;
+        sup[r] = (z < Z) ? __ldg(support + z) : 0.0f;
+        x[r] = (z < Z) ? row[z] : -CUDART_INF_F;
+      }
+      const float v = c51_risk_value<C51_R>(x, sup, Z, lane, risk_kind, risk_eta);
+      if (v > best_v) {  // first maximum wins, like torch.argmax
+        best_v = v;
+        best_known = a;
+      }
+    }
+    q_tg += (size_t)best_known * Z;
+  }
+  c51_core<C51_R, VT>(s_sc[warp], lane, i, B, A, Z, q_on_ns + (size_t)i * A * Z, q_tg,
            q_on_s + ((size_t)i * A + act) * Z, __ldg(returns + i), __ldg(nonterminals + i), __ldg(weights + i), support, vmin,
-           vmax, delta_z, gamma_n, loss, m_out, astar_out, g, -1, support_q, eps);
+           vmax, delta_z, gamma_n, loss, m_out, astar_out, g, best_known, support_q, eps);
   float* gq = grad + (size_t)i * A * Z;
   for (int j = lane; j < A * Z; j += 32) gq[j] = 0.0f;
   __syncwarp();
@@ -1281,13 +1390,18 @@ __device__ __forceinline__ int first_argmax(const float* s, int n) {
 //   phase 3  all threads write dz:  dzv[z] = g[z],  dza[a][z] = g[z] * ([a == act] - 1/A).
 constexpr int C51D_T = 256;
 
-template <int C51_R, bool VT>
+// RISK (R with RISK_INST set): phase 1 computes c51_risk_value in place of the expected value; risk_kind / risk_eta
+// are read only there.
+template <int C51_R_RISK, bool VT>
 __global__ void __launch_bounds__(C51D_T)
 k_c51_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
-              const float* __restrict__ returns, const float* __restrict__ nonterminals, const float* __restrict__ weights,
-              const float* __restrict__ support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z,
-              float* __restrict__ loss, float* __restrict__ dz, float* __restrict__ m_out, int64_t* __restrict__ astar_out,
-              const float* __restrict__ support_q, float eps) {
+              const float* __restrict__ returns, const float* __restrict__ nonterminals,
+              const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax,
+              float delta_z, float gamma_n, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ dz,
+              float* __restrict__ m_out, int64_t* __restrict__ astar_out, const float* __restrict__ support_q,
+              float eps, int risk_kind, float risk_eta) {
+  constexpr int C51_R = C51_R_RISK & ~RISK_INST;
+  constexpr bool RISK = (C51_R_RISK & RISK_INST) != 0;
   extern __shared__ __align__(16) float s_dyn[];
   __shared__ C51Scratch s_sc;
   const int N2 = Z + A * Z;
@@ -1297,7 +1411,10 @@ k_c51_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, co
   float* s_g = q_s + Z;           // [Z] gradient row
   float* s_ev = s_g + Z;          // [A] expected values
   const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  {
+  if constexpr (RISK) {
+    // the same three rows in the same order through the shared stager, which keeps no stack array of row pointers
+    stage_z_rows<C51D_T>(zs, z_on, z_tg, i, B, N2, 1, 1);
+  } else {
     const int total = 3 * N2;
     const float* src[3] = {z_on + (size_t)i * N2, z_on + (size_t)(B + i) * N2, z_tg + (size_t)i * N2};
     for (int base = tid; base < total; base += C51D_T * 8) {
@@ -1343,7 +1460,9 @@ k_c51_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, co
         const int c = lane + 32 * r;
         x[r] = (c < Z) ? r1[c] + r1[Z + a * Z + c] - mean[r] : -CUDART_INF_F;
       }
-      const float ev = c51_expected_value<C51_R>(x, sup, Z, lane);
+      float ev;
+      if constexpr (RISK) ev = c51_risk_value<C51_R>(x, sup, Z, lane, risk_kind, risk_eta);
+      else ev = c51_expected_value<C51_R>(x, sup, Z, lane);
       if (lane == 0) s_ev[a] = ev;
     }
   }
@@ -1589,9 +1708,12 @@ k_c51_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg
 // atoms (model.py:79), expected value sum_z support_z p_z (agent.py:55), then the arg-max / max over actions --
 // everything after the network body in ONE launch, results stay on the device (no .item() per state).
 // ================================================================================================
+// RISK: c51_risk_value in place of the expected value (risk_kind / risk_eta are read only there).
+template <bool RISK>
 __global__ void __launch_bounds__(128)
-k_q_select(const float* __restrict__ z, int M, int A, int Z, const float* __restrict__ support, float* __restrict__ q_out,
-           int64_t* __restrict__ best_action, float* __restrict__ best_q) {
+k_q_select(const float* __restrict__ z, int M, int A, int Z, const float* __restrict__ support,
+           float* __restrict__ q_out, int64_t* __restrict__ best_action, float* __restrict__ best_q, int risk_kind,
+           float risk_eta) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m = blockIdx.x * 4 + warp;
   if (m >= M) return;
@@ -1617,7 +1739,9 @@ k_q_select(const float* __restrict__ z, int M, int A, int Z, const float* __rest
       const int c = lane + 32 * r;
       x[r] = (c < Z) ? dueling_q(zv[r], __ldg(zr + Z + a * Z + c), mean[r]) : -CUDART_INF_F;
     }
-    const float ev = c51_expected_value<R>(x, sup, Z, lane);
+    float ev;
+    if constexpr (RISK) ev = c51_risk_value<R>(x, sup, Z, lane, risk_kind, risk_eta);
+    else ev = c51_expected_value<R>(x, sup, Z, lane);
     if (q_out && lane == 0) q_out[(size_t)m * A + a] = ev;
     if (ev > best_ev) {   // first maximum wins, like torch.argmax / max
       best_ev = ev;
@@ -1715,12 +1839,17 @@ __device__ __forceinline__ void qr_core(const float* s_theta, const float* s_T, 
 // Dueling entry point: z rows as k_c51_dueling takes them (online 2B rows, s then s'; target B rows).
 // VT (value rescaling, quantiles in h units): a* = argmax_a mean_j h^-1(q_online(s', a)_j) and
 // T_j = h(r + fl32(scale * h^-1(q_target(s', a*)_j))); theta, the loss and the gradient stay in h units.
-template <int R, bool VT>
+// RISK (R with RISK_INST set): phase 1 computes qr_risk_value in place of the mean (risk_kind / risk_eta are read
+// only there).
+template <int R_RISK, bool VT>
 __global__ void __launch_bounds__(QR_T)
 k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
-             const float* __restrict__ returns, const float* __restrict__ nonterminals, const float* __restrict__ weights,
-             float kappa, float gamma_n, int B, int A, int N, float* __restrict__ loss, float* __restrict__ dz,
-             float* __restrict__ theta_out, int64_t* __restrict__ astar_out, float eps) {
+             const float* __restrict__ returns, const float* __restrict__ nonterminals,
+             const float* __restrict__ weights, float kappa, float gamma_n, int B, int A, int N,
+             float* __restrict__ loss, float* __restrict__ dz, float* __restrict__ theta_out,
+             int64_t* __restrict__ astar_out, float eps, int risk_kind, float risk_eta) {
+  constexpr int R = R_RISK & ~RISK_INST;
+  constexpr bool RISK = (R_RISK & RISK_INST) != 0;
   extern __shared__ __align__(16) float s_dyn[];
   const int N2 = N + A * N;
   float* zs = s_dyn;              // [3][N2]: online(s), online(s'), target(s')
@@ -1741,6 +1870,8 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
       const int c = lane + 32 * r;
       mean[r] = (c < N) ? dueling_mean(r1, A, N, c) : 0.0f;
     }
+    float w[R];
+    if constexpr (RISK) qr_risk_weights<R>(N, lane, risk_kind, risk_eta, w);
     for (int a = warp; a < A; a += QR_WARPS) {
       float x[R];
 #pragma unroll
@@ -1749,7 +1880,9 @@ k_qr_dueling(const float* __restrict__ z_on, const float* __restrict__ z_tg, con
         x[r] = (c < N) ? dueling_q(r1[c], r1[N + a * N + c], mean[r]) : 0.0f;
         if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
       }
-      const float q = qr_row_mean<R>(x, N);
+      float q;
+      if constexpr (RISK) q = qr_risk_value<R>(x, w, N, lane);
+      else q = qr_row_mean<R>(x, N);
       if (lane == 0) s_mean[a] = q;
     }
   }
@@ -1849,12 +1982,16 @@ k_qr_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg,
 
 // Plain entry point: quantile rows [B][A][N] of online(s), online(s') and target(s'); grad [B][A][N] is the gradient row
 // at the taken action and 0 elsewhere.
-template <int R, bool VT>
+// RISK: as k_qr_dueling's.
+template <int R_RISK, bool VT>
 __global__ void __launch_bounds__(QR_T)
 k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
      const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
      const float* __restrict__ weights, float kappa, float gamma_n, int B, int A, int N, float* __restrict__ loss,
-     float* __restrict__ grad, float* __restrict__ theta_out, int64_t* __restrict__ astar_out, float eps) {
+     float* __restrict__ grad, float* __restrict__ theta_out, int64_t* __restrict__ astar_out, float eps,
+     int risk_kind, float risk_eta) {
+  constexpr int R = R_RISK & ~RISK_INST;
+  constexpr bool RISK = (R_RISK & RISK_INST) != 0;
   extern __shared__ __align__(16) float s_dyn[];
   float* s_theta = s_dyn;
   float* s_T = s_theta + N;
@@ -1863,6 +2000,8 @@ k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const 
   float* s_mean = s_l + N;        // [A]
   const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const size_t row0 = (size_t)i * A;
+  float w[R];
+  if constexpr (RISK) qr_risk_weights<R>(N, lane, risk_kind, risk_eta, w);
   for (int a = warp; a < A; a += QR_WARPS) {  // phase 1
     float x[R];
 #pragma unroll
@@ -1871,7 +2010,9 @@ k_qr(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const 
       x[r] = (c < N) ? __ldg(q_on_ns + (row0 + a) * N + c) : 0.0f;
       if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
     }
-    const float q = qr_row_mean<R>(x, N);
+    float q;
+    if constexpr (RISK) q = qr_risk_value<R>(x, w, N, lane);
+    else q = qr_row_mean<R>(x, N);
     if (lane == 0) s_mean[a] = q;
   }
   __syncthreads();
@@ -2085,10 +2226,11 @@ k_qr_munchausen(const float* __restrict__ q_on_s, const float* __restrict__ q_tg
 // Greedy values for acting / evaluation under quantiles: k_q_select with the mean over quantiles in place of
 // softmax . support.  One warp per state; the dueling combination and the mean are k_qr_dueling's phase 1, bitwise.
 // VT: the mean of h^-1 of the quantiles (return units).
-template <bool VT>
+// RISK: qr_risk_value in place of the mean (risk_kind / risk_eta are read only there).
+template <bool VT, bool RISK>
 __global__ void __launch_bounds__(128)
-k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict__ q_out, int64_t* __restrict__ best_action,
-            float* __restrict__ best_q, float eps) {
+k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict__ q_out,
+            int64_t* __restrict__ best_action, float* __restrict__ best_q, float eps, int risk_kind, float risk_eta) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m = blockIdx.x * 4 + warp;
   if (m >= M) return;
@@ -2106,6 +2248,8 @@ k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict_
   }
   int best = 0;
   float best_v = -CUDART_INF_F;
+  float w[R];
+  if constexpr (RISK) qr_risk_weights<R>(N, lane, risk_kind, risk_eta, w);
   for (int a = 0; a < A; ++a) {
     float x[R];
 #pragma unroll
@@ -2114,7 +2258,9 @@ k_qr_select(const float* __restrict__ z, int M, int A, int N, float* __restrict_
       x[r] = (c < N) ? dueling_q(zv[r], __ldg(zr + N + a * N + c), mean[r]) : 0.0f;
       if constexpr (VT) x[r] = (c < N) ? vt_hinv(x[r], eps) : 0.0f;
     }
-    const float q = qr_row_mean<R>(x, N);
+    float q;
+    if constexpr (RISK) q = qr_risk_value<R>(x, w, N, lane);
+    else q = qr_row_mean<R>(x, N);
     if (q_out && lane == 0) q_out[(size_t)m * A + a] = q;
     if (q > best_v) {   // first maximum wins, like torch.argmax / max
       best_v = q;
@@ -3194,23 +3340,43 @@ static int smem_check(const char* name, size_t smem, const char* what) {
   return RB_OK;
 }
 
+// The risk entries' own refusals: a known kind; CVaR eta in (0, 1], Wang eta finite (NaN fails every comparison).
+static int risk_check(const char* name, int kind, float eta) {
+  char msg[128];
+  if (kind != RB_RISK_CVAR && kind != RB_RISK_WANG) {
+    snprintf(msg, sizeof msg, "%s: risk_kind must be RB_RISK_CVAR or RB_RISK_WANG", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (kind == RB_RISK_CVAR && !(eta > 0.0f && eta <= 1.0f)) {
+    snprintf(msg, sizeof msg, "%s: CVaR eta must be in (0, 1]", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  if (kind == RB_RISK_WANG && !isfinite(eta)) {
+    snprintf(msg, sizeof msg, "%s: Wang eta must be finite", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  return RB_OK;
+}
+
 extern "C++" {   // the shared launchers are templates, which cannot have C linkage
-template <bool VT>
+template <bool VT, bool RISK = false>
 static int c51_launch(const char* name, const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
                       const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
                       const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z,
                       float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, const float* support_q, float eps,
-                      rb_stream_t stream) {
+                      rb_stream_t stream, int risk_kind = 0, float risk_eta = 0.0f) {
   int rc = VT ? vt_check(name, support_q != nullptr, eps) : RB_OK;
   if (rc == RB_OK)
     rc = c51_check(name, q_online_s && q_online_ns && q_target_ns && actions && returns && nonterminals && weights &&
                    support && loss && grad_q_online_s, B, A, Z, "A", "Z");
+  if (rc == RB_OK && RISK) rc = risk_check(name, risk_kind, risk_eta);
   if (rc != RB_OK) return rc;
-  const auto k = Z <= 64 ? k_c51<2, VT> : k_c51<4, VT>;
+  constexpr int F = RISK ? RISK_INST : 0;
+  const auto k = Z <= 64 ? k_c51<2 | F, VT> : k_c51<4 | F, VT>;
   { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
     k<<<(B + C51_WARPS - 1) / C51_WARPS, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(
         q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n,
-        B, A, Z, loss, grad_q_online_s, m_out, astar_out, support_q, eps); }
+        B, A, Z, loss, grad_q_online_s, m_out, astar_out, support_q, eps, risk_kind, risk_eta); }
   return check_launch(name);
 }
 }
@@ -3232,6 +3398,16 @@ int rb_c51_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const
   return c51_launch<true>("rb_c51_vt_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals,
                           weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss, grad_q_online_s, m_out, astar_out,
                           support_q, eps, stream);
+}
+
+int rb_c51_risk_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                          const float* returns, const float* nonterminals, const float* weights, const float* support,
+                          float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z, float* loss,
+                          float* grad_q_online_s, float* m_out, int64_t* astar_out, int risk_kind, float risk_eta,
+                          rb_stream_t stream) {
+  return c51_launch<false, true>("rb_c51_risk_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns,
+                                 nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss, grad_q_online_s,
+                                 m_out, astar_out, nullptr, 0.0f, stream, risk_kind, risk_eta);
 }
 
 static int noisy_launch(float* const* weight_eps, float* const* bias_eps, const int* in_features, const int* out_features,
@@ -3296,27 +3472,30 @@ int rb_noisy_outer(float* const* weight_eps, float* const* bias_eps, const int* 
 }
 
 extern "C++" {
-template <bool VT>
+template <bool VT, bool RISK = false>
 static int c51_dueling_launch(const char* name, const float* z_online, const float* z_target, int actions_n, int atoms,
                               const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
                               const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, float* loss,
                               float* dz, float* m_out, int64_t* astar_out, const float* support_q, float eps,
-                              rb_stream_t stream) {
+                              rb_stream_t stream, int risk_kind = 0, float risk_eta = 0.0f) {
   const int Z = atoms, A = actions_n;
   int rc = VT ? vt_check(name, support_q != nullptr, eps) : RB_OK;
   if (rc == RB_OK)
     rc = c51_check(name, z_online && z_target && actions && returns && nonterminals && weights && support && loss && dz, B,
                    A, Z, "actions", "atoms");
+  if (rc == RB_OK && RISK) rc = risk_check(name, risk_kind, risk_eta);
   if (rc != RB_OK) return rc;
   const size_t smem = (size_t)(3 * (Z + A * Z) + 3 * Z + A) * sizeof(float);
   rc = smem_check(name, smem, "actions * atoms too large");
-  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling<2, VT>, smem, name);
-  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling<4, VT>, smem, name);
+  constexpr int F = RISK ? RISK_INST : 0;
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling<2 | F, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling<4 | F, VT>, smem, name);
   if (rc != RB_OK) return rc;
-  const auto k = Z <= 64 ? k_c51_dueling<2, VT> : k_c51_dueling<4, VT>;
+  const auto k = Z <= 64 ? k_c51_dueling<2 | F, VT> : k_c51_dueling<4 | F, VT>;
   { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
     k<<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, support, vmin,
-                                                 vmax, delta_z, gamma_n, B, A, Z, loss, dz, m_out, astar_out, support_q, eps); }
+                                                 vmax, delta_z, gamma_n, B, A, Z, loss, dz, m_out, astar_out, support_q, eps,
+                                                 risk_kind, risk_eta); }
   return check_launch(name);
 }
 }
@@ -3337,6 +3516,16 @@ int rb_c51_dueling_vt_loss_grad(const float* z_online, const float* z_target, in
   return c51_dueling_launch<true>("rb_c51_dueling_vt_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
                                   nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, loss, dz, m_out, astar_out,
                                   support_q, eps, stream);
+}
+
+int rb_c51_dueling_risk_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                  const int64_t* actions, const float* returns, const float* nonterminals,
+                                  const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                  float gamma_n, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                  int risk_kind, float risk_eta, rb_stream_t stream) {
+  return c51_dueling_launch<false, true>("rb_c51_dueling_risk_loss_grad", z_online, z_target, actions_n, atoms, actions,
+                                         returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, loss, dz,
+                                         m_out, astar_out, nullptr, 0.0f, stream, risk_kind, risk_eta);
 }
 
 extern "C++" {
@@ -3393,8 +3582,27 @@ int rb_q_values(const float* z, int M, int actions, int atoms, const float* supp
   if (M <= 0 || actions <= 0 || atoms <= 1) return fail(RB_ERR_INVAL, "rb_q_values: M, actions > 0 and atoms > 1 are required");
   if (atoms > RB_MAX_ATOMS) return fail(RB_ERR_RANGE, "rb_q_values: atoms exceeds RB_MAX_ATOMS");
   { ProfScope prof_(RB_K_Q_VALUES, (cudaStream_t)stream);
-    k_q_select<<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, support, q, best_action, best_q); }
+    k_q_select<false><<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, support, q, best_action, best_q, 0,
+                                                                    0.0f); }
   return check_launch("rb_q_values");
+}
+
+int rb_q_values_risk(const float* z, int M, int actions, int atoms, const float* support, float* q, int64_t* best_action,
+                     float* best_q, int risk_kind, float risk_eta, rb_stream_t stream) {
+  const char* name = "rb_q_values_risk";
+  if (!z || !support) return null_pointer(name);
+  char msg[128];
+  if (!q && !best_action && !best_q) {
+    snprintf(msg, sizeof msg, "%s: no output requested", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  int rc = c51_check(name, true, M, actions, atoms, "actions", "atoms");
+  if (rc == RB_OK) rc = risk_check(name, risk_kind, risk_eta);
+  if (rc != RB_OK) return rc;
+  { ProfScope prof_(RB_K_Q_VALUES, (cudaStream_t)stream);
+    k_q_select<true><<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, support, q, best_action, best_q,
+                                                                   risk_kind, risk_eta); }
+  return check_launch(name);
 }
 
 static int qr_check(const char* name, int B, int A, int N, float kappa) {
@@ -3415,26 +3623,28 @@ static int qr_check(const char* name, int B, int A, int N, float kappa) {
 }
 
 extern "C++" {
-template <bool VT>
+template <bool VT, bool RISK = false>
 static int qr_dueling_launch(const char* name, const float* z_online, const float* z_target, int actions_n, int atoms,
                              const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
                              float kappa, float gamma_n, int B, float* loss, float* dz, float* theta_out, int64_t* astar_out,
-                             float eps, rb_stream_t stream) {
+                             float eps, rb_stream_t stream, int risk_kind = 0, float risk_eta = 0.0f) {
   const int N = atoms, A = actions_n;
   int rc = VT ? vt_check(name, true, eps) : RB_OK;
   if (rc == RB_OK && !(z_online && z_target && actions && returns && nonterminals && weights && loss && dz))
     rc = null_pointer(name);
   if (rc == RB_OK) rc = qr_check(name, B, A, N, kappa);
+  if (rc == RB_OK && RISK) rc = risk_check(name, risk_kind, risk_eta);
   if (rc != RB_OK) return rc;
   const size_t smem = (size_t)(3 * (N + A * N) + 4 * N + A) * sizeof(float);
   rc = smem_check(name, smem, "actions * atoms too large");
-  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<2, VT>, smem, name);
-  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<4, VT>, smem, name);
+  constexpr int F = RISK ? RISK_INST : 0;
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<2 | F, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr_dueling<4 | F, VT>, smem, name);
   if (rc != RB_OK) return rc;
-  const auto k = N <= 64 ? k_qr_dueling<2, VT> : k_qr_dueling<4, VT>;
+  const auto k = N <= 64 ? k_qr_dueling<2 | F, VT> : k_qr_dueling<4 | F, VT>;
   { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
     k<<<B, QR_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, kappa, gamma_n, B,
-                                               A, N, loss, dz, theta_out, astar_out, eps); }
+                                               A, N, loss, dz, theta_out, astar_out, eps, risk_kind, risk_eta); }
   return check_launch(name);
 }
 }
@@ -3452,6 +3662,15 @@ int rb_qr_dueling_vt_loss_grad(const float* z_online, const float* z_target, int
                                rb_stream_t stream) {
   return qr_dueling_launch<true>("rb_qr_dueling_vt_loss_grad", z_online, z_target, actions_n, atoms, actions, returns,
                                  nonterminals, weights, kappa, gamma_n, B, loss, dz, theta_out, astar_out, eps, stream);
+}
+
+int rb_qr_dueling_risk_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                 const int64_t* actions, const float* returns, const float* nonterminals,
+                                 const float* weights, float kappa, float gamma_n, int B, float* loss, float* dz,
+                                 float* theta_out, int64_t* astar_out, int risk_kind, float risk_eta, rb_stream_t stream) {
+  return qr_dueling_launch<false, true>("rb_qr_dueling_risk_loss_grad", z_online, z_target, actions_n, atoms, actions,
+                                        returns, nonterminals, weights, kappa, gamma_n, B, loss, dz, theta_out, astar_out,
+                                        0.0f, stream, risk_kind, risk_eta);
 }
 
 extern "C++" {
@@ -3499,26 +3718,29 @@ int rb_qr_dueling_avg_vt_loss_grad(const float* z_online, const float* z_target,
 }
 
 extern "C++" {
-template <bool VT>
+template <bool VT, bool RISK = false>
 static int qr_launch(const char* name, const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
                      const int64_t* actions, const float* returns, const float* nonterminals, const float* weights, float kappa,
                      float gamma_n, int B, int A, int N, float* loss, float* grad_q_online_s, float* theta_out,
-                     int64_t* astar_out, float eps, rb_stream_t stream) {
+                     int64_t* astar_out, float eps, rb_stream_t stream, int risk_kind = 0, float risk_eta = 0.0f) {
   int rc = VT ? vt_check(name, true, eps) : RB_OK;
   if (rc == RB_OK && !(q_online_s && q_online_ns && q_target_ns && actions && returns && nonterminals && weights && loss &&
                        grad_q_online_s))
     rc = null_pointer(name);
   if (rc == RB_OK) rc = qr_check(name, B, A, N, kappa);
+  if (rc == RB_OK && RISK) rc = risk_check(name, risk_kind, risk_eta);
   if (rc != RB_OK) return rc;
   const size_t smem = (size_t)(4 * N + A) * sizeof(float);
   rc = smem_check(name, smem, "too many actions");
-  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<2, VT>, smem, name);
-  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<4, VT>, smem, name);
+  constexpr int F = RISK ? RISK_INST : 0;
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<2 | F, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_qr<4 | F, VT>, smem, name);
   if (rc != RB_OK) return rc;
-  const auto k = N <= 64 ? k_qr<2, VT> : k_qr<4, VT>;
+  const auto k = N <= 64 ? k_qr<2 | F, VT> : k_qr<4 | F, VT>;
   { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
     k<<<B, QR_T, smem, (cudaStream_t)stream>>>(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights,
-                                               kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, eps); }
+                                               kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, eps,
+                                               risk_kind, risk_eta); }
   return check_launch(name);
 }
 }
@@ -3537,6 +3759,15 @@ int rb_qr_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const 
                        float eps, rb_stream_t stream) {
   return qr_launch<true>("rb_qr_vt_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights,
                          kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, eps, stream);
+}
+
+int rb_qr_risk_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                         const float* returns, const float* nonterminals, const float* weights, float kappa, float gamma_n,
+                         int B, int A, int N, float* loss, float* grad_q_online_s, float* theta_out, int64_t* astar_out,
+                         int risk_kind, float risk_eta, rb_stream_t stream) {
+  return qr_launch<false, true>("rb_qr_risk_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals,
+                                weights, kappa, gamma_n, B, A, N, loss, grad_q_online_s, theta_out, astar_out, 0.0f, stream,
+                                risk_kind, risk_eta);
 }
 
 // The Munchausen entries' own refusals: alpha in [0, 1], tau finite and >= FLT_MIN (a normal fp32), l0 finite and < 0;
@@ -3607,9 +3838,10 @@ int rb_qr_munchausen_loss_grad(const float* q_online_s, const float* q_target_s,
 }
 
 extern "C++" {
-template <bool VT>
+template <bool VT, bool RISK = false>
 static int qr_q_values_launch(const char* name, const float* z, int M, int actions, int atoms, float* q,
-                              int64_t* best_action, float* best_q, float eps, rb_stream_t stream) {
+                              int64_t* best_action, float* best_q, float eps, rb_stream_t stream, int risk_kind = 0,
+                              float risk_eta = 0.0f) {
   int rc = VT ? vt_check(name, true, eps) : RB_OK;
   if (rc != RB_OK) return rc;
   if (!z) return null_pointer(name);
@@ -3626,8 +3858,11 @@ static int qr_q_values_launch(const char* name, const float* z, int M, int actio
     snprintf(msg, sizeof msg, "%s: atoms exceeds RB_MAX_ATOMS", name);
     return fail(RB_ERR_RANGE, msg);
   }
+  rc = RISK ? risk_check(name, risk_kind, risk_eta) : RB_OK;
+  if (rc != RB_OK) return rc;
   { ProfScope prof_(RB_K_Q_VALUES, (cudaStream_t)stream);
-    k_qr_select<VT><<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, q, best_action, best_q, eps); }
+    k_qr_select<VT, RISK><<<(M + 3) / 4, 128, 0, (cudaStream_t)stream>>>(z, M, actions, atoms, q, best_action, best_q, eps,
+                                                                         risk_kind, risk_eta); }
   return check_launch(name);
 }
 }
@@ -3640,6 +3875,12 @@ int rb_qr_q_values(const float* z, int M, int actions, int atoms, float* q, int6
 int rb_qr_vt_q_values(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
                       float eps, rb_stream_t stream) {
   return qr_q_values_launch<true>("rb_qr_vt_q_values", z, M, actions, atoms, q, best_action, best_q, eps, stream);
+}
+
+int rb_qr_q_values_risk(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
+                        int risk_kind, float risk_eta, rb_stream_t stream) {
+  return qr_q_values_launch<false, true>("rb_qr_q_values_risk", z, M, actions, atoms, q, best_action, best_q, 0.0f, stream,
+                                         risk_kind, risk_eta);
 }
 
 static int stats_batch_check(const float* loss, const float* weights, const int64_t* actions, const float* m,
