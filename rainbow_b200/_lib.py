@@ -3,7 +3,9 @@
 The product path has NO CPU fallback: if librainbow_b200.so is missing and cannot be built, or a
 kernel is asked to run on a non-CUDA tensor, this module raises.
 """
+import contextlib
 import ctypes as C
+import gc
 import os
 
 from . import _build
@@ -242,6 +244,24 @@ def side_branch(side, fn):
         done = torch.cuda.Event()
         done.record(side)
     return out, done
+
+
+@contextlib.contextmanager
+def graph_capture(graph):
+    """torch.cuda.graph(graph) with Python's cyclic garbage collector run first and held off until the capture ends.
+    Destroying a CUDA graph while a stream captures invalidates the capture, and torch no longer collects garbage before
+    it captures: a dead reference cycle that holds a graph (a dropped Agent, say) could otherwise be freed by a collection
+    that an allocation inside the capture happens to trigger."""
+    import torch
+    gc.collect()
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(graph):
+            yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 # Every kernel id, indexed by its value in the RB_K_* enum of include/rainbow_b200.h (RB_K_FOO -> "foo"); a host test checks

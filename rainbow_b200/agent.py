@@ -899,7 +899,7 @@ class Agent:
             if g["graph"] is None:
                 torch.cuda.synchronize(self.device)
                 graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
+                with _lib.graph_capture(graph):
                     run()
                 g["graph"] = graph
             g["graph"].replay()
@@ -1396,7 +1396,7 @@ class Agent:
         mem.push_beta()  # outside the capture: a captured fill_ would freeze beta at today's value
         torch.cuda.synchronize(self.device)
         graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
+        with _lib.graph_capture(graph):
             _, loss = self._sample_and_update(mem, ws)
         return graph, ws, loss
 

@@ -47,8 +47,7 @@ def normals(seed, counter, B, copies):
     for j in range(copies):
         w = philox_words(seed, counter, B, INTS_STREAM + j)
         for side, (a, b) in enumerate(((w[:, 0], w[:, 1]), (w[:, 2], w[:, 3]))):
-            u1 = (a.astype(np.float32) + np.float32(1.0)).astype(np.float64) * 2.0 ** -32
-            u2 = b.astype(np.float32).astype(np.float64) * 2.0 ** -32
+            u1, u2 = P.box_muller_uniforms(a, b)
             out[side, j] = np.sqrt(-2.0 * np.log(u1)) * np.cos(2.0 * np.pi * u2)
     return out
 

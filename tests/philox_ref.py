@@ -1,6 +1,7 @@
 """numpy references of the random-shift augmentation (rb_gather_shift): Philox4x32-10 (Salmon et al. 2011, the Random123
 construction the device code implements in rainbow_b200/csrc/rb_internal.cuh), the offsets drawn from it, and the shift
-itself as ReplicationPad2d(pad) followed by an 84 x 84 crop."""
+itself as ReplicationPad2d(pad) followed by an 84 x 84 crop.  Also the two uniforms box_muller forms from a pair of
+Philox words, which the intensity (drq_ref) and noise (noise_ref) references share."""
 import numpy as np
 
 M0, M1 = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57)
@@ -20,6 +21,14 @@ def philox4x32_10(ctr, key):
         c = [hi1 ^ c[1] ^ k0, lo1, hi0 ^ c[3] ^ k1, lo0]
         k0, k1 = (k0 + W0) & _LO, (k1 + W1) & _LO
     return np.stack([x.astype(np.uint32) for x in c], axis=-1)
+
+
+def box_muller_uniforms(a, b):
+    """float64 (u1, u2) of box_muller (rb_internal.cuh) for words a, b: u1 = fl32(fl32(a) + 1) 2^-32 in (0, 1] and
+    u2 = fl32(b) 2^-32 in [0, 1), the device's exact fp32 values (scaling by 2^-32 is exact)."""
+    u1 = (np.asarray(a).astype(np.float32) + np.float32(1.0)).astype(np.float64) * 2.0 ** -32
+    u2 = np.asarray(b).astype(np.float32).astype(np.float64) * 2.0 ** -32
+    return u1, u2
 
 
 def shift_offsets(seed, counter, B, pad):
