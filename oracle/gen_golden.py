@@ -11,6 +11,7 @@ the reference files are never edited or copied.
 
     python oracle/gen_golden.py            # writes tests/golden/*.npz + MANIFEST.json
     python oracle/gen_golden.py ref_pickle_state   # only tests/golden/ref_pickle_state.json
+    python oracle/gen_golden.py replay_history     # only tests/golden/replay_history.npz + its MANIFEST.json key
 
 Versions are recorded in MANIFEST.json (numpy/torch behaviour is the effective
 pin: the reference's requirements.txt pins nothing).
@@ -238,6 +239,72 @@ def gen_replay():
         out[pfx + "iter"] = np.stack([next(it).numpy() for _ in range(12)])
         cases.append(dict(name=name, cap=cap, n=n, B=B, fill=fill, beta=beta, attempts=attempts))
     np.savez_compressed(os.path.join(OUT, "replay.npz"), **out)
+    return cases
+
+
+def history_case_frame(i):
+    """uint8 frame the reference stores for pattern_state(i) (memory.py:106); tests regenerate it with the same two lines."""
+    return pattern_state(i)[-1].mul(255).to(torch.uint8).numpy().reshape(-1)
+
+
+def as_frame_bytes(x, what):
+    """float32 gathered frames -> uint8, asserting that every value is byte / 255 (0 for a blank)."""
+    u8 = np.rint(x * 255).astype(np.uint8)
+    assert np.array_equal(u8.astype(np.float32) / np.float32(255), x), what
+    return u8
+
+
+def gen_replay_history():
+    """ReplayMemory.append / sample / the iterator at histories other than 4, on rings of short episodes (terminal
+    probability 0.3) so that most windows cross an episode boundary.  Gathered frames are stored as their bytes; the ring's
+    frames are history_case_frame(i) of the i-th append and are not stored."""
+    out = {}
+    cases = []
+    for name, H, n, cap, B, fill in (("h1n3", 1, 3, 64, 8, 90), ("h2n1", 2, 1, 64, 8, 90), ("h5n5", 5, 5, 64, 6, 100),
+                                     ("h5n2", 5, 2, 64, 6, 40), ("h8n3", 8, 3, 64, 4, 100),
+                                     ("h16n48", 16, 48, 128, 2, 150)):   # history + n = 64: the longest window
+        rs = np.random.RandomState(23)
+        np.random.seed(29)
+        mem = ref_memory.ReplayMemory(make_args(history_length=H, multi_step=n), cap)
+        for i in range(fill):
+            mem.append(pattern_state(i), int(rs.randint(0, 6)), float(rs.randint(-1, 2)), bool(rs.uniform() < 0.3))
+        ts = mem.transitions.tree_start
+        count = cap if mem.transitions.full else mem.transitions.index
+        mem.update_priorities(np.arange(count) + ts, rs.uniform(0.01, 4, count).astype(np.float32))
+        pfx = name + "_"
+        ring = {}
+        dump_ring(mem, ring, pfx)
+        frames = ring.pop(pfx + "frames")
+        expect = np.zeros_like(frames)
+        for i in range(fill):
+            expect[i % cap] = history_case_frame(i)
+        assert np.array_equal(frames, expect), "ring frames are history_case_frame of each append"
+        out.update(ring)
+        attempts = []
+        for s in range(2):
+            with UniformRecorder() as rec:
+                tidx, states, actions, returns, nstates, nonterm, weights = mem.sample(B)
+            attempts.append(len(rec.calls))
+            out[f"{pfx}s{s}_u01"] = np.stack(rec.calls)
+            out[f"{pfx}s{s}_tidx"] = np.asarray(tidx, np.int64)
+            out[f"{pfx}s{s}_states"] = as_frame_bytes(states.numpy(), "states")
+            out[f"{pfx}s{s}_nstates"] = as_frame_bytes(nstates.numpy(), "next states")
+            out[f"{pfx}s{s}_actions"] = actions.numpy()
+            out[f"{pfx}s{s}_returns"] = returns.numpy()
+            out[f"{pfx}s{s}_nonterm"] = nonterm.numpy()
+            mem.update_priorities(tidx, rs.uniform(0, 2, B).astype(np.float32))
+            out[f"{pfx}s{s}_tree_after"] = mem.transitions.sum_tree.copy()
+        # the iterator (memory.py:162-180) at both ends of the ring and in between, through its own current_idx
+        cur = np.array(sorted({0, 1, H - 1, cap // 2, cap - H + 1, cap - 1} - {cap}), np.int64)
+        it = iter(mem)
+        iters = []
+        for c in cur:
+            it.current_idx = int(c)
+            iters.append(as_frame_bytes(next(it).numpy(), "iterator state"))
+        out[pfx + "iter_cur"] = cur
+        out[pfx + "iter"] = np.stack(iters)
+        cases.append(dict(name=name, history=H, n=n, cap=cap, B=B, fill=fill, attempts=attempts))
+    np.savez_compressed(os.path.join(OUT, "replay_history.npz"), **out)
     return cases
 
 
@@ -599,6 +666,7 @@ def main():
                     torch=torch.__version__, python=sys.version.split()[0])
     manifest["big_trees"] = gen_tree()
     manifest["replay_cases"] = gen_replay()
+    manifest["replay_history_cases"] = gen_replay_history()
     gen_append()
     gen_pow()
     manifest["learn_cases"] = gen_learn()
@@ -615,8 +683,21 @@ def main():
         print(fn, os.path.getsize(os.path.join(OUT, fn)))
 
 
+def main_replay_history():
+    """Only tests/golden/replay_history.npz and its MANIFEST.json key; every other fixture is left as it is."""
+    path = os.path.join(OUT, "MANIFEST.json")
+    with open(path) as f:
+        manifest = json.load(f)
+    manifest["replay_history_cases"] = gen_replay_history()
+    with open(path, "w") as f:
+        json.dump(manifest, f, indent=1)
+    print("replay_history.npz", os.path.getsize(os.path.join(OUT, "replay_history.npz")))
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["ref_pickle_state"]:
         gen_ref_pickle_state()
+    elif sys.argv[1:] == ["replay_history"]:
+        main_replay_history()
     else:
         main()

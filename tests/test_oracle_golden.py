@@ -104,6 +104,56 @@ def test_replay_sample(case):
     assert_bits_equal(it, g[pfx + "iter"], "iterator states")
 
 
+def history_case_frame(i):
+    """The frame the reference stored for its i-th append in replay_history.npz (oracle/gen_golden.py pattern_state)."""
+    import torch
+    pix = torch.arange(84 * 84, dtype=torch.int64)
+    f = (((pix * (2 * (i % 5) + 1) + 13 * i) % 256).to(torch.float32) / 255).reshape(84, 84)
+    if i % 3 == 0:
+        f += 0.0009
+        f.clamp_(0, 1)
+    return f.mul(255).to(torch.uint8).numpy().reshape(-1)
+
+
+@pytest.mark.parametrize("case", manifest()["replay_history_cases"], ids=lambda c: c["name"])
+def test_replay_history(case):
+    """The oracle's sampling, gather and iterator at histories 1, 2, 5, 8 and 16 (window 64) on rings of short episodes,
+    against the reference: indices, states, next states, actions and nonterminals bitwise."""
+    g = golden("replay_history")
+    pfx = case["name"] + "_"
+    H, n, B, cap, fill = case["history"], case["n"], case["B"], case["cap"], case["fill"]
+    meta = g[pfx + "meta"]
+    t = oracle.OracleTree(cap)
+    for i in range(fill):
+        t.frames[i % cap] = history_case_frame(i)
+    t.sum_tree[:] = g[pfx + "sum_tree"]
+    t.timestep[:], t.action[:], t.reward[:] = g[pfx + "timestep"], g[pfx + "action"], g[pfx + "reward"]
+    t.nonterminal[:] = g[pfx + "nonterminal"]
+    t.index, t.full = int(meta[0]), bool(meta[1])
+    gamma = np.array([0.99 ** i for i in range(n)], np.float32)
+    crossed = 0
+    for s in range(2):
+        u = g[f"{pfx}s{s}_u01"]
+        assert u.shape[0] == case["attempts"][s]
+        for a in range(u.shape[0]):
+            probs, didx, tidx = t.find(oracle.segment_samples(t.total(), B, u[a]))
+            assert oracle.batch_valid(didx, probs, t.index, cap, n, H) == (a == u.shape[0] - 1)
+        assert_bits_equal(tidx, g[f"{pfx}s{s}_tidx"], "tree idx")
+        states, actions, returns, nstates, nonterm = oracle.gather(t, didx, H, n, gamma)
+        assert_bits_equal(states, g[f"{pfx}s{s}_states"].astype(np.float32) / np.float32(255), "states")
+        assert_bits_equal(nstates, g[f"{pfx}s{s}_nstates"].astype(np.float32) / np.float32(255), "next states")
+        assert_bits_equal(actions, g[f"{pfx}s{s}_actions"], "actions")
+        assert_bits_equal(nonterm, g[f"{pfx}s{s}_nonterm"], "nonterminals")
+        np.testing.assert_allclose(returns, g[f"{pfx}s{s}_returns"], rtol=0, atol=1e-6)   # BLAS dot order
+        # windows that reach into another episode (a first record past slot 0)
+        window = (didx[:, None] - (H - 1) + np.arange(H + n)) % cap
+        crossed += int((t.timestep[window][:, 1:] == 0).any(axis=1).sum())
+        t.sum_tree[:] = g[f"{pfx}s{s}_tree_after"]   # the priorities the reference wrote back before its next sample
+    assert crossed >= B, "at least half the sampled windows cross an episode boundary"
+    it = np.stack([oracle.iter_state(t, int(c), H) for c in g[pfx + "iter_cur"]])
+    assert_bits_equal(it, g[pfx + "iter"].astype(np.float32) / np.float32(255), "iterator states")
+
+
 def test_append_sequence():
     g = golden("append")
     t = oracle.OracleTree(8)
