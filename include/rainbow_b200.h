@@ -58,6 +58,7 @@ extern "C" {
 #define RB_MAX_NOISY_LAYERS 8
 #define RB_MAX_PEERS 8           /* ranks of one NVLink domain handled by rb_peer_clip_adam */
 #define RB_APPEND_BATCH 8        /* transitions per rb_append_batch launch */
+#define RB_NONTERMINAL_FINAL 2   /* nonterminal byte of a final-observation record (rb_append_batch_trunc) */
 #define RB_MAX_SHIFT_PAD 16      /* largest pad of rb_gather_shift */
 #define RB_MAX_AUG_COPIES 8      /* most copies of a state (M) or next state (K) in rb_gather_aug */
 #define RB_MAX_RESET_SEGMENTS 32 /* most parameter tensors one rb_param_reset call covers */
@@ -207,6 +208,21 @@ int rb_gather_horizon(const uint8_t* frames, const int32_t* timestep, const int3
                       float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
                       const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream);
 
+/* Bootstrapping through time-limit truncations (no reference counterpart).  rb_gather_horizon's arguments, checks,
+ * kernel choice, layouts and draws, and the same outputs for every sample whose records idx + 1 .. idx + n_t - 1 hold no
+ * final-observation record (nonterminal byte RB_NONTERMINAL_FINAL, written by rb_append_batch_trunc).  A sample whose
+ * first such record is idx + k, k < n_t, is cut there: every output is bitwise what rb_gather_horizon writes for it with a
+ * row of n = k, gamma_pow[0 .. k - 1] of *current and gamma_n = current->gamma_pow[k] -- the return of k steps, the next
+ * state stacked back from the final observation, and the nonterminal fl32(nonterminal * gamma^k) for a loss launched with
+ * gamma_n = 1.  A fixed horizon passes a constant row (n, fl32(gamma ** n), fl32(gamma ** k)).  The rows built by
+ * rainbow_b200.horizon hold fl32(gamma ** k) at every k < n, which is the gamma_n of a horizon of k steps.  Refusals as
+ * rb_gather_horizon's, named rb_gather_trunc. */
+int rb_gather_trunc(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                    const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n_max,
+                    const rb_horizon* current, float* states, float* next_states, int64_t* actions, float* returns,
+                    float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
+                    const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream);
+
 /* memory.py:166-178 ReplayMemory.__next__, batched: states for current_idx = first .. first+count-1,
  * backward-only blanking, negative indices wrap.  out is float32[count][history][84*84]. */
 int rb_iter_states(const uint8_t* frames, const int32_t* timestep, int64_t size, int64_t first, int count,
@@ -230,6 +246,17 @@ int rb_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* fram
                     float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max,
                     const float* const* last_frames, const int32_t* actions, const float* rewards, const int32_t* terminals,
                     int k, rb_stream_t stream);
+
+/* rb_append_batch that can also store final-observation records: terminals[j] == RB_NONTERMINAL_FINAL stores record j with
+ * action 0 and reward 0 (actions[j] and rewards[j] are not read), the timestep that continues its episode, nonterminal
+ * byte RB_NONTERMINAL_FINAL and leaf 0 -- never sampled, and the running max unchanged -- and the next record starts an
+ * episode (timestep 0), as after a terminal.  Other terminals[j] as in rb_append_batch, with the same result.  A time
+ * limit's last step is the pair (s_T-1, a, r, 0), (final observation, -, -, RB_NONTERMINAL_FINAL).  Refusals as
+ * rb_append_batch's, named rb_append_batch_trunc. */
+int rb_append_batch_trunc(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep,
+                          int32_t* action, float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max,
+                          const float* const* last_frames, const int32_t* actions, const float* rewards,
+                          const int32_t* terminals, int k, rb_stream_t stream);
 
 /* agent.py:66-96 Agent.learn minus the three network bodies, given PRE-softmax logits [B,A,Z]
  * (model.py:75 `q`; the softmax / log_softmax of model.py:76-79 are folded in):

@@ -90,9 +90,13 @@ SIGNATURES = {
     "rb_horizon_advance": (C.c_int, [_vp, _i32, _vp, _vp, _vp]),
     "rb_gather_horizon": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                     _i32, _f32, _i32, _i32, _u64, _vp, _vp, _vp, _vp]),
+    "rb_gather_trunc": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                  _i32, _f32, _i32, _i32, _u64, _vp, _vp, _vp, _vp]),
     "rb_iter_states": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _i32, _vp, _vp]),
     "rb_append": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int32, _f32, _i32, _vp]),
     "rb_append_batch": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "rb_append_batch_trunc": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32,
+                                        _vp]),
     "rb_c51_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i32, _i32, _i32,
                                    _vp, _vp, _vp, _vp, _vp]),
     "rb_noisy_resample": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp, _u64, _vp, _vp]),

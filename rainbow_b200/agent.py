@@ -10,7 +10,10 @@ One `learn(mem)` (agent.py:61-100) is:
                                                args.augment_intensity > 0 or augment_m / augment_k > 1: rb_gather_aug --
                                                shift + intensity augmentation of M copies of s and K copies of s';
                                                args.anneal_steps > 0: rb_gather_horizon, any of the three with the
-                                               annealed n and gamma, nonterminals as gamma^n or 0 and K3 with gamma_n = 1]
+                                               annealed n and gamma, nonterminals as gamma^n or 0 and K3 with gamma_n = 1;
+                                               args.bootstrap_truncation: rb_gather_trunc, any of these with each
+                                               sample's window cut at a final observation k <= n steps on, nonterminals
+                                               as gamma^k or 0 and K3 with gamma_n = 1]
     3 x conv body (torch: cuDNN)              (agent.py:66,71,75 -> model.py:70-71)
     K6 rb_noisy_resample (target net)         (agent.py:74)
     fused noisy dueling heads (rb_head_forward) on the conv features -- online net on [s; s'], target on s'
@@ -725,6 +728,9 @@ class Agent:
         self._horizon = HorizonSchedule.from_args(args, self.device)
         if self._horizon is not None and self._horizon.n_max + self.history > 64:
             raise ValueError("history_length + max(multi_step, multi_step_start) must not exceed 64")
+        # bootstrapping through time limits (opt-in): the replay (built with the same switch) cuts a sample's window at a
+        # final observation, k <= n steps on, and writes its nonterminal in discount form, so the losses take gamma_n = 1
+        self.bootstrap_truncation = bool(getattr(args, "bootstrap_truncation", False))
 
         self.online_net = DQN(args, self.action_space).to(device=self.device)
         model_path = getattr(args, "model", None)
@@ -1226,8 +1232,9 @@ class Agent:
     def _gamma_n(self):
         """The gamma_n the loss kernels take: gamma ** n, or 1 with an annealed horizon, whose gather writes the nonterminals
         as fl32(nonterminal * gamma_u ** n_u) -- the kernels use a nonterminal only in fl32(nonterminal * gamma_n), so
-        the products, and everything after them, are bitwise those of the fixed horizon (n_u, gamma_u)."""
-        return 1.0 if self._horizon is not None else self.discount ** self.n
+        the products, and everything after them, are bitwise those of the fixed horizon (n_u, gamma_u).  Likewise 1 with
+        bootstrap_truncation, whose gather writes fl32(nonterminal * gamma ** k) for a sample cut k steps on."""
+        return 1.0 if self._horizon is not None or self.bootstrap_truncation else self.discount ** self.n
 
     def horizon(self):
         """(n, gamma) the next update trains with: the annealed schedule's current step, or (multi_step, discount)."""
@@ -1421,6 +1428,10 @@ class Agent:
             raise _lib.RainbowB200Error(
                 f"args.anneal_steps needs a rainbow_b200 ReplayMemory built for n >= {self._horizon.n_max} (it reads "
                 "args.multi_step_start): the annealed horizon is gathered on the device")
+        if self.bootstrap_truncation != bool(getattr(mem, "bootstrap_truncation", False)):
+            raise _lib.RainbowB200Error(
+                f"args.bootstrap_truncation is {self.bootstrap_truncation} for the agent and not for its replay: both must "
+                "be built with the same switch (with it the replay writes nonterminals in discount form)")
         if self.augment_copies != (1, 1) and not self._fused_path(self.batch_size):
             raise self._copies_error(self.augment_copies)   # before sampling: a refused learn() leaves the replay as it was
         # the captured graph bakes in: this memory's buffers, the batch size and training-mode (noisy) weights

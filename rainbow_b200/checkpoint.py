@@ -383,6 +383,8 @@ def _meta(agent, mem):
         hyper["munchausen_alpha"], hyper["munchausen_temperature"], hyper["munchausen_clip"] = agent.munchausen
     if agent.risk is not None:   # absent: the mean selects (no risk measure)
         hyper["risk_measure"], hyper["risk_eta"] = agent.risk
+    if agent.bootstrap_truncation:   # absent: off
+        hyper["bootstrap_truncation"] = True
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
         learner["redo_count"] = agent.redo_count
     if opt.grouped:   # the group optimiser's bias-correction counts, [encoder, head]
@@ -404,6 +406,9 @@ def _meta(agent, mem):
         tr = mem.transitions
         replay = {k: getattr(mem, k) for k in PERSISTENT_HOST}
         replay.update(index=tr.index, full=tr.full)
+        if mem.bootstrap_truncation:   # absent: off, and then the ring holds no final-observation record
+            replay["bootstrap_truncation"] = True
+            replay["final_records"] = mem.holds_final_records()
         meta["replay"] = replay
     return meta
 
@@ -542,6 +547,10 @@ def _validate(agent, mem, man):
     live = agent.risk or (None, None)
     if risk != live:
         raise _Error(f"risk measure (measure, eta) differs: checkpoint {risk}, live {live}")
+    # a ring with final-observation records means nothing to a replay that gathers without cutting windows at them
+    if mem is not None and (man.get("replay") or {}).get("final_records") and not mem.bootstrap_truncation:
+        raise _Error("the checkpoint's replay holds final-observation records (args.bootstrap_truncation) and this "
+                     "replay was built without args.bootstrap_truncation")
     layout = agent.optimiser.state_dict(clone=False)["layout"]
     if man.get("optimiser") != layout:
         raise _Error(f"optimiser layout differs: checkpoint {man.get('optimiser')}, this learner {layout}")

@@ -475,14 +475,33 @@ struct GatherSlot {
   }
 };
 
-template <bool HZ>
+// TRUNC (rb_gather_trunc): k = the offset of the first final-observation record (nonterminal byte RB_NONTERMINAL_FINAL) in
+// records idx + 1 .. idx + n - 1, or n if there is none, from a 64-bit ballot like window_first_bits'.  Every warp forms it
+// itself, so the CTA needs no barrier before it maps its slot.
+__device__ __forceinline__ int first_final(const uint8_t* __restrict__ nonterminal, int64_t size, int64_t idx, int n) {
+  const int lane = threadIdx.x & 31;
+  bool f0 = false, f1 = false;
+  if (lane < n - 1) f0 = __ldg(nonterminal + pymod(idx + 1 + lane, size)) == RB_NONTERMINAL_FINAL;
+  if (lane + 32 < n - 1) f1 = __ldg(nonterminal + pymod(idx + 33 + lane, size)) == RB_NONTERMINAL_FINAL;
+  const uint64_t m = (uint64_t)__ballot_sync(0xffffffffu, f0) | ((uint64_t)__ballot_sync(0xffffffffu, f1) << 32);
+  return m ? __ffsll((long long)m) : n;   // bit j is record idx + 1 + j, so the first set bit's 1-based position is k
+}
+
+// TRUNC: the window is then gathered exactly as at n = k, with the nonterminal in discount form at gamma_k, which is the
+// row's gamma_pow[k] for k < n (fl32(gamma ** k), the gamma_n of a horizon of k steps) and its gamma_n for k = n.
+template <bool HZ, bool TRUNC = false>
 __device__ __forceinline__ bool gather_slot(GatherSlot& g, int64_t size, const int64_t* __restrict__ data_idx, int history,
                                             int n, const float* __restrict__ gamma_pow, int split,
-                                            const rb_horizon* __restrict__ hz) {
+                                            const rb_horizon* __restrict__ hz,
+                                            const uint8_t* __restrict__ nonterminal = nullptr) {
   g.b = blockIdx.y;
   g.W = history + n;
   g.n = n; g.gamma_pow = gamma_pow; g.gamma_n = 1.0f;
   if constexpr (HZ) { g.n = min(max(__ldg(&hz->n), 1), n); g.gamma_pow = hz->gamma_pow; g.gamma_n = __ldg(&hz->gamma_n); }
+  if constexpr (TRUNC) {
+    const int k = first_final(nonterminal, size, data_idx[g.b], g.n);
+    if (k < g.n) { g.gamma_n = __ldg(g.gamma_pow + k); g.n = k; }
+  }
   const int used = blockIdx.x / split;
   g.part = blockIdx.x % split;
   if (HZ && used >= history + min(g.n, history)) return false;
@@ -532,7 +551,7 @@ __device__ __forceinline__ void gather_scalars(const GatherSlot& g, uint64_t fir
   else nonterminals[g.b] = nt;
 }
 
-template <bool HZ>
+template <bool HZ, bool TRUNC = false>
 __device__ __forceinline__ void
 gather_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
             const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
@@ -541,7 +560,7 @@ gather_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ time
             float* __restrict__ returns, float* __restrict__ nonterminals, int split, const rb_horizon* __restrict__ hz) {
   __shared__ uint64_t s_first;
   GatherSlot g;
-  if (!gather_slot<HZ>(g, size, data_idx, history, n, gamma_pow, split, hz)) return;
+  if (!gather_slot<HZ, TRUNC>(g, size, data_idx, history, n, gamma_pow, split, hz, nonterminal)) return;
   const int per = (FRAME_VEC + split - 1) / split;
   const int v0 = g.part * per, v1 = min(FRAME_VEC, v0 + per);
   const uint4 pre = gather_prefetch(g, frames, timestep, size, history, v0, v1, s_first);
@@ -583,6 +602,17 @@ k_gather_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ time
             float* __restrict__ returns, float* __restrict__ nonterminals, int split) {
   gather_body<true>(frames, timestep, action, reward, nonterminal, size, data_idx, history, n_max, nullptr, states,
                     next_states, actions, returns, nonterminals, split, hz);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_hz_trunc(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep,
+                  const int32_t* __restrict__ action, const float* __restrict__ reward,
+                  const uint8_t* __restrict__ nonterminal, int64_t size, const int64_t* __restrict__ data_idx, int B,
+                  int history, int n_max, const rb_horizon* __restrict__ hz, float* __restrict__ states,
+                  float* __restrict__ next_states, int64_t* __restrict__ actions, float* __restrict__ returns,
+                  float* __restrict__ nonterminals, int split) {
+  gather_body<true, true>(frames, timestep, action, reward, nonterminal, size, data_idx, history, n_max, nullptr, states,
+                          next_states, actions, returns, nonterminals, split, hz);
 }
 
 // ================================================================================================
@@ -646,7 +676,7 @@ __device__ __forceinline__ float intensity_mult(float s, float normal) {
 // SHIFT (k_gather_shift*): one copy of each side and no intensity, fixed at compile time; `scales` is neither read nor
 // written.  Copy 0 draws from SHIFT_STREAM + 0 and [2][1][B][2] is the [2][B][2] offsets layout, so the draws and
 // `shifts` are those documented for k_gather_shift above.
-template <bool HZ, bool SHIFT>
+template <bool HZ, bool SHIFT, bool TRUNC = false>
 __device__ __forceinline__ void
 gather_aug_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep, const int32_t* __restrict__ action,
                 const float* __restrict__ reward, const uint8_t* __restrict__ nonterminal, int64_t size,
@@ -661,7 +691,7 @@ gather_aug_body(const uint8_t* __restrict__ frames, const int32_t* __restrict__ 
   __shared__ float s_mult[2][MAX_COPIES];
   __shared__ __align__(16) uint8_t s_frame[RB_FRAME_BYTES];
   GatherSlot g;
-  if (!gather_slot<HZ>(g, size, data_idx, history, n, gamma_pow, split, hz)) return;
+  if (!gather_slot<HZ, TRUNC>(g, size, data_idx, history, n, gamma_pow, split, hz, nonterminal)) return;
   const int b = g.b, s = g.s;
   const int copies = SHIFT ? 1 : max(m_copies, k_copies);
   const bool scaled = !SHIFT && intensity > 0.0f;
@@ -777,6 +807,33 @@ k_gather_aug_hz(const uint8_t* __restrict__ frames, const int32_t* __restrict__ 
                                k_copies, seed, rng_counter, shifts, scales, hz);
 }
 
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_shift_hz_trunc(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep,
+                        const int32_t* __restrict__ action, const float* __restrict__ reward,
+                        const uint8_t* __restrict__ nonterminal, int64_t size, const int64_t* __restrict__ data_idx, int B,
+                        int history, int n_max, const rb_horizon* __restrict__ hz, float* __restrict__ states,
+                        float* __restrict__ next_states, int64_t* __restrict__ actions, float* __restrict__ returns,
+                        float* __restrict__ nonterminals, int split, int pad, uint64_t seed,
+                        const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts) {
+  gather_aug_body<true, true, true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max,
+                                    nullptr, states, next_states, actions, returns, nonterminals, split, pad, 0.0f, 1, 1,
+                                    seed, rng_counter, shifts, nullptr, hz);
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+k_gather_aug_hz_trunc(const uint8_t* __restrict__ frames, const int32_t* __restrict__ timestep,
+                      const int32_t* __restrict__ action, const float* __restrict__ reward,
+                      const uint8_t* __restrict__ nonterminal, int64_t size, const int64_t* __restrict__ data_idx, int B,
+                      int history, int n_max, const rb_horizon* __restrict__ hz, float* __restrict__ states,
+                      float* __restrict__ next_states, int64_t* __restrict__ actions, float* __restrict__ returns,
+                      float* __restrict__ nonterminals, int split, int pad, float intensity, int m_copies, int k_copies,
+                      uint64_t seed, const unsigned long long* __restrict__ rng_counter, int32_t* __restrict__ shifts,
+                      float* __restrict__ scales) {
+  gather_aug_body<true, false, true>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max,
+                                     nullptr, states, next_states, actions, returns, nonterminals, split, pad, intensity,
+                                     m_copies, k_copies, seed, rng_counter, shifts, scales, hz);
+}
+
 // One thread: current <- table[min(*counter, T)] (a negative counter reads row 0), then ++*counter.  The first node of an
 // update that anneals its horizon; it runs beside rb_tree_sample, and the gather waits for it.
 __global__ void __launch_bounds__(1)
@@ -836,10 +893,13 @@ struct AppendBatch {
   int k;
 };
 
-__global__ void __launch_bounds__(APPEND_THREADS)
-k_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* __restrict__ frames, int32_t* timestep,
-               int32_t* action, float* reward, uint8_t* nonterminal, int64_t* ring_state, const float* running_max,
-               const __grid_constant__ AppendBatch ab) {
+// FINAL (rb_append_batch_trunc): terminal[j] == RB_NONTERMINAL_FINAL stores a final-observation record -- nonterminal byte
+// RB_NONTERMINAL_FINAL, leaf 0 -- and, like a terminal, makes the next record start an episode.
+template <bool FINAL>
+__device__ __forceinline__ void
+append_batch_body(float* tree, int64_t tree_start, int64_t size, uint8_t* __restrict__ frames, int32_t* timestep,
+                  int32_t* action, float* reward, uint8_t* nonterminal, int64_t* ring_state, const float* running_max,
+                  const AppendBatch& ab) {
   // grid = k CTAs: CTA j quantises frame j (all of a thread's 16-byte loads in flight at once -- the frames may sit in
   // pinned host memory, where every dependent load is a PCIe round trip); warp 0 of CTA 0 also writes the k records and
   // walks the tree.  ring_state is read by every CTA when it starts and advanced by the LAST CTA to finish (ticket in
@@ -888,7 +948,12 @@ k_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* __restric
       timestep[slot] = (int32_t)t;
       action[slot] = ab.action[lane];
       reward[slot] = ab.reward[lane];
-      nonterminal[slot] = ab.terminal[lane] ? 0 : 1;
+      if (FINAL && ab.terminal[lane] == RB_NONTERMINAL_FINAL) {
+        nonterminal[slot] = RB_NONTERMINAL_FINAL;
+        val = 0.0f;
+      } else {
+        nonterminal[slot] = ab.terminal[lane] ? 0 : 1;
+      }
     }
     float sib[32];
 #pragma unroll
@@ -936,6 +1001,22 @@ k_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* __restric
       ring_state[3] = ring_state[3] + k;
     }
   }
+}
+
+__global__ void __launch_bounds__(APPEND_THREADS)
+k_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* __restrict__ frames, int32_t* timestep,
+               int32_t* action, float* reward, uint8_t* nonterminal, int64_t* ring_state, const float* running_max,
+               const __grid_constant__ AppendBatch ab) {
+  append_batch_body<false>(tree, tree_start, size, frames, timestep, action, reward, nonterminal, ring_state, running_max,
+                           ab);
+}
+
+__global__ void __launch_bounds__(APPEND_THREADS)
+k_append_batch_final(float* tree, int64_t tree_start, int64_t size, uint8_t* __restrict__ frames, int32_t* timestep,
+                     int32_t* action, float* reward, uint8_t* nonterminal, int64_t* ring_state, const float* running_max,
+                     const __grid_constant__ AppendBatch ab) {
+  append_batch_body<true>(tree, tree_start, size, frames, timestep, action, reward, nonterminal, ring_state, running_max,
+                          ab);
 }
 
 // ================================================================================================
@@ -2987,10 +3068,15 @@ k_redo_recycle(float* __restrict__ param, float* __restrict__ exp_avg, float* __
 // The launch of rb_append and rb_append_batch, after each has checked its own arguments.
 int append_launch(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
                   float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max, const AppendBatch& ab,
-                  rb_stream_t stream, const char* who) {
+                  rb_stream_t stream, const char* who, bool final_records = false) {
   { ProfScope prof_(RB_K_APPEND, (cudaStream_t)stream);
-    k_append_batch<<<ab.k, APPEND_THREADS, 0, (cudaStream_t)stream>>>(tree, tree_start, size, frames, timestep, action,
-                                                                      reward, nonterminal, ring_state, running_max, ab); }
+    if (final_records)
+      k_append_batch_final<<<ab.k, APPEND_THREADS, 0, (cudaStream_t)stream>>>(tree, tree_start, size, frames, timestep,
+                                                                              action, reward, nonterminal, ring_state,
+                                                                              running_max, ab);
+    else
+      k_append_batch<<<ab.k, APPEND_THREADS, 0, (cudaStream_t)stream>>>(tree, tree_start, size, frames, timestep, action,
+                                                                        reward, nonterminal, ring_state, running_max, ab); }
   return check_launch(who);
 }
 
@@ -3191,22 +3277,27 @@ int rb_horizon_advance(const rb_horizon* table, int T, int64_t* counter, rb_hori
   return check_launch("rb_horizon_advance");
 }
 
-int rb_gather_horizon(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
-                      const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n_max,
-                      const rb_horizon* current, float* states, float* next_states, int64_t* actions, float* returns,
-                      float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
-                      const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream) {
-  if (!current) return fail(RB_ERR_INVAL, "rb_gather_horizon: null pointer");
-  const int rc = gather_check("rb_gather_horizon", frames, timestep, action, reward, nonterminal, size, data_idx, B, history,
-                              n_max, reinterpret_cast<const float*>(current), states, next_states, actions, returns,
-                              nonterminals);
+}  // extern "C"
+
+// rb_gather_horizon (TRUNC false) and rb_gather_trunc (TRUNC true): the same checks, grid and kernel choice
+template <bool TRUNC>
+static int horizon_launch(const char* who, const uint8_t* frames, const int32_t* timestep, const int32_t* action,
+                          const float* reward, const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B,
+                          int history, int n_max, const rb_horizon* current, float* states, float* next_states,
+                          int64_t* actions, float* returns, float* nonterminals, int pad, float intensity, int m_copies,
+                          int k_copies, uint64_t seed, const uint64_t* rng_counter, int32_t* shifts, float* scales,
+                          rb_stream_t stream) {
+  char what[96];
+  snprintf(what, sizeof what, "%s: null pointer", who);
+  if (!current) return fail(RB_ERR_INVAL, what);
+  const int rc = gather_check(who, frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max,
+                              reinterpret_cast<const float*>(current), states, next_states, actions, returns, nonterminals);
   if (rc != RB_OK) return rc;
-  const int arc = aug_check("rb_gather_horizon", pad, 0, intensity, m_copies, k_copies);
+  const int arc = aug_check(who, pad, 0, intensity, m_copies, k_copies);
   if (arc != RB_OK) return arc;
   const bool plain = pad == 0 && intensity == 0.0f && m_copies == 1 && k_copies == 1;
   const bool shift = !plain && intensity == 0.0f && m_copies == 1 && k_copies == 1;
-  if (!plain && (!rng_counter || !shifts || (!shift && !scales)))
-    return fail(RB_ERR_INVAL, "rb_gather_horizon: null pointer");
+  if (!plain && (!rng_counter || !shifts || (!shift && !scales))) return fail(RB_ERR_INVAL, what);
   int split;
   const dim3 grid = gather_grid(history, n_max, B, &split);
   const unsigned long long* ctr = (const unsigned long long*)rng_counter;
@@ -3214,19 +3305,40 @@ int rb_gather_horizon(const uint8_t* frames, const int32_t* timestep, const int3
   // profiled under the id of the gather this launch stands for
   { ProfScope prof_(plain ? RB_K_GATHER : shift ? RB_K_GATHER_SHIFT : RB_K_GATHER_AUG, s);
     if (plain)
-      k_gather_hz<<<grid, GATHER_THREADS, 0, s>>>(frames, timestep, action, reward, nonterminal, size, data_idx, B, history,
-                                                  n_max, current, states, next_states, actions, returns, nonterminals,
-                                                  split);
+      (TRUNC ? k_gather_hz_trunc : k_gather_hz)<<<grid, GATHER_THREADS, 0, s>>>(
+        frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, current, states, next_states,
+        actions, returns, nonterminals, split);
     else if (shift)
-      k_gather_shift_hz<<<grid, GATHER_THREADS, 0, s>>>(frames, timestep, action, reward, nonterminal, size, data_idx, B,
-                                                        history, n_max, current, states, next_states, actions, returns,
-                                                        nonterminals, split, pad, seed, ctr, shifts);
+      (TRUNC ? k_gather_shift_hz_trunc : k_gather_shift_hz)<<<grid, GATHER_THREADS, 0, s>>>(
+        frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, current, states, next_states,
+        actions, returns, nonterminals, split, pad, seed, ctr, shifts);
     else
-      k_gather_aug_hz<<<grid, GATHER_THREADS, 0, s>>>(frames, timestep, action, reward, nonterminal, size, data_idx, B,
-                                                      history, n_max, current, states, next_states, actions, returns,
-                                                      nonterminals, split, pad, intensity, m_copies, k_copies, seed, ctr,
-                                                      shifts, scales); }
-  return check_launch("rb_gather_horizon");
+      (TRUNC ? k_gather_aug_hz_trunc : k_gather_aug_hz)<<<grid, GATHER_THREADS, 0, s>>>(
+        frames, timestep, action, reward, nonterminal, size, data_idx, B, history, n_max, current, states, next_states,
+        actions, returns, nonterminals, split, pad, intensity, m_copies, k_copies, seed, ctr, shifts, scales); }
+  return check_launch(who);
+}
+
+extern "C" {
+
+int rb_gather_horizon(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                      const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n_max,
+                      const rb_horizon* current, float* states, float* next_states, int64_t* actions, float* returns,
+                      float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
+                      const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream) {
+  return horizon_launch<false>("rb_gather_horizon", frames, timestep, action, reward, nonterminal, size, data_idx, B,
+                               history, n_max, current, states, next_states, actions, returns, nonterminals, pad,
+                               intensity, m_copies, k_copies, seed, rng_counter, shifts, scales, stream);
+}
+
+int rb_gather_trunc(const uint8_t* frames, const int32_t* timestep, const int32_t* action, const float* reward,
+                    const uint8_t* nonterminal, int64_t size, const int64_t* data_idx, int B, int history, int n_max,
+                    const rb_horizon* current, float* states, float* next_states, int64_t* actions, float* returns,
+                    float* nonterminals, int pad, float intensity, int m_copies, int k_copies, uint64_t seed,
+                    const uint64_t* rng_counter, int32_t* shifts, float* scales, rb_stream_t stream) {
+  return horizon_launch<true>("rb_gather_trunc", frames, timestep, action, reward, nonterminal, size, data_idx, B,
+                              history, n_max, current, states, next_states, actions, returns, nonterminals, pad,
+                              intensity, m_copies, k_copies, seed, rng_counter, shifts, scales, stream);
 }
 
 int rb_iter_states(const uint8_t* frames, const int32_t* timestep, int64_t size, int64_t first, int count, int history,
@@ -3260,28 +3372,66 @@ int rb_append(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, in
                        stream, "rb_append");
 }
 
-int rb_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
-                    float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max,
-                    const float* const* last_frames, const int32_t* actions, const float* rewards, const int32_t* terminals,
-                    int k, rb_stream_t stream) {
+}  // extern "C"
+
+// rb_append_batch (final_records false) and rb_append_batch_trunc (true)
+static int append_batch_launch(const char* who, bool final_records, float* tree, int64_t tree_start, int64_t size,
+                               uint8_t* frames, int32_t* timestep, int32_t* action, float* reward, uint8_t* nonterminal,
+                               int64_t* ring_state, float* running_max, const float* const* last_frames,
+                               const int32_t* actions, const float* rewards, const int32_t* terminals, int k,
+                               rb_stream_t stream) {
+  char what[112];
   if (!tree || !frames || !timestep || !action || !reward || !nonterminal || !ring_state || !running_max || !last_frames ||
-      !actions || !rewards || !terminals)
-    return fail(RB_ERR_INVAL, "rb_append_batch: null pointer");
-  if (size <= 0 || (size & 1)) return fail(RB_ERR_INVAL, "rb_append_batch: an even size is required");
-  if (k <= 0 || k > RB_APPEND_BATCH || k > size) return fail(RB_ERR_RANGE, "rb_append_batch: 1 <= k <= RB_APPEND_BATCH (and k <= size)");
-  if (tree_depth(tree_start) > 30) return fail(RB_ERR_RANGE, "rb_append_batch: tree deeper than 30 levels");
+      !actions || !rewards || !terminals) {
+    snprintf(what, sizeof what, "%s: null pointer", who);
+    return fail(RB_ERR_INVAL, what);
+  }
+  if (size <= 0 || (size & 1)) {
+    snprintf(what, sizeof what, "%s: an even size is required", who);
+    return fail(RB_ERR_INVAL, what);
+  }
+  if (k <= 0 || k > RB_APPEND_BATCH || k > size) {
+    snprintf(what, sizeof what, "%s: 1 <= k <= RB_APPEND_BATCH (and k <= size)", who);
+    return fail(RB_ERR_RANGE, what);
+  }
+  if (tree_depth(tree_start) > 30) {
+    snprintf(what, sizeof what, "%s: tree deeper than 30 levels", who);
+    return fail(RB_ERR_RANGE, what);
+  }
   AppendBatch ab;
   memset(&ab, 0, sizeof(ab));
   ab.k = k;
   for (int j = 0; j < k; ++j) {
-    if (!last_frames[j] || ((uintptr_t)last_frames[j] & 15)) return fail(RB_ERR_INVAL, "rb_append_batch: frames must be non-null and 16-byte aligned");
+    if (!last_frames[j] || ((uintptr_t)last_frames[j] & 15)) {
+      snprintf(what, sizeof what, "%s: frames must be non-null and 16-byte aligned", who);
+      return fail(RB_ERR_INVAL, what);
+    }
+    const bool final_record = final_records && terminals[j] == RB_NONTERMINAL_FINAL;
     ab.frame[j] = last_frames[j];
-    ab.action[j] = actions[j];
-    ab.reward[j] = rewards[j];
-    ab.terminal[j] = terminals[j] ? 1 : 0;
+    ab.action[j] = final_record ? 0 : actions[j];
+    ab.reward[j] = final_record ? 0.0f : rewards[j];
+    ab.terminal[j] = final_record ? RB_NONTERMINAL_FINAL : terminals[j] ? 1 : 0;
   }
   return append_launch(tree, tree_start, size, frames, timestep, action, reward, nonterminal, ring_state, running_max, ab,
-                       stream, "rb_append_batch");
+                       stream, who, final_records);
+}
+
+extern "C" {
+
+int rb_append_batch(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
+                    float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max,
+                    const float* const* last_frames, const int32_t* actions, const float* rewards, const int32_t* terminals,
+                    int k, rb_stream_t stream) {
+  return append_batch_launch("rb_append_batch", false, tree, tree_start, size, frames, timestep, action, reward,
+                             nonterminal, ring_state, running_max, last_frames, actions, rewards, terminals, k, stream);
+}
+
+int rb_append_batch_trunc(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep,
+                          int32_t* action, float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max,
+                          const float* const* last_frames, const int32_t* actions, const float* rewards,
+                          const int32_t* terminals, int k, rb_stream_t stream) {
+  return append_batch_launch("rb_append_batch_trunc", true, tree, tree_start, size, frames, timestep, action, reward,
+                             nonterminal, ring_state, running_max, last_frames, actions, rewards, terminals, k, stream);
 }
 
 // The value-rescaled entries' own refusals: support_q (C51) given, 0 <= eps <= 1 (NaN refused).

@@ -6,12 +6,14 @@ state is a structure of arrays on the device and every operation is one hand-wri
 called through the C ABI in include/rainbow_b200.h:
 
     append             -> rb_append        (K5)   memory.py:105-108, 56-61
+    append_truncated   -> rb_append_batch_trunc   (args.bootstrap_truncation: a time limit's last step and the
+                                                   observation it stopped at, no reference counterpart)
     sample             -> rb_tree_sample   (K1)   memory.py:124-132, 148-154
                           rb_gather        (K2)   memory.py:111-121, 134-146
                           (rb_gather_shift with shift_pad > 0: the same plus random-shift augmentation, no reference
                           counterpart; rb_gather_aug with intensity > 0 or copies != (1, 1): shift and intensity
                           augmentation of M copies of s and K of s'; rb_gather_horizon with an annealed horizon, see
-                          rainbow_b200.horizon)
+                          rainbow_b200.horizon; rb_gather_trunc with args.bootstrap_truncation)
     update_priorities  -> rb_tree_update   (K4)   memory.py:157-159, 23-48
     __next__           -> rb_iter_states          memory.py:166-178
 
@@ -31,10 +33,12 @@ import torch
 from . import _lib
 
 FRAME = 84 * 84
+FINAL = 2   # RB_NONTERMINAL_FINAL: the nonterminal byte of a final-observation record (append_truncated)
 
 # memory.py:7 -- only used to exchange state with reference-format consumers (pickles)
 Transition_dtype = np.dtype([("timestep", np.int32), ("state", np.uint8, (84, 84)), ("action", np.int32),
                              ("reward", np.float32), ("nonterminal", np.bool_)])
+Final_transition_dtype = np.dtype(Transition_dtype.descr + [("final", np.bool_)])
 
 
 # The replay's persistent fields, one list for pickling (ReplayMemory.__getstate__ / __setstate__) and for
@@ -86,6 +90,7 @@ class SegmentTree:
         self.action = torch.zeros(size, dtype=torch.int32, device=self.device)
         self.reward = torch.zeros(size, dtype=torch.float32, device=self.device)
         self.nonterminal = torch.zeros(size, dtype=torch.uint8, device=self.device)
+        self.final_records = False   # get() adds a `final` field (ReplayMemory with args.bootstrap_truncation)
         self.ring_state = torch.zeros(5, dtype=torch.int64, device=self.device)  # head, full, t_episode, appended, ticket
         self.running_max = torch.ones(1, dtype=torch.float32, device=self.device)  # memory.py:20
         self._status = torch.zeros(4, dtype=torch.int32, device=self.device)
@@ -176,15 +181,20 @@ class SegmentTree:
         self.full = self.full or self.index == 0
 
     def get(self, data_index):
-        """memory.py:85-86 (host copy of the selected records; inspection only)."""
+        """memory.py:85-86 (host copy of the selected records; inspection only).  With final_records set the records
+        carry one more bool field, `final`: a final-observation record (whose `nonterminal` reads True)."""
         idx = np.asarray(data_index) % self.size
         flat = torch.as_tensor(idx.reshape(-1), dtype=torch.int64, device=self.device)
-        out = np.zeros(idx.size, dtype=Transition_dtype)
+        dtype = Final_transition_dtype if self.final_records else Transition_dtype
+        out = np.zeros(idx.size, dtype=dtype)
         out["timestep"] = self.timestep[flat].cpu().numpy()
         out["state"] = self.frames[flat].cpu().numpy().reshape(-1, 84, 84)
         out["action"] = self.action[flat].cpu().numpy()
         out["reward"] = self.reward[flat].cpu().numpy()
-        out["nonterminal"] = self.nonterminal[flat].cpu().numpy().astype(np.bool_)
+        nonterminal = self.nonterminal[flat].cpu().numpy()
+        out["nonterminal"] = nonterminal.astype(np.bool_)
+        if self.final_records:
+            out["final"] = nonterminal == FINAL
         return out.reshape(idx.shape)
 
     # ---- bulk state exchange (tests, pickling, synthetic fill) -----------------------------------
@@ -258,6 +268,9 @@ class ReplayMemory:
             self.n = max(self.n, int(getattr(args, "multi_step_start", None) or self.n))
         self.priority_weight = args.priority_weight  # beta; main.py:161 overwrites this attribute every step
         self.priority_exponent = args.priority_exponent
+        # bootstrapping through time limits: append_truncated stores the observation a time limit stopped the episode
+        # at, and the gather cuts a sample's window there (rb_gather_trunc, nonterminals in discount form)
+        self.bootstrap_truncation = bool(getattr(args, "bootstrap_truncation", False))
         if self.history + self.n > 64:
             raise ValueError("history_length + multi_step must not exceed 64")
         if rng not in ("philox", "numpy"):
@@ -276,6 +289,9 @@ class ReplayMemory:
         self.n_step_scaling = torch.tensor([self.discount ** i for i in range(self.n)], dtype=torch.float32,
                                            device=self.device)
         self.transitions = SegmentTree(self.capacity, self.device)
+        if self.bootstrap_truncation:
+            self.transitions.final_records = True
+        self._fixed_row = self._fixed_horizon_row()
         if seed is None:   # data-parallel ranks launched with one torch seed must not draw the same stratified uniforms
             from .dist import GradSync, shard_seed
             rank = GradSync().rank
@@ -287,6 +303,21 @@ class ReplayMemory:
         self._lib = _lib.load()
         self._last = None
         self._stage = None
+
+    def _fixed_horizon_row(self):
+        """With bootstrap_truncation: the constant rb_horizon row of this replay's n and discount that rb_gather_trunc
+        reads when no annealed horizon is given -- n, fl32(gamma ** n) and fl32(gamma ** k) for k < n, in Python doubles
+        like n_step_scaling.  None without it."""
+        if not self.bootstrap_truncation:
+            return None
+        from .horizon import horizon_table
+        row = horizon_table(1, self.n, self.n, self.discount, self.discount)[:1]
+        return torch.from_numpy(row.view(np.uint8).copy()).to(self.device)
+
+    def holds_final_records(self):
+        """Synchronises.  Whether the ring holds a final-observation record (append_truncated)."""
+        self.flush_appends()
+        return bool((self.transitions.nonterminal == FINAL).any().item())
 
     def push_beta(self):
         """Mirror the host attribute `priority_weight` (main.py:161 rewrites it every step) into the device
@@ -326,18 +357,21 @@ class ReplayMemory:
             for k in slots:
                 self._stage_evt[k] = evt
 
+    def _newest_frame(self, state):
+        """(staging slot or None, the newest frame of `state` as a 16-byte aligned float32 frame the kernel reads)."""
+        last = state[-1]
+        if not last.is_cuda:
+            return self._stage_host_frame(last)
+        last = last.to(torch.float32).contiguous()
+        if last.data_ptr() % 16:
+            last = last.clone()
+        return None, last
+
     def append(self, state, action, reward, terminal):
         """memory.py:105-108.  `state` is the float32 [history,84,84] frame stack in [0,1]; only the newest
         frame is stored (quantised to uint8 on the device).  Host frames are staged through owned pinned memory and read
         by the kernel in place (no separate H2D copy launch); device frames are read in place."""
-        last = state[-1]
-        slot_id = None
-        if not last.is_cuda:
-            slot_id, last = self._stage_host_frame(last)
-        else:
-            last = last.to(torch.float32).contiguous()
-            if last.data_ptr() % 16:
-                last = last.clone()
+        slot_id, last = self._newest_frame(state)
         if self.defer_appends:
             # queued by reference: a DEVICE frame must not be modified by the caller before the flush (main.py's env
             # builds a fresh state tensor every step); host frames are already copied into the staging ring
@@ -354,24 +388,56 @@ class ReplayMemory:
             self._release_stage_slots([slot_id])
         self.t = 0 if terminal else self.t + 1
 
+    def append_truncated(self, state, action, reward, final_state):
+        """A time limit's last step (needs args.bootstrap_truncation): the transition (state, action, reward) with
+        nonterminal 1, then a final-observation record F holding the newest frame of `final_state` -- the observation the
+        time limit stopped the episode at.  F continues the episode's timesteps, has action 0, reward 0, leaf priority 0
+        (it is never sampled, and the running max stays) and the nonterminal byte FINAL; the next append starts an
+        episode.  A sample whose n-step window reaches F bootstraps from the stack ending at F, k < n steps on
+        (rb_gather_trunc).  One rb_append_batch_trunc launch, or two queued records with defer_appends."""
+        if not self.bootstrap_truncation:
+            raise _lib.RainbowB200Error("append_truncated needs args.bootstrap_truncation = True: without it the replay "
+                                        "cannot store the final observation a time limit stopped the episode at")
+        slot_id, last = self._newest_frame(state)
+        final_slot_id, final = self._newest_frame(final_state)
+        records = [(last, int(action), float(reward), 0, slot_id), (final, 0, 0.0, FINAL, final_slot_id)]
+        tr = self.transitions
+        if self.defer_appends:
+            if len(self._queue) + 2 > self.APPEND_BATCH:
+                self.flush_appends()
+            self._queue += records
+        else:
+            self._append_batch(records)
+        tr.index = (tr.index + 2) % tr.size
+        tr.full = tr.full or tr.index < 2
+        self.t = 0
+        if self.defer_appends and len(self._queue) >= self.APPEND_BATCH:
+            self.flush_appends()
+
     def flush_appends(self):
         """Write the queued transitions (defer_appends=True) with one rb_append_batch launch."""
         if not self._queue:
             return
-        import ctypes as C
         q, self._queue = self._queue, []
+        self._append_batch(q)
+        self._flushed_refs = q   # keep device frames alive until the next flush (the launch is asynchronous)
+
+    def _append_batch(self, q):
+        """One rb_append_batch launch (rb_append_batch_trunc with bootstrap_truncation, whose records may be FINAL) for
+        the records (frame, action, reward, terminal or FINAL, staging slot or None)."""
+        import ctypes as C
         k = len(q)
         tr = self.transitions
         frames = (C.c_void_p * k)(*[e[0].data_ptr() for e in q])   # device or pinned-host pointers (UVA)
         acts = (C.c_int32 * k)(*[e[1] for e in q])
         rews = (C.c_float * k)(*[e[2] for e in q])
-        terms = (C.c_int32 * k)(*[1 if e[3] else 0 for e in q])
-        _lib.check(self._lib.rb_append_batch(
+        terms = (C.c_int32 * k)(*[int(e[3]) for e in q])
+        launch = self._lib.rb_append_batch_trunc if self.bootstrap_truncation else self._lib.rb_append_batch
+        _lib.check(launch(
             _lib.ptr(tr.tree), tr.tree_start, tr.size, _lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action),
             _lib.ptr(tr.reward), _lib.ptr(tr.nonterminal), _lib.ptr(tr.ring_state), _lib.ptr(tr.running_max), frames, acts,
             rews, terms, k, _lib.stream()))
         self._release_stage_slots([e[4] for e in q if e[4] is not None])
-        self._flushed_refs = q   # keep device frames alive until the next flush (the launch is asynchronous)
 
     # ---- sample --------------------------------------------------------------------------------
     def _launch_sample(self, ws, u01=None, attempts=0):
@@ -407,18 +473,24 @@ class ReplayMemory:
 
     def _launch_gather(self, ws, shift_pad=0, intensity=0.0, copies=(1, 1), horizon=None):
         """The gather these settings select: rb_gather, rb_gather_shift (shifts only), rb_gather_aug (intensity or
-        copies), or with an annealed horizon rb_gather_horizon, which takes every augmentation setting."""
+        copies), or with an annealed horizon rb_gather_horizon, which takes every augmentation setting; with
+        bootstrap_truncation always rb_gather_trunc, which takes them all too."""
         tr = self.transitions
         shifts, scales = self._aug_buffers(ws, shift_pad, intensity, copies)
-        # the n-step window: this replay's n and discount powers, or the horizon's n_max and its current row
+        # the n-step window: this replay's n and discount powers (its constant row with bootstrap_truncation), or the
+        # horizon's n_max and its current row
         window = (self.n, self.n_step_scaling) if horizon is None else (horizon.n_max, horizon.current)
+        if self.bootstrap_truncation and horizon is None:
+            window = (self.n, self._fixed_row)
         common = (_lib.ptr(tr.frames), _lib.ptr(tr.timestep), _lib.ptr(tr.action), _lib.ptr(tr.reward),
                   _lib.ptr(tr.nonterminal), tr.size, _lib.ptr(ws.data_idx), ws.B, self.history, window[0],
                   _lib.ptr(window[1]), _lib.ptr(ws.states), _lib.ptr(ws.next_states), _lib.ptr(ws.actions),
                   _lib.ptr(ws.returns), _lib.ptr(ws.nonterminals))
         aug = (shift_pad, intensity, copies[0], copies[1], self.seed, _lib.ptr(self._rng_counter), _lib.ptr(shifts),
                _lib.ptr(scales))
-        if horizon is not None:
+        if self.bootstrap_truncation:
+            rc = self._lib.rb_gather_trunc(*common, *aug, _lib.stream())
+        elif horizon is not None:
             rc = self._lib.rb_gather_horizon(*common, *aug, _lib.stream())
         elif scales is not None:
             rc = self._lib.rb_gather_aug(*common, *aug, _lib.stream())
@@ -575,11 +647,16 @@ class ReplayMemory:
         state.update(device=str(self.device), rng_counter=int(self._rng_counter.item()), index=tr.index, full=tr.full,
                      max=tr.max)
         state.update((key, getattr(tr, attr).cpu().numpy()) for key, attr in PERSISTENT_ARRAYS)
+        if self.bootstrap_truncation:   # absent: off, as in files written before the switch existed
+            state["bootstrap_truncation"] = True
         return state
 
     def _init_runtime(self, rng_counter=0):
         self.n_step_scaling = torch.tensor([self.discount ** i for i in range(self.n)], dtype=torch.float32,
                                            device=self.device)
+        if self.bootstrap_truncation:
+            self.transitions.final_records = True
+        self._fixed_row = self._fixed_horizon_row()
         self.defer_appends, self._queue = False, []
         self._rng_counter = torch.tensor([int(rng_counter)], dtype=torch.int64, device=self.device)
         self._beta_dev = torch.full((1,), float(self.priority_weight), dtype=torch.float32, device=self.device)
@@ -594,6 +671,7 @@ class ReplayMemory:
         self.device = _require_cuda(s["device"])
         for k in PERSISTENT_HOST:
             setattr(self, k, s[k])
+        self.bootstrap_truncation = bool(s.get("bootstrap_truncation", False))
         self.transitions = SegmentTree(self.capacity, self.device)
         self.transitions.load_arrays(**{key: s[key] for key, _ in PERSISTENT_ARRAYS}, index=s["index"], full=s["full"],
                                      t_episode=s["t"], max_value=s["max"])
@@ -608,6 +686,7 @@ class ReplayMemory:
         self.capacity, self.history, self.discount, self.n = int(s["capacity"]), int(s["history"]), s["discount"], int(s["n"])
         self.priority_weight, self.priority_exponent, self.t = s["priority_weight"], s["priority_exponent"], int(s["t"])
         self.rng, self.max_attempts, self.strict = "philox", 64, False
+        self.bootstrap_truncation = False
         self.seed = int(torch.initial_seed()) & (2 ** 64 - 1)
         tr = s["transitions"]
         if isinstance(tr, SegmentTree):
@@ -620,8 +699,11 @@ class ReplayMemory:
         self._init_runtime()
 
     def reference_state(self, device="cpu"):
-        """(ReplayMemory.__dict__, SegmentTree.__dict__) exactly as the reference's objects hold them."""
-        self.flush_appends()
+        """(ReplayMemory.__dict__, SegmentTree.__dict__) exactly as the reference's objects hold them.  Refuses a ring
+        holding final-observation records (append_truncated): the reference's memory has no way to represent them."""
+        if self.holds_final_records():
+            raise _lib.RainbowB200Error("the replay holds final-observation records (append_truncated), which the "
+                                        "reference's memory cannot represent: no reference-format copy of it can be made")
         dev = torch.device(device)
         mem = dict(device=dev, capacity=self.capacity, history=self.history, discount=self.discount, n=self.n,
                    priority_weight=self.priority_weight, priority_exponent=self.priority_exponent, t=self.t,
