@@ -564,6 +564,32 @@ int rb_q_values_risk(const float* z, int M, int actions, int atoms, const float*
 int rb_qr_q_values_risk(const float* z, int M, int actions, int atoms, float* q, int64_t* best_action, float* best_q,
                         int risk_kind, float risk_eta, rb_stream_t stream);
 
+/* HL-Gauss targets for the categorical loss (Farebrother et al. 2024, "Stop Regressing"; DESIGN.md §20): cross-entropy
+ * against the histogram that N(y, sigma^2) puts on the support's bins, in place of C51's projection.  Per sample:
+ *   a*    = the double-DQN arg-max of the expected values of online(s') (first maximum wins), as the parents take it;
+ *   ybar  = the expected value of target(s') at a*;  y = clamp(fl32(r + fl32(fl32(nonterminal gamma_n) ybar)), vmin, vmax);
+ *   bins  e_k = fl32(support_k - h) for k < Z, e_Z = fl32(support_{Z-1} + h), h = fl32(delta_z / 2): the atoms are the
+ *         bin centres;
+ *   mass  t_k = fl32(fl32(e_k - y) c), c = fl32(1 / fl32(sqrt(2) sigma)); u_k = 1/2 (erfc(t_k) - erfc(t_{k+1})) when
+ *         t_k >= 0, 1/2 (erfc(-t_{k+1}) - erfc(-t_k)) when t_{k+1} <= 0, else 1/2 (erf(t_{k+1}) - erf(t_k));
+ *         U = sum_k u_k (per lane over its atoms k = lane + 32 r in r order, then the xor butterfly), m_k = fl32(u_k / U);
+ *   loss  -sum_k m_k log p_k(s, a) and the gradient row (w / B)(p sum(m) - m) of the taken action, as the parents form
+ *         them against their projection; priorities are this cross-entropy, whose floor is the entropy H(m) > 0.
+ * sigma is in return units (the agent passes fl32(ratio * delta_z)).  Each entry takes its parent's arguments (the name
+ * without _hlg), sigma after gamma_n, and the optional y_out [B] (y per sample) after astar_out; m_out and astar_out are
+ * the parent's.  RB_ERR_INVAL: the parent's refusals, plus a sigma that is not a positive normal fp32 (NaN, +-inf, 0,
+ * negatives and subnormals).  A refused call writes nothing.  Profiled under the parent's kernel id. */
+int rb_c51_hlg_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                         const float* returns, const float* nonterminals, const float* weights, const float* support,
+                         float vmin, float vmax, float delta_z, float gamma_n, float sigma, int B, int A, int Z,
+                         float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, float* y_out,
+                         rb_stream_t stream);
+int rb_c51_dueling_hlg_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                 const int64_t* actions, const float* returns, const float* nonterminals,
+                                 const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                 float gamma_n, float sigma, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                 float* y_out, rb_stream_t stream);
+
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */
 int rb_noisy_compose(const float* mu, const float* sigma, const float* eps, int64_t count, float* out,

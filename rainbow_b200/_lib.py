@@ -179,6 +179,11 @@ SIGNATURES = {
                                        _i32, _f32, _vp]),
     "rb_q_values_risk": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _vp]),
     "rb_qr_q_values_risk": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _f32, _vp]),
+    # HL-Gauss targets: each is its parent's signature with sigma after gamma_n and y_out after astar_out
+    "rb_c51_hlg_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32, _i32, _i32,
+                                       _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rb_c51_dueling_hlg_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32,
+                                               _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 # rb_learn_stats_record of include/rainbow_b200.h (48 bytes): field name -> numpy dtype, in memory order

@@ -28,7 +28,9 @@ One `learn(mem)` (agent.py:61-100) is:
                                                args.munchausen: rb_qr_dueling_munchausen_loss_grad -- the target net's
                                                softmax policy in place of the arg-max, and a clipped log-policy bonus;
                                                args.risk_measure: the _risk twin of the loss entry -- the arg-max on a
-                                               distorted expectation (CVaR / Wang) in place of the mean]
+                                               distorted expectation (CVaR / Wang) in place of the mean;
+                                               args.categorical_target = "hl_gauss": rb_c51_dueling_hlg_loss_grad --
+                                               cross-entropy against the Gaussian histogram of the scalar target]
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
@@ -111,6 +113,34 @@ def c51_dueling_loss_grad(z_online, z_target, actions_n, atoms, actions, returns
          float(gamma_n), B),
         _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (m_out, astar_out),
         None if eps is None else (_lib.ptr(support_q), float(eps)), risk)
+
+
+def c51_hlg_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax,
+                      delta_z, gamma_n, sigma, loss=None, grad=None, m_out=None, astar_out=None, y_out=None):
+    """K3 against HL-Gauss targets (rb_c51_hlg_loss_grad, DESIGN.md §20) on pre-softmax logits [B,A,Z]: the histogram of
+    N(y, sigma^2) over the support's bins in place of the projection, sigma in return units; returns (loss[B],
+    grad[B,A,Z]).  y_out [B]: the scalar target y per sample."""
+    B, A, Z = q_online_s.shape
+    return _loss_grad(
+        ("rb_c51_hlg_loss_grad",),
+        (_lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
+         float(gamma_n), float(sigma), B, A, Z),
+        _empty(B, like=q_online_s) if loss is None else loss, _empty(B, A, Z, like=q_online_s) if grad is None else grad,
+        (m_out, astar_out, y_out), None)
+
+
+def c51_dueling_hlg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin,
+                              vmax, delta_z, gamma_n, sigma, m_out=None, astar_out=None, y_out=None):
+    """K3 against HL-Gauss targets fed straight by the fused heads (rb_c51_dueling_hlg_loss_grad), rows as
+    c51_dueling_loss_grad takes them; returns (loss[B], dz[B, Z(1+A)])."""
+    B = actions.shape[0]
+    return _loss_grad(
+        ("rb_c51_dueling_hlg_loss_grad",),
+        (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
+         float(gamma_n), float(sigma), B),
+        _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (m_out, astar_out, y_out), None)
 
 
 def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin,
@@ -342,6 +372,42 @@ def risk_options(args):
     if not (ok(float(eta)) and ok(eta32)):
         raise ValueError(f"risk_eta must be {want}, got {eta}")
     return measure, eta32
+
+
+CATEGORICAL_TARGETS = ("projection", "hl_gauss")
+
+
+def hl_gauss_options(args):
+    """sigma / delta_z of HL-Gauss targets (Farebrother et al. 2024, DESIGN.md §20) from `args`, or None when
+    args.categorical_target is absent, None or "projection" (C51's projection).  categorical_target "hl_gauss" trains the
+    categorical head by cross-entropy against the histogram of N(y, sigma^2) over the support's bins, y the scalar
+    double-DQN target; args.hl_gauss_sigma (absent or None: 0.75, the paper's setting) is sigma in bin widths, in
+    (0, 100] and a normal fp32.  Refused with it: distribution "quantile", value_transform "rescale", a risk measure and
+    augment_m / augment_k other than (1, 1)."""
+    target = getattr(args, "categorical_target", None)
+    if target is None or (isinstance(target, str) and target == "projection"):
+        return None
+    if not isinstance(target, str) or target not in CATEGORICAL_TARGETS:
+        raise ValueError(f"categorical_target must be one of {CATEGORICAL_TARGETS} or None, got {target!r}")
+    if getattr(args, "distribution", None) == "quantile":
+        raise ValueError("categorical_target 'hl_gauss' does not compose with distribution 'quantile': it is a target for "
+                         "the categorical head")
+    if getattr(args, "value_transform", None) not in (None, "none"):
+        raise ValueError("categorical_target 'hl_gauss' does not compose with value_transform 'rescale'")
+    if getattr(args, "risk_measure", None) not in (None, "neutral"):
+        raise ValueError("categorical_target 'hl_gauss' does not compose with risk_measure "
+                         f"{getattr(args, 'risk_measure')!r}")
+    copies = (getattr(args, "augment_m", 1), getattr(args, "augment_k", 1))
+    if copies != (1, 1):
+        raise ValueError(f"categorical_target 'hl_gauss' needs augment_m = augment_k = 1, got {copies}")
+    ratio = getattr(args, "hl_gauss_sigma", None)
+    ratio = 0.75 if ratio is None else ratio
+    if isinstance(ratio, bool) or not isinstance(ratio, (int, float, np.floating, np.integer)):
+        raise ValueError(f"hl_gauss_sigma must be a number, got {ratio!r}")
+    ratio = float(ratio)
+    if not (0.0 < ratio <= 100.0 and np.float32(ratio) >= np.finfo(np.float32).tiny):
+        raise ValueError(f"hl_gauss_sigma (sigma in bin widths) must be in (0, 100] and a normal fp32, got {ratio}")
+    return ratio
 
 
 def risk_beta(t, measure, eta):
@@ -688,6 +754,8 @@ class Agent:
         self.Vmax = args.V_max
         self.support = torch.linspace(args.V_min, args.V_max, self.atoms).to(device=self.device)  # agent.py:18
         self.delta_z = (args.V_max - args.V_min) / (self.atoms - 1)
+        # HL-Gauss targets (off by default): sigma / delta_z, or None for C51's projection
+        self.hl_gauss_sigma = hl_gauss_options(args)
         # the support in return units, fl32(h^-1(z_j)) from the fp32 support in float64 (the support itself when off): the
         # double-DQN arg-max, the target atoms, acting and the statistics take it
         self.q_support = self.support
@@ -1179,6 +1247,8 @@ class Agent:
             return (*qr_dueling_avg_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), M, K, theta_out=m,
                                               eps=vt["eps"]), m)
         c51 = (self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n())
+        if self.hl_gauss_sigma is not None:   # refused with copies other than (1, 1)
+            return (*c51_dueling_hlg_loss_grad(*rows, *c51, self._hlg_sigma(), m_out=m), m)
         if (M, K) == (1, 1):
             return (*c51_dueling_loss_grad(*rows, *c51, m_out=m, **vt, risk=self._risk_args()), m)
         return (*c51_dueling_avg_loss_grad(*rows, *c51, M, K, m_out=m, **vt), m)
@@ -1196,8 +1266,15 @@ class Agent:
         risk = self._risk_args()
         if self.quantile:
             return (*qr_loss_grad(*rows, self.quantile_kappa, self._gamma_n(), theta_out=m, eps=vt["eps"], risk=risk), m)
+        if self.hl_gauss_sigma is not None:
+            return (*c51_hlg_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(),
+                                       self._hlg_sigma(), m_out=m), m)
         return (*c51_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m, **vt,
                                risk=risk), m)
+
+    def _hlg_sigma(self):
+        """The sigma the HL-Gauss entries take, in return units: fl32(hl_gauss_sigma * delta_z)."""
+        return float(np.float32(self.hl_gauss_sigma * self.delta_z))
 
     def _risk_args(self):
         """(kind, eta) of the _risk entries (RB_RISK_CVAR / RB_RISK_WANG), or None when no risk measure is set."""

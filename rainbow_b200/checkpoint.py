@@ -383,6 +383,9 @@ def _meta(agent, mem):
         hyper["munchausen_alpha"], hyper["munchausen_temperature"], hyper["munchausen_clip"] = agent.munchausen
     if agent.risk is not None:   # absent: the mean selects (no risk measure)
         hyper["risk_measure"], hyper["risk_eta"] = agent.risk
+    hlg = getattr(agent, "hl_gauss_sigma", None)   # an agent without the attribute reads as off
+    if hlg is not None:   # absent: C51's projection
+        hyper["categorical_target"], hyper["hl_gauss_sigma"] = "hl_gauss", hlg
     if agent.bootstrap_truncation:   # absent: off
         hyper["bootstrap_truncation"] = True
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
@@ -547,6 +550,12 @@ def _validate(agent, mem, man):
     live = agent.risk or (None, None)
     if risk != live:
         raise _Error(f"risk measure (measure, eta) differs: checkpoint {risk}, live {live}")
+    # and one trained against another categorical target, or with another HL-Gauss width
+    hlg = (hyper.get("categorical_target"), hyper.get("hl_gauss_sigma"))
+    live = getattr(agent, "hl_gauss_sigma", None)
+    live = (None, None) if live is None else ("hl_gauss", live)
+    if hlg != live:
+        raise _Error(f"categorical target (categorical_target, hl_gauss_sigma) differs: checkpoint {hlg}, live {live}")
     # a ring with final-observation records means nothing to a replay that gathers without cutting windows at them
     if mem is not None and (man.get("replay") or {}).get("final_records") and not mem.bootstrap_truncation:
         raise _Error("the checkpoint's replay holds final-observation records (args.bootstrap_truncation) and this "

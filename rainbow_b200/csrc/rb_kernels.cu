@@ -1783,6 +1783,174 @@ k_c51_dueling_avg(const float* __restrict__ z_on, const float* __restrict__ z_tg
   }
 }
 
+// ---- HL-Gauss targets (Farebrother et al. 2024; DESIGN.md §20): the scalar double-DQN target as a Gaussian histogram ----
+// y = clamp(fl32(ret + fl32(sc ybar)), vmin, vmax).  Bin k is [e_k, e_{k+1}]: e_k = fl32(z_k - h) for k < Z,
+// e_Z = fl32(z_{Z-1} + h), h = fl32(delta_z / 2), so the atoms are the bin centres.  t_k = fl32(fl32(e_k - y) c),
+// c = fl32(1 / fl32(sqrt(2) sigma)); the mass of N(y, sigma^2) in bin k is u_k = 1/2 (erfc(t_k) - erfc(t_{k+1})) above y,
+// 1/2 (erfc(-t_{k+1}) - erfc(-t_k)) below y and 1/2 (erf(t_{k+1}) - erf(t_k)) in the bin holding y: each tail keeps its
+// relative accuracy.  U = sum u_k (each lane over its atoms in r order, then the xor butterfly), m_k = fl32(u_k / U), 0
+// past Z.  erff / erfcf at full precision.  Returns y; all lanes hold it.
+template <int C51_R>
+__device__ __forceinline__ float hlg_target(int lane, int Z, const float* __restrict__ support, float delta_z, float vmin,
+                                            float vmax, float sigma, float ret, float sc, float ybar, float (&m)[C51_R]) {
+  const float y = fminf(fmaxf(__fadd_rn(ret, __fmul_rn(sc, ybar)), vmin), vmax);
+  const float h = __fmul_rn(delta_z, 0.5f);
+  const float c = __fdiv_rn(1.0f, __fmul_rn(1.41421356f, sigma));
+  float u[C51_R], usum = 0.0f;
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) {
+    const int k = lane + 32 * r;
+    u[r] = 0.0f;
+    if (k < Z) {
+      const float zk = __ldg(support + k);
+      const float hi = k + 1 < Z ? __fsub_rn(__ldg(support + k + 1), h) : __fadd_rn(zk, h);
+      const float t0 = __fmul_rn(__fsub_rn(__fsub_rn(zk, h), y), c), t1 = __fmul_rn(__fsub_rn(hi, y), c);
+      float d;
+      if (t0 >= 0.0f) d = __fsub_rn(erfcf(t0), erfcf(t1));
+      else if (t1 <= 0.0f) d = __fsub_rn(erfcf(-t1), erfcf(-t0));
+      else d = __fsub_rn(erff(t1), erff(t0));
+      u[r] = __fmul_rn(0.5f, d);
+      usum = __fadd_rn(usum, u[r]);
+    }
+  }
+  usum = warp_sum(usum);
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) m[r] = lane + 32 * r < Z ? __fdiv_rn(u[r], usum) : 0.0f;
+  return y;
+}
+
+// HL-Gauss loss on the fused heads' rows, laid out as k_c51_dueling (one CTA of C51D_T threads per sample):
+//   phase 0  all threads stage online(s), online(s') and target(s') (stage_z_rows);
+//   phase 1  warp a: the expected value of action a of online(s');
+//   phase 2  warp 0: a* (first maximum wins), ybar = the expected value of target(s') at a*, y and m (hlg_target), then the
+//            loss and gradient row of online(s) at the taken action against m (c51_loss_row);
+//   phase 3  dz (dueling_dz).
+template <int C51_R>
+__global__ void __launch_bounds__(C51D_T)
+k_c51_dueling_hlg(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
+                  const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                  const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax,
+                  float delta_z, float gamma_n, float sigma, int B, int A, int Z, float* __restrict__ loss,
+                  float* __restrict__ dz, float* __restrict__ m_out, int64_t* __restrict__ astar_out,
+                  float* __restrict__ y_out) {
+  extern __shared__ __align__(16) float s_dyn[];
+  const int N2 = Z + A * Z;
+  float* zs = s_dyn;              // [3][N2]: online(s), online(s'), target(s')
+  float* q_s = zs + 3 * N2;       // [Z] online logits of the taken action
+  float* s_g = q_s + Z;           // [Z] gradient row
+  float* s_ev = s_g + Z;          // [A] expected values
+  const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  stage_z_rows<C51D_T>(zs, z_on, z_tg, i, B, N2, 1, 1);
+  __syncthreads();
+  const int act = (int)actions[i];
+  float sup[C51_R];
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  {  // phase 1
+    const float* r1 = zs + N2;
+    float mean[C51_R];
+#pragma unroll
+    for (int r = 0; r < C51_R; ++r) mean[r] = lane + 32 * r < Z ? dueling_mean(r1, A, Z, lane + 32 * r) : 0.0f;
+    for (int a = warp; a < A; a += C51D_T / 32) {
+      float x[C51_R];
+#pragma unroll
+      for (int r = 0; r < C51_R; ++r) {
+        const int c = lane + 32 * r;
+        x[r] = (c < Z) ? dueling_q(r1[c], r1[Z + a * Z + c], mean[r]) : -CUDART_INF_F;
+      }
+      const float ev = c51_expected_value<C51_R>(x, sup, Z, lane);
+      if (lane == 0) s_ev[a] = ev;
+    }
+  }
+  __syncthreads();
+  if (warp == 0) {  // phase 2
+    const int best = first_argmax(s_ev, A);
+    float x[C51_R];
+#pragma unroll
+    for (int r = 0; r < C51_R; ++r) {
+      const int c = lane + 32 * r;
+      x[r] = (c < Z) ? dueling_q(zs + 2 * N2, A, Z, c, best) : -CUDART_INF_F;
+      if (c < Z) q_s[c] = dueling_q(zs, A, Z, c, act);
+    }
+    __syncwarp();
+    const float ybar = c51_expected_value<C51_R>(x, sup, Z, lane);
+    float m[C51_R], g[C51_R];
+    const float y = hlg_target<C51_R>(lane, Z, support, delta_z, vmin, vmax, sigma, __ldg(returns + i),
+                                      __fmul_rn(__ldg(nonterminals + i), gamma_n), ybar, m);
+    const float l = c51_loss_row<C51_R>(lane, Z, q_s, m, __fdiv_rn(__ldg(weights + i), (float)B), g);
+    if (lane == 0) {
+      loss[i] = l;
+      if (astar_out) astar_out[i] = best;
+      if (y_out) y_out[i] = y;
+    }
+#pragma unroll
+    for (int r = 0; r < C51_R; ++r) {
+      const int c = lane + 32 * r;
+      if (c < Z) {
+        s_g[c] = g[r];
+        if (m_out) m_out[(size_t)i * Z + c] = m[r];
+      }
+    }
+  }
+  __syncthreads();
+  dueling_dz<C51D_T>(dz + (size_t)i * N2, s_g, A, Z, act);  // phase 3
+}
+
+// HL-Gauss loss on plain logit rows [B][A][Z] (the library head), k_c51's layout: one warp per sample, grad [B][A][Z]
+// zero but for the taken action's row.
+template <int C51_R>
+__global__ void __launch_bounds__(C51_WARPS * 32)
+k_c51_hlg(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
+          const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
+          const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax, float delta_z,
+          float gamma_n, float sigma, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ grad,
+          float* __restrict__ m_out, int64_t* __restrict__ astar_out, float* __restrict__ y_out) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int i = blockIdx.x * C51_WARPS + warp;
+  if (i >= B) return;
+  const int act = (int)actions[i];
+  float sup[C51_R], x[C51_R];
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  int best = 0;
+  float best_ev = -CUDART_INF_F;
+  for (int a = 0; a < A; ++a) {
+    const float* row = q_on_ns + ((size_t)i * A + a) * Z;
+#pragma unroll
+    for (int r = 0; r < C51_R; ++r) x[r] = (lane + 32 * r < Z) ? row[lane + 32 * r] : -CUDART_INF_F;
+    const float ev = c51_expected_value<C51_R>(x, sup, Z, lane);
+    if (ev > best_ev) {  // first maximum wins, like torch.argmax
+      best_ev = ev;
+      best = a;
+    }
+  }
+  const float* row_t = q_tg_ns + ((size_t)i * A + best) * Z;
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) x[r] = (lane + 32 * r < Z) ? row_t[lane + 32 * r] : -CUDART_INF_F;
+  const float ybar = c51_expected_value<C51_R>(x, sup, Z, lane);
+  float m[C51_R], g[C51_R];
+  const float y = hlg_target<C51_R>(lane, Z, support, delta_z, vmin, vmax, sigma, __ldg(returns + i),
+                                    __fmul_rn(__ldg(nonterminals + i), gamma_n), ybar, m);
+  const float l = c51_loss_row<C51_R>(lane, Z, q_on_s + ((size_t)i * A + act) * Z, m,
+                                      __fdiv_rn(__ldg(weights + i), (float)B), g);
+  if (lane == 0) {
+    loss[i] = l;
+    if (astar_out) astar_out[i] = best;
+    if (y_out) y_out[i] = y;
+  }
+  float* gq = grad + (size_t)i * A * Z;
+  for (int j = lane; j < A * Z; j += 32) gq[j] = 0.0f;
+  __syncwarp();
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) {
+    const int c = lane + 32 * r;
+    if (c < Z) {
+      gq[(size_t)act * Z + c] = g[r];
+      if (m_out) m_out[(size_t)i * Z + c] = m[r];
+    }
+  }
+}
+
 // ================================================================================================
 // Q-values for acting / evaluation (agent.py:53-55 act, :110-112 evaluate_q): one warp per state.
 // From the head output z = (z_value | z_advantage): q[a][z] = zv + za[a] - mean_a za (model.py:75), softmax over
@@ -3676,6 +3844,58 @@ int rb_c51_dueling_risk_loss_grad(const float* z_online, const float* z_target, 
   return c51_dueling_launch<false, true>("rb_c51_dueling_risk_loss_grad", z_online, z_target, actions_n, atoms, actions,
                                          returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, loss, dz,
                                          m_out, astar_out, nullptr, 0.0f, stream, risk_kind, risk_eta);
+}
+
+// The HL-Gauss entries' own refusal: sigma a positive normal fp32 (NaN, +-inf, 0, negatives and subnormals refused).
+static int hlg_check(const char* name, float sigma) {
+  if (!(sigma >= 1.17549435e-38f && sigma <= 3.40282347e+38f)) {
+    char msg[128];
+    snprintf(msg, sizeof msg, "%s: sigma must be a positive normal fp32", name);
+    return fail(RB_ERR_INVAL, msg);
+  }
+  return RB_OK;
+}
+
+int rb_c51_hlg_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns, const int64_t* actions,
+                         const float* returns, const float* nonterminals, const float* weights, const float* support,
+                         float vmin, float vmax, float delta_z, float gamma_n, float sigma, int B, int A, int Z,
+                         float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, float* y_out,
+                         rb_stream_t stream) {
+  const char* name = "rb_c51_hlg_loss_grad";
+  int rc = c51_check(name, q_online_s && q_online_ns && q_target_ns && actions && returns && nonterminals && weights &&
+                     support && loss && grad_q_online_s, B, A, Z, "A", "Z");
+  if (rc == RB_OK) rc = hlg_check(name, sigma);
+  if (rc != RB_OK) return rc;
+  const auto k = Z <= 64 ? k_c51_hlg<2> : k_c51_hlg<4>;
+  { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
+    k<<<(B + C51_WARPS - 1) / C51_WARPS, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n,
+        sigma, B, A, Z, loss, grad_q_online_s, m_out, astar_out, y_out); }
+  return check_launch(name);
+}
+
+int rb_c51_dueling_hlg_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                 const int64_t* actions, const float* returns, const float* nonterminals,
+                                 const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                 float gamma_n, float sigma, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                 float* y_out, rb_stream_t stream) {
+  const char* name = "rb_c51_dueling_hlg_loss_grad";
+  const int Z = atoms, A = actions_n;
+  int rc = c51_check(name, z_online && z_target && actions && returns && nonterminals && weights && support && loss && dz,
+                     B, A, Z, "actions", "atoms");
+  if (rc == RB_OK) rc = hlg_check(name, sigma);
+  if (rc != RB_OK) return rc;
+  // k_c51_dueling's size (the kernel leaves its [Z] slot of target logits unused), so both refuse the same shapes
+  const size_t smem = (size_t)(3 * (Z + A * Z) + 3 * Z + A) * sizeof(float);
+  rc = smem_check(name, smem, "actions * atoms too large");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling_hlg<2>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling_hlg<4>, smem, name);
+  if (rc != RB_OK) return rc;
+  const auto k = Z <= 64 ? k_c51_dueling_hlg<2> : k_c51_dueling_hlg<4>;
+  { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
+    k<<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, support, vmin,
+                                                 vmax, delta_z, gamma_n, sigma, B, A, Z, loss, dz, m_out, astar_out, y_out); }
+  return check_launch(name);
 }
 
 extern "C++" {
