@@ -590,6 +590,45 @@ int rb_c51_dueling_hlg_loss_grad(const float* z_online, const float* z_target, i
                                  float gamma_n, float sigma, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
                                  float* y_out, rb_stream_t stream);
 
+/* Two-hot targets for the categorical loss (Farebrother et al. 2024; MuZero, Schrittwieser et al. 2020, Appendix F;
+ * DESIGN.md §21): cross-entropy against the scalar double-DQN target y split between its two neighbouring atoms, in place
+ * of C51's projection.  Per sample:
+ *   a*    = the double-DQN arg-max of the expected values of online(s') (first maximum wins), as the parents take it;
+ *   ybar  = the expected value of target(s') at a*;  y = clamp(fl32(r + fl32(fl32(nonterminal gamma_n) ybar)), vmin, vmax);
+ *   split b = fl32(fl32(y - vmin) / delta_z), l = floor(b), u = ceil(b), then the projection's fix-ups (u > 0 and l == u:
+ *         l -= 1; then l < Z - 1 and l == u: u += 1); m_l = fl32(u - b), m_u = fl32(b - l), every other m_k = 0 (an
+ *         index u = Z, where rounding puts b past Z - 1, is dropped as the projection drops it);
+ *   loss  -sum_k m_k log p_k(s, a) and the gradient row (w / B)(p sum(m) - m) of the taken action, as the parents form
+ *         them; priorities are this cross-entropy, whose floor is the entropy H(m) <= ln 2 (0 when y is on an atom).
+ * Each entry takes its parent's arguments (rb_c51_loss_grad / rb_c51_dueling_loss_grad) and the optional y_out [B]
+ * (y per sample) after astar_out; m_out and astar_out are the parent's.  RB_ERR_INVAL / RB_ERR_RANGE: the parent's
+ * refusals.  A refused call writes nothing.  Profiled under the parent's kernel id. */
+int rb_c51_twohot_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
+                            const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                            const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z,
+                            float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, float* y_out,
+                            rb_stream_t stream);
+int rb_c51_dueling_twohot_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                    const int64_t* actions, const float* returns, const float* nonterminals,
+                                    const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                    float gamma_n, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                    float* y_out, rb_stream_t stream);
+
+/* The two-hot entries under value rescaling (DESIGN.md §16, §21): support_q = fl32(h^-1(support)) in place of the support
+ * for the arg-max and ybar (return units), and y = clamp(h(fl32(r + fl32(sc ybar))), vmin, vmax), h first as
+ * rb_c51_vt_loss_grad forms its target atoms; y_out is then in h units.  support_q and eps after y_out.  Refusals:
+ * rb_c51_vt_loss_grad's first (a null support_q, eps outside [0, 1] or NaN), then the parent's. */
+int rb_c51_twohot_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
+                               const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                               const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A,
+                               int Z, float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, float* y_out,
+                               const float* support_q, float eps, rb_stream_t stream);
+int rb_c51_dueling_twohot_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                       const int64_t* actions, const float* returns, const float* nonterminals,
+                                       const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                       float gamma_n, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                       float* y_out, const float* support_q, float eps, rb_stream_t stream);
+
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */
 int rb_noisy_compose(const float* mu, const float* sigma, const float* eps, int64_t count, float* out,

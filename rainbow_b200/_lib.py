@@ -184,6 +184,15 @@ SIGNATURES = {
                                        _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rb_c51_dueling_hlg_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32,
                                                _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    # two-hot targets: each is its parent's signature with y_out after astar_out; the _vt twins add support_q, eps after it
+    "rb_c51_twohot_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i32, _i32, _i32,
+                                          _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rb_c51_twohot_vt_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i32, _i32,
+                                             _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _vp]),
+    "rb_c51_dueling_twohot_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32,
+                                                  _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rb_c51_dueling_twohot_vt_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32,
+                                                     _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _vp]),
 }
 
 # rb_learn_stats_record of include/rainbow_b200.h (48 bytes): field name -> numpy dtype, in memory order

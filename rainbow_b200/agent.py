@@ -30,7 +30,10 @@ One `learn(mem)` (agent.py:61-100) is:
                                                args.risk_measure: the _risk twin of the loss entry -- the arg-max on a
                                                distorted expectation (CVaR / Wang) in place of the mean;
                                                args.categorical_target = "hl_gauss": rb_c51_dueling_hlg_loss_grad --
-                                               cross-entropy against the Gaussian histogram of the scalar target]
+                                               cross-entropy against the Gaussian histogram of the scalar target;
+                                               args.categorical_target = "two_hot": rb_c51_dueling_twohot_loss_grad
+                                               (_vt twin under value rescaling) -- the scalar target split between its
+                                               two neighbouring atoms]
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
@@ -141,6 +144,39 @@ def c51_dueling_hlg_loss_grad(z_online, z_target, actions_n, atoms, actions, ret
          _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
          float(gamma_n), float(sigma), B),
         _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (m_out, astar_out, y_out), None)
+
+
+def c51_twohot_loss_grad(q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin,
+                         vmax, delta_z, gamma_n, loss=None, grad=None, m_out=None, astar_out=None, y_out=None,
+                         support_q=None, eps=None):
+    """K3 against two-hot targets (rb_c51_twohot_loss_grad, DESIGN.md §21) on pre-softmax logits [B,A,Z]: the scalar
+    double-DQN target y split between its two neighbouring atoms in place of the projection; returns (loss[B],
+    grad[B,A,Z]).  y_out [B]: y per sample.  eps given: value rescaling (rb_c51_twohot_vt_loss_grad) with
+    support_q = fl32(h^-1(support)), y_out then in h units."""
+    B, A, Z = q_online_s.shape
+    return _loss_grad(
+        ("rb_c51_twohot_loss_grad", "rb_c51_twohot_vt_loss_grad"),
+        (_lib.ptr(q_online_s), _lib.ptr(q_online_ns), _lib.ptr(q_target_ns), _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
+         float(gamma_n), B, A, Z),
+        _empty(B, like=q_online_s) if loss is None else loss, _empty(B, A, Z, like=q_online_s) if grad is None else grad,
+        (m_out, astar_out, y_out), None if eps is None else (_lib.ptr(support_q), float(eps)))
+
+
+def c51_dueling_twohot_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support,
+                                 vmin, vmax, delta_z, gamma_n, m_out=None, astar_out=None, y_out=None, support_q=None,
+                                 eps=None):
+    """K3 against two-hot targets fed straight by the fused heads (rb_c51_dueling_twohot_loss_grad, or
+    rb_c51_dueling_twohot_vt_loss_grad with eps given), rows as c51_dueling_loss_grad takes them; returns (loss[B],
+    dz[B, Z(1+A)])."""
+    B = actions.shape[0]
+    return _loss_grad(
+        ("rb_c51_dueling_twohot_loss_grad", "rb_c51_dueling_twohot_vt_loss_grad"),
+        (_lib.ptr(z_online), _lib.ptr(z_target), actions_n, atoms, _lib.ptr(actions), _lib.ptr(returns),
+         _lib.ptr(nonterminals), _lib.ptr(weights), _lib.ptr(support), float(vmin), float(vmax), float(delta_z),
+         float(gamma_n), B),
+        _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (m_out, astar_out, y_out),
+        None if eps is None else (_lib.ptr(support_q), float(eps)))
 
 
 def c51_dueling_avg_loss_grad(z_online, z_target, actions_n, atoms, actions, returns, nonterminals, weights, support, vmin,
@@ -374,7 +410,7 @@ def risk_options(args):
     return measure, eta32
 
 
-CATEGORICAL_TARGETS = ("projection", "hl_gauss")
+CATEGORICAL_TARGETS = ("projection", "hl_gauss", "two_hot")
 
 
 def hl_gauss_options(args):
@@ -385,7 +421,7 @@ def hl_gauss_options(args):
     (0, 100] and a normal fp32.  Refused with it: distribution "quantile", value_transform "rescale", a risk measure and
     augment_m / augment_k other than (1, 1)."""
     target = getattr(args, "categorical_target", None)
-    if target is None or (isinstance(target, str) and target == "projection"):
+    if target is None or (isinstance(target, str) and target in ("projection", "two_hot")):
         return None
     if not isinstance(target, str) or target not in CATEGORICAL_TARGETS:
         raise ValueError(f"categorical_target must be one of {CATEGORICAL_TARGETS} or None, got {target!r}")
@@ -408,6 +444,27 @@ def hl_gauss_options(args):
     if not (0.0 < ratio <= 100.0 and np.float32(ratio) >= np.finfo(np.float32).tiny):
         raise ValueError(f"hl_gauss_sigma (sigma in bin widths) must be in (0, 100] and a normal fp32, got {ratio}")
     return ratio
+
+
+def two_hot_options(args):
+    """Whether args.categorical_target is "two_hot" (DESIGN.md §21): the categorical head trained by cross-entropy against
+    the scalar double-DQN target y split between its two neighbouring atoms, in place of C51's projection (absent, None,
+    "projection" or "hl_gauss": False; hl_gauss_options reads those).  Composes with value_transform "rescale" (y is then
+    h of the return-units target, on the h-space support); hl_gauss_sigma is not read.  Refused with it: distribution
+    "quantile", a risk measure and augment_m / augment_k other than (1, 1)."""
+    target = getattr(args, "categorical_target", None)
+    if not (isinstance(target, str) and target == "two_hot"):
+        return False
+    if getattr(args, "distribution", None) == "quantile":
+        raise ValueError("categorical_target 'two_hot' does not compose with distribution 'quantile': it is a target for "
+                         "the categorical head")
+    if getattr(args, "risk_measure", None) not in (None, "neutral"):
+        raise ValueError("categorical_target 'two_hot' does not compose with risk_measure "
+                         f"{getattr(args, 'risk_measure')!r}")
+    copies = (getattr(args, "augment_m", 1), getattr(args, "augment_k", 1))
+    if copies != (1, 1):
+        raise ValueError(f"categorical_target 'two_hot' needs augment_m = augment_k = 1, got {copies}")
+    return True
 
 
 def risk_beta(t, measure, eta):
@@ -756,6 +813,8 @@ class Agent:
         self.delta_z = (args.V_max - args.V_min) / (self.atoms - 1)
         # HL-Gauss targets (off by default): sigma / delta_z, or None for C51's projection
         self.hl_gauss_sigma = hl_gauss_options(args)
+        # two-hot targets (off by default; hl_gauss_options returns None for them)
+        self.two_hot = two_hot_options(args)
         # the support in return units, fl32(h^-1(z_j)) from the fp32 support in float64 (the support itself when off): the
         # double-DQN arg-max, the target atoms, acting and the statistics take it
         self.q_support = self.support
@@ -1249,6 +1308,8 @@ class Agent:
         c51 = (self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n())
         if self.hl_gauss_sigma is not None:   # refused with copies other than (1, 1)
             return (*c51_dueling_hlg_loss_grad(*rows, *c51, self._hlg_sigma(), m_out=m), m)
+        if self.two_hot:   # refused with copies other than (1, 1)
+            return (*c51_dueling_twohot_loss_grad(*rows, *c51, m_out=m, **vt), m)
         if (M, K) == (1, 1):
             return (*c51_dueling_loss_grad(*rows, *c51, m_out=m, **vt, risk=self._risk_args()), m)
         return (*c51_dueling_avg_loss_grad(*rows, *c51, M, K, m_out=m, **vt), m)
@@ -1269,6 +1330,9 @@ class Agent:
         if self.hl_gauss_sigma is not None:
             return (*c51_hlg_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(),
                                        self._hlg_sigma(), m_out=m), m)
+        if self.two_hot:
+            return (*c51_twohot_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(),
+                                          m_out=m, **vt), m)
         return (*c51_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m, **vt,
                                risk=risk), m)
 

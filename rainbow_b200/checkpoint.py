@@ -386,6 +386,8 @@ def _meta(agent, mem):
     hlg = getattr(agent, "hl_gauss_sigma", None)   # an agent without the attribute reads as off
     if hlg is not None:   # absent: C51's projection
         hyper["categorical_target"], hyper["hl_gauss_sigma"] = "hl_gauss", hlg
+    if getattr(agent, "two_hot", False):   # two-hot targets record the switch alone
+        hyper["categorical_target"] = "two_hot"
     if agent.bootstrap_truncation:   # absent: off
         hyper["bootstrap_truncation"] = True
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
@@ -554,6 +556,8 @@ def _validate(agent, mem, man):
     hlg = (hyper.get("categorical_target"), hyper.get("hl_gauss_sigma"))
     live = getattr(agent, "hl_gauss_sigma", None)
     live = (None, None) if live is None else ("hl_gauss", live)
+    if getattr(agent, "two_hot", False):
+        live = ("two_hot", None)
     if hlg != live:
         raise _Error(f"categorical target (categorical_target, hl_gauss_sigma) differs: checkpoint {hlg}, live {live}")
     # a ring with final-observation records means nothing to a replay that gathers without cutting windows at them

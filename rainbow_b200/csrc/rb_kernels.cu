@@ -1819,20 +1819,63 @@ __device__ __forceinline__ float hlg_target(int lane, int Z, const float* __rest
   return y;
 }
 
-// HL-Gauss loss on the fused heads' rows, laid out as k_c51_dueling (one CTA of C51D_T threads per sample):
-//   phase 0  all threads stage online(s), online(s') and target(s') (stage_z_rows);
-//   phase 1  warp a: the expected value of action a of online(s');
-//   phase 2  warp 0: a* (first maximum wins), ybar = the expected value of target(s') at a*, y and m (hlg_target), then the
-//            loss and gradient row of online(s) at the taken action against m (c51_loss_row);
-//   phase 3  dz (dueling_dz).
+// ---- Two-hot targets (Farebrother et al. 2024; MuZero, Schrittwieser et al. 2020, App. F; DESIGN.md §21) ----
+// y = clamp(fl32(ret + fl32(sc ybar)), vmin, vmax), or under VT clamp(h(fl32(ret + fl32(sc ybar))), vmin, vmax) (c51_core's
+// order for its target atoms: h first, then the clamp).  b = fl32(fl32(y - vmin) / delta_z), l = floor(b), u = ceil(b)
+// with c51_core's two fix-ups (so a y on an atom keeps its mass), m_l = fl32(u - b), m_u = fl32(b - l), m_k = 0 elsewhere
+// (an index u = Z, where fp32 rounding puts b past Z - 1, is dropped, as c51_core drops it).  Returns y; all lanes hold it.
+template <int C51_R, bool VT>
+__device__ __forceinline__ float twohot_target(int lane, int Z, float delta_z, float vmin, float vmax, float eps, float ret,
+                                               float sc, float ybar, float (&m)[C51_R]) {
+  float y = __fadd_rn(ret, __fmul_rn(sc, ybar));
+  if constexpr (VT) y = vt_h(y, eps);
+  y = fminf(fmaxf(y, vmin), vmax);
+  const float b = __fdiv_rn(__fsub_rn(y, vmin), delta_z);
+  int lo = (int)floorf(b), up = (int)ceilf(b);
+  if (up > 0 && lo == up) lo -= 1;
+  if (lo < Z - 1 && lo == up) up += 1;
+  const float ml = __fsub_rn((float)up, b), mu = __fsub_rn(b, (float)lo);
+#pragma unroll
+  for (int r = 0; r < C51_R; ++r) {
+    const int k = lane + 32 * r;
+    m[r] = k >= Z ? 0.0f : (k == lo ? ml : (k == up ? mu : 0.0f));
+  }
+  return y;
+}
+
+// The one stage the scalar-target kernels differ in, as a functor the shared bodies below call: stage(lane, Z, ret, sc,
+// ybar, m) forms m from ybar and returns y.
 template <int C51_R>
-__global__ void __launch_bounds__(C51D_T)
-k_c51_dueling_hlg(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
-                  const float* __restrict__ returns, const float* __restrict__ nonterminals,
-                  const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax,
-                  float delta_z, float gamma_n, float sigma, int B, int A, int Z, float* __restrict__ loss,
-                  float* __restrict__ dz, float* __restrict__ m_out, int64_t* __restrict__ astar_out,
-                  float* __restrict__ y_out) {
+struct HlgStage {
+  const float* __restrict__ support;
+  float delta_z, vmin, vmax, sigma;
+  __device__ __forceinline__ float operator()(int lane, int Z, float ret, float sc, float ybar, float (&m)[C51_R]) const {
+    return hlg_target<C51_R>(lane, Z, support, delta_z, vmin, vmax, sigma, ret, sc, ybar, m);
+  }
+};
+
+template <int C51_R, bool VT>
+struct TwoHotStage {
+  float delta_z, vmin, vmax, eps;
+  __device__ __forceinline__ float operator()(int lane, int Z, float ret, float sc, float ybar, float (&m)[C51_R]) const {
+    return twohot_target<C51_R, VT>(lane, Z, delta_z, vmin, vmax, eps, ret, sc, ybar, m);
+  }
+};
+
+// Scalar-target loss on the fused heads' rows, laid out as k_c51_dueling (one CTA of C51D_T threads per sample):
+//   phase 0  all threads stage online(s), online(s') and target(s') (stage_z_rows);
+//   phase 1  warp a: the expected value of action a of online(s') over sup_ev;
+//   phase 2  warp 0: a* (first maximum wins), ybar = the expected value of target(s') at a* over sup_ev, y and m (the
+//            stage), then the loss and gradient row of online(s) at the taken action against m (c51_loss_row);
+//   phase 3  dz (dueling_dz).
+// sup_ev: the support the expected values take (support_q, in return units, under value rescaling).
+template <int C51_R, typename Stage>
+__device__ __forceinline__ void
+c51_dueling_scalar(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
+                   const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                   const float* __restrict__ weights, const float* __restrict__ sup_ev, float gamma_n, int B, int A, int Z,
+                   float* __restrict__ loss, float* __restrict__ dz, float* __restrict__ m_out,
+                   int64_t* __restrict__ astar_out, float* __restrict__ y_out, const Stage& stage) {
   extern __shared__ __align__(16) float s_dyn[];
   const int N2 = Z + A * Z;
   float* zs = s_dyn;              // [3][N2]: online(s), online(s'), target(s')
@@ -1845,7 +1888,7 @@ k_c51_dueling_hlg(const float* __restrict__ z_on, const float* __restrict__ z_tg
   const int act = (int)actions[i];
   float sup[C51_R];
 #pragma unroll
-  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(sup_ev + lane + 32 * r) : 0.0f;
   {  // phase 1
     const float* r1 = zs + N2;
     float mean[C51_R];
@@ -1875,8 +1918,7 @@ k_c51_dueling_hlg(const float* __restrict__ z_on, const float* __restrict__ z_tg
     __syncwarp();
     const float ybar = c51_expected_value<C51_R>(x, sup, Z, lane);
     float m[C51_R], g[C51_R];
-    const float y = hlg_target<C51_R>(lane, Z, support, delta_z, vmin, vmax, sigma, __ldg(returns + i),
-                                      __fmul_rn(__ldg(nonterminals + i), gamma_n), ybar, m);
+    const float y = stage(lane, Z, __ldg(returns + i), __fmul_rn(__ldg(nonterminals + i), gamma_n), ybar, m);
     const float l = c51_loss_row<C51_R>(lane, Z, q_s, m, __fdiv_rn(__ldg(weights + i), (float)B), g);
     if (lane == 0) {
       loss[i] = l;
@@ -1896,22 +1938,22 @@ k_c51_dueling_hlg(const float* __restrict__ z_on, const float* __restrict__ z_tg
   dueling_dz<C51D_T>(dz + (size_t)i * N2, s_g, A, Z, act);  // phase 3
 }
 
-// HL-Gauss loss on plain logit rows [B][A][Z] (the library head), k_c51's layout: one warp per sample, grad [B][A][Z]
-// zero but for the taken action's row.
-template <int C51_R>
-__global__ void __launch_bounds__(C51_WARPS * 32)
-k_c51_hlg(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
-          const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
-          const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax, float delta_z,
-          float gamma_n, float sigma, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ grad,
-          float* __restrict__ m_out, int64_t* __restrict__ astar_out, float* __restrict__ y_out) {
+// Scalar-target loss on plain logit rows [B][A][Z] (the library head), k_c51's layout: one warp per sample, grad [B][A][Z]
+// zero but for the taken action's row.  sup_ev as in c51_dueling_scalar.
+template <int C51_R, typename Stage>
+__device__ __forceinline__ void
+c51_scalar(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
+           const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
+           const float* __restrict__ weights, const float* __restrict__ sup_ev, float gamma_n, int B, int A, int Z,
+           float* __restrict__ loss, float* __restrict__ grad, float* __restrict__ m_out, int64_t* __restrict__ astar_out,
+           float* __restrict__ y_out, const Stage& stage) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i = blockIdx.x * C51_WARPS + warp;
   if (i >= B) return;
   const int act = (int)actions[i];
   float sup[C51_R], x[C51_R];
 #pragma unroll
-  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  for (int r = 0; r < C51_R; ++r) sup[r] = (lane + 32 * r < Z) ? __ldg(sup_ev + lane + 32 * r) : 0.0f;
   int best = 0;
   float best_ev = -CUDART_INF_F;
   for (int a = 0; a < A; ++a) {
@@ -1929,8 +1971,7 @@ k_c51_hlg(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, c
   for (int r = 0; r < C51_R; ++r) x[r] = (lane + 32 * r < Z) ? row_t[lane + 32 * r] : -CUDART_INF_F;
   const float ybar = c51_expected_value<C51_R>(x, sup, Z, lane);
   float m[C51_R], g[C51_R];
-  const float y = hlg_target<C51_R>(lane, Z, support, delta_z, vmin, vmax, sigma, __ldg(returns + i),
-                                    __fmul_rn(__ldg(nonterminals + i), gamma_n), ybar, m);
+  const float y = stage(lane, Z, __ldg(returns + i), __fmul_rn(__ldg(nonterminals + i), gamma_n), ybar, m);
   const float l = c51_loss_row<C51_R>(lane, Z, q_on_s + ((size_t)i * A + act) * Z, m,
                                       __fdiv_rn(__ldg(weights + i), (float)B), g);
   if (lane == 0) {
@@ -1949,6 +1990,58 @@ k_c51_hlg(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, c
       if (m_out) m_out[(size_t)i * Z + c] = m[r];
     }
   }
+}
+
+// HL-Gauss loss on the fused heads' rows: c51_dueling_scalar with hlg_target, the expected values over the support.
+template <int C51_R>
+__global__ void __launch_bounds__(C51D_T)
+k_c51_dueling_hlg(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
+                  const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                  const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax,
+                  float delta_z, float gamma_n, float sigma, int B, int A, int Z, float* __restrict__ loss,
+                  float* __restrict__ dz, float* __restrict__ m_out, int64_t* __restrict__ astar_out,
+                  float* __restrict__ y_out) {
+  c51_dueling_scalar<C51_R>(z_on, z_tg, actions, returns, nonterminals, weights, support, gamma_n, B, A, Z, loss, dz, m_out,
+                            astar_out, y_out, HlgStage<C51_R>{support, delta_z, vmin, vmax, sigma});
+}
+
+// HL-Gauss loss on plain logit rows [B][A][Z] (the library head): c51_scalar with hlg_target.
+template <int C51_R>
+__global__ void __launch_bounds__(C51_WARPS * 32)
+k_c51_hlg(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
+          const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
+          const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax, float delta_z,
+          float gamma_n, float sigma, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ grad,
+          float* __restrict__ m_out, int64_t* __restrict__ astar_out, float* __restrict__ y_out) {
+  c51_scalar<C51_R>(q_on_s, q_on_ns, q_tg_ns, actions, returns, nonterminals, weights, support, gamma_n, B, A, Z, loss, grad,
+                    m_out, astar_out, y_out, HlgStage<C51_R>{support, delta_z, vmin, vmax, sigma});
+}
+
+// Two-hot loss on the fused heads' rows: c51_dueling_scalar with twohot_target.  VT (value rescaling): the expected values
+// (arg-max and ybar) over support_q, y = h(.) before the clamp; support_q / eps are read only there.
+template <int C51_R, bool VT>
+__global__ void __launch_bounds__(C51D_T)
+k_c51_dueling_twohot(const float* __restrict__ z_on, const float* __restrict__ z_tg, const int64_t* __restrict__ actions,
+                     const float* __restrict__ returns, const float* __restrict__ nonterminals,
+                     const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax,
+                     float delta_z, float gamma_n, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ dz,
+                     float* __restrict__ m_out, int64_t* __restrict__ astar_out, float* __restrict__ y_out,
+                     const float* __restrict__ support_q, float eps) {
+  c51_dueling_scalar<C51_R>(z_on, z_tg, actions, returns, nonterminals, weights, VT ? support_q : support, gamma_n, B, A, Z,
+                            loss, dz, m_out, astar_out, y_out, TwoHotStage<C51_R, VT>{delta_z, vmin, vmax, eps});
+}
+
+// Two-hot loss on plain logit rows [B][A][Z] (the library head): c51_scalar with twohot_target; VT as above.
+template <int C51_R, bool VT>
+__global__ void __launch_bounds__(C51_WARPS * 32)
+k_c51_twohot(const float* __restrict__ q_on_s, const float* __restrict__ q_on_ns, const float* __restrict__ q_tg_ns,
+             const int64_t* __restrict__ actions, const float* __restrict__ returns, const float* __restrict__ nonterminals,
+             const float* __restrict__ weights, const float* __restrict__ support, float vmin, float vmax, float delta_z,
+             float gamma_n, int B, int A, int Z, float* __restrict__ loss, float* __restrict__ grad,
+             float* __restrict__ m_out, int64_t* __restrict__ astar_out, float* __restrict__ y_out,
+             const float* __restrict__ support_q, float eps) {
+  c51_scalar<C51_R>(q_on_s, q_on_ns, q_tg_ns, actions, returns, nonterminals, weights, VT ? support_q : support, gamma_n, B,
+                    A, Z, loss, grad, m_out, astar_out, y_out, TwoHotStage<C51_R, VT>{delta_z, vmin, vmax, eps});
 }
 
 // ================================================================================================
@@ -3896,6 +3989,95 @@ int rb_c51_dueling_hlg_loss_grad(const float* z_online, const float* z_target, i
     k<<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, support, vmin,
                                                  vmax, delta_z, gamma_n, sigma, B, A, Z, loss, dz, m_out, astar_out, y_out); }
   return check_launch(name);
+}
+
+// The two-hot entries: the parents' refusals in the parents' order (under VT rb_c51_vt_loss_grad's first), then
+// k_c51_twohot / k_c51_dueling_twohot in the parents' launch shapes.
+extern "C++" {
+template <bool VT>
+static int c51_twohot_launch(const char* name, const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
+                             const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                             const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z,
+                             float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, float* y_out,
+                             const float* support_q, float eps, rb_stream_t stream) {
+  int rc = VT ? vt_check(name, support_q != nullptr, eps) : RB_OK;
+  if (rc == RB_OK)
+    rc = c51_check(name, q_online_s && q_online_ns && q_target_ns && actions && returns && nonterminals && weights &&
+                   support && loss && grad_q_online_s, B, A, Z, "A", "Z");
+  if (rc != RB_OK) return rc;
+  const auto k = Z <= 64 ? k_c51_twohot<2, VT> : k_c51_twohot<4, VT>;
+  { ProfScope prof_(RB_K_C51, (cudaStream_t)stream);
+    k<<<(B + C51_WARPS - 1) / C51_WARPS, C51_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        q_online_s, q_online_ns, q_target_ns, actions, returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n,
+        B, A, Z, loss, grad_q_online_s, m_out, astar_out, y_out, support_q, eps); }
+  return check_launch(name);
+}
+
+template <bool VT>
+static int c51_dueling_twohot_launch(const char* name, const float* z_online, const float* z_target, int actions_n,
+                                     int atoms, const int64_t* actions, const float* returns, const float* nonterminals,
+                                     const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                     float gamma_n, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                     float* y_out, const float* support_q, float eps, rb_stream_t stream) {
+  const int Z = atoms, A = actions_n;
+  int rc = VT ? vt_check(name, support_q != nullptr, eps) : RB_OK;
+  if (rc == RB_OK)
+    rc = c51_check(name, z_online && z_target && actions && returns && nonterminals && weights && support && loss && dz, B,
+                   A, Z, "actions", "atoms");
+  if (rc != RB_OK) return rc;
+  // k_c51_dueling's size (the kernel leaves its [Z] slot of target logits unused), so both refuse the same shapes
+  const size_t smem = (size_t)(3 * (Z + A * Z) + 3 * Z + A) * sizeof(float);
+  rc = smem_check(name, smem, "actions * atoms too large");
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling_twohot<2, VT>, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k_c51_dueling_twohot<4, VT>, smem, name);
+  if (rc != RB_OK) return rc;
+  const auto k = Z <= 64 ? k_c51_dueling_twohot<2, VT> : k_c51_dueling_twohot<4, VT>;
+  { ProfScope prof_(RB_K_C51_DUELING, (cudaStream_t)stream);
+    k<<<B, C51D_T, smem, (cudaStream_t)stream>>>(z_online, z_target, actions, returns, nonterminals, weights, support, vmin,
+                                                 vmax, delta_z, gamma_n, B, A, Z, loss, dz, m_out, astar_out, y_out,
+                                                 support_q, eps); }
+  return check_launch(name);
+}
+}
+
+int rb_c51_twohot_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
+                            const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                            const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A, int Z,
+                            float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, float* y_out,
+                            rb_stream_t stream) {
+  return c51_twohot_launch<false>("rb_c51_twohot_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns,
+                                  nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss,
+                                  grad_q_online_s, m_out, astar_out, y_out, nullptr, 0.0f, stream);
+}
+
+int rb_c51_twohot_vt_loss_grad(const float* q_online_s, const float* q_online_ns, const float* q_target_ns,
+                               const int64_t* actions, const float* returns, const float* nonterminals, const float* weights,
+                               const float* support, float vmin, float vmax, float delta_z, float gamma_n, int B, int A,
+                               int Z, float* loss, float* grad_q_online_s, float* m_out, int64_t* astar_out, float* y_out,
+                               const float* support_q, float eps, rb_stream_t stream) {
+  return c51_twohot_launch<true>("rb_c51_twohot_vt_loss_grad", q_online_s, q_online_ns, q_target_ns, actions, returns,
+                                 nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, A, Z, loss,
+                                 grad_q_online_s, m_out, astar_out, y_out, support_q, eps, stream);
+}
+
+int rb_c51_dueling_twohot_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                    const int64_t* actions, const float* returns, const float* nonterminals,
+                                    const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                    float gamma_n, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                    float* y_out, rb_stream_t stream) {
+  return c51_dueling_twohot_launch<false>("rb_c51_dueling_twohot_loss_grad", z_online, z_target, actions_n, atoms, actions,
+                                          returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B, loss, dz,
+                                          m_out, astar_out, y_out, nullptr, 0.0f, stream);
+}
+
+int rb_c51_dueling_twohot_vt_loss_grad(const float* z_online, const float* z_target, int actions_n, int atoms,
+                                       const int64_t* actions, const float* returns, const float* nonterminals,
+                                       const float* weights, const float* support, float vmin, float vmax, float delta_z,
+                                       float gamma_n, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
+                                       float* y_out, const float* support_q, float eps, rb_stream_t stream) {
+  return c51_dueling_twohot_launch<true>("rb_c51_dueling_twohot_vt_loss_grad", z_online, z_target, actions_n, atoms,
+                                         actions, returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B,
+                                         loss, dz, m_out, astar_out, y_out, support_q, eps, stream);
 }
 
 extern "C++" {
