@@ -629,6 +629,25 @@ int rb_c51_dueling_twohot_vt_loss_grad(const float* z_online, const float* z_tar
                                        float gamma_n, int B, float* loss, float* dz, float* m_out, int64_t* astar_out,
                                        float* y_out, const float* support_q, float eps, rb_stream_t stream);
 
+/* CQL(H)'s regulariser for training from a fixed replay (Kumar et al. 2020; DESIGN.md §22), added onto the gradient a
+ * loss entry has just written.  For copy j < M of sample i (row jB + i of the online net's rows of s) with values Q_a --
+ * the expected value sum_k softmax(q_a)_k support_k (the loss entries' arithmetic), or with a NULL support the mean
+ * quantile (sum_k q_ak) / Z of the quantile head:
+ *   R_ij = logsumexp_a Q_a - Q_{a_i}, stable (maximum first, sums in action order), pi = softmax_a Q;
+ *   c    = fl32(fl32(alpha w_i) / (M B)), c_a = fl32(c (pi_a - [a == a_i]));
+ *   grad += c_a fl32(p_ak fl32(support_k - Q_a)) (categorical) or fl32(c_a / Z) (quantile) on the logits of every action:
+ * the gradient of sum_i w_i alpha (1/M) sum_j R_ij / B.  rb_cql_grad takes logit rows [M B][A][Z] (rb_c51_loss_grad's
+ * layout) and adds onto grad [M B][A][Z]; rb_cql_dueling_grad takes the fused heads' z rows [Z + A Z] (their first M B
+ * rows are read) and adds onto dz [M B][Z + A Z] through the dueling combination: dzv_k += gv_k = sum_a g_ak (action
+ * order), dza_ak += g_ak - gv_k / A.  gap_out [B] (optional) = fl32(sum_j R_ij (j order) / M).  No atomics: results do
+ * not depend on scheduling.  RB_ERR_INVAL: a NULL rows, actions, weights or grad, B or A <= 0, Z < 2, or alpha not a
+ * positive finite normal fp32; RB_ERR_RANGE: Z > RB_MAX_ATOMS, M outside [1, RB_MAX_AUG_COPIES], or rows too large for
+ * shared memory.  A refused call writes nothing.  Profiled under RB_K_C51 / RB_K_C51_DUELING. */
+int rb_cql_grad(const float* q_online_s, const int64_t* actions, const float* weights, const float* support, float alpha,
+                int M, int B, int A, int Z, float* grad, float* gap_out, rb_stream_t stream);
+int rb_cql_dueling_grad(const float* z_online, const int64_t* actions, const float* weights, const float* support,
+                        float alpha, int M, int B, int A, int Z, float* dz, float* gap_out, rb_stream_t stream);
+
 /* model.py:43-44 NoisyLinear.forward weight composition W = mu + sigma*eps (elementwise),
  * used for both weights ([out*in]) and biases ([out]). */
 int rb_noisy_compose(const float* mu, const float* sigma, const float* eps, int64_t count, float* out,

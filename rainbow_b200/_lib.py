@@ -193,6 +193,9 @@ SIGNATURES = {
                                                   _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rb_c51_dueling_twohot_vt_loss_grad": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32,
                                                      _i32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _vp]),
+    # CQL(H)'s regulariser: rows, actions, weights, support (NULL: quantiles), alpha, M, B, A, Z, grad / dz, gap_out
+    "rb_cql_grad": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "rb_cql_dueling_grad": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
 }
 
 # rb_learn_stats_record of include/rainbow_b200.h (48 bytes): field name -> numpy dtype, in memory order

@@ -34,6 +34,8 @@ One `learn(mem)` (agent.py:61-100) is:
                                                args.categorical_target = "two_hot": rb_c51_dueling_twohot_loss_grad
                                                (_vt twin under value rescaling) -- the scalar target split between its
                                                two neighbouring atoms]
+    [args.cql_alpha > 0: rb_cql_dueling_grad (rb_cql_grad on the library head) -- CQL(H)'s regulariser over the online
+     rows of s, added onto dz; the losses and priorities stay the TD loss's]
     rb_head_backward (16 head gradients + d conv features), torch autograd backward through the online convs
     [NCCL all-reduce of the flat gradient when world_size > 1]
     K7 rb_clip_adam                           (agent.py:97-98)
@@ -263,6 +265,26 @@ def qr_dueling_munchausen_loss_grad(z_online, z_target, actions_n, atoms, action
         _empty(B, like=actions), _empty(B, atoms * (1 + actions_n), like=actions), (theta_out, bonus_out), None)
 
 
+def cql_grad(q_online_s, actions, weights, support, alpha, grad, M=1, gap_out=None):
+    """CQL(H)'s regulariser (rb_cql_grad, DESIGN.md §22) on the online net's logit rows of s [M B, A, Z] (M copies,
+    copy-major), added onto grad [M B, A, Z]: alpha w_i / (M B) times the gradient of logsumexp_a Q(s, a) - Q(s, a_i).
+    support None: the quantile head (Q the mean quantile).  gap_out [B]: (1/M) sum_j R_ij.  Returns grad."""
+    _, A, Z = q_online_s.shape
+    _lib.check(_lib.load().rb_cql_grad(_lib.ptr(q_online_s), _lib.ptr(actions), _lib.ptr(weights), _lib.ptr(support),
+                                       float(alpha), M, actions.shape[0], A, Z, _lib.ptr(grad), _lib.ptr(gap_out),
+                                       _lib.stream()))
+    return grad
+
+
+def cql_dueling_grad(z_online, actions_n, atoms, actions, weights, support, alpha, dz, M=1, gap_out=None):
+    """cql_grad on the fused heads' rows (rb_cql_dueling_grad): z_online's first M B rows [Z(1+A)] are the copies of s,
+    and the gradient is added onto dz [M B, Z(1+A)] through the dueling combination.  Returns dz."""
+    _lib.check(_lib.load().rb_cql_dueling_grad(_lib.ptr(z_online), _lib.ptr(actions), _lib.ptr(weights), _lib.ptr(support),
+                                               float(alpha), M, actions.shape[0], actions_n, atoms, _lib.ptr(dz),
+                                               _lib.ptr(gap_out), _lib.stream()))
+    return dz
+
+
 DISTRIBUTIONS = ("categorical", "quantile")
 
 
@@ -465,6 +487,23 @@ def two_hot_options(args):
     if copies != (1, 1):
         raise ValueError(f"categorical_target 'two_hot' needs augment_m = augment_k = 1, got {copies}")
     return True
+
+
+def cql_options(args):
+    """CQL(H)'s regulariser for training from a fixed replay (Kumar et al. 2020; DESIGN.md §22): args.cql_alpha rounded to
+    the fp32 the kernels take, or None when it is absent, None or 0.  It must be finite and > 0 as a normal fp32.  Refused
+    with value_transform "rescale" (the regulariser would act on h units); everything else composes."""
+    alpha = getattr(args, "cql_alpha", None)
+    if isinstance(alpha, bool) or not (alpha is None or isinstance(alpha, (int, float))):
+        raise ValueError(f"cql_alpha must be a number, got {alpha!r}")
+    if alpha is None or alpha == 0:
+        return None
+    a32 = float(np.float32(alpha)) if abs(alpha) < 3.5e38 else math.inf
+    if not np.finfo(np.float32).tiny <= a32 < math.inf:
+        raise ValueError(f"cql_alpha must be finite and > 0 as a normal fp32, got {alpha!r}")
+    if getattr(args, "value_transform", None) == "rescale":
+        raise ValueError("cql_alpha does not compose with value_transform 'rescale': the regulariser would act on h units")
+    return a32
 
 
 def risk_beta(t, measure, eta):
@@ -815,6 +854,8 @@ class Agent:
         self.hl_gauss_sigma = hl_gauss_options(args)
         # two-hot targets (off by default; hl_gauss_options returns None for them)
         self.two_hot = two_hot_options(args)
+        # CQL(H)'s regulariser (off by default): alpha as the fp32 the kernels take, or None
+        self.cql_alpha = cql_options(args)
         # the support in return units, fl32(h^-1(z_j)) from the fp32 support in float64 (the support itself when off): the
         # double-DQN arg-max, the target atoms, acting and the statistics take it
         self.q_support = self.support
@@ -948,6 +989,7 @@ class Agent:
         self._rejected_seen = 0
         self._q_graphs = {}       # training-mode flag -> captured one-state act / evaluate_q graph
         self.last_loss = None  # per-sample losses of the most recent update (device tensor)
+        self.last_cql_gap = None  # args.cql_alpha: the CQL gap (1/M) sum_j R_ij per sample of that update (device tensor)
         self._warm = 0
         self._stats = None        # learn-statistics ring (set_learn_stats)
         self.learn_stats_capacity = 0
@@ -1200,6 +1242,7 @@ class Agent:
                 # the priority write-back (agent.py:100) needs nothing but the per-sample losses: it runs on a side
                 # stream beside the whole backward instead of at the end of the critical path
                 wb_done = _lib.side_branch(s_ns, lambda: after_loss(loss))[1]
+            self._cql(z_on, dz, batch, Bs // B)
             hd = on.head()
             dh = torch.empty((FusedHead.dh_rows(Bs), 2 * on.hidden_size), dtype=torch.float32, device=self.device)   # dh, then its transpose
             dx = torch.empty_like(xs_d)
@@ -1263,6 +1306,7 @@ class Agent:
                 q_ns, q_t = q_t[:B], q_t[B:]
             loss, grad, m = self._library_loss(q_s.detach(), q_ns, q_t, batch)
             stats_done = self._stats_batch(batch, loss, m, q=q_s.detach())
+            self._cql(q_s.detach(), grad, batch, 1)
         self.optimiser.zero_grad()
         q_s.backward(grad)
         self.sync.all_reduce_(self.optimiser.flat_grad)
@@ -1335,6 +1379,24 @@ class Agent:
                                           m_out=m, **vt), m)
         return (*c51_loss_grad(*rows, self.support, self.Vmin, self.Vmax, self.delta_z, self._gamma_n(), m_out=m, **vt,
                                risk=risk), m)
+
+    def _cql(self, rows, grad, batch, M):
+        """args.cql_alpha: CQL(H)'s regulariser added onto the loss kernel's gradient, on the caller's stream after the loss
+        entry whichever loss it was (one node of the update graph), with the gap into last_cql_gap.  rows: the online net's
+        fused-head z rows (first M B: the copies of s) and grad dz, or its library logits [B, A, Z] and their gradient.
+        The losses, and so the priorities, stay the TD loss's.  A no-op when the switch is off."""
+        if self.cql_alpha is None:
+            return
+        actions, weights = batch[2], batch[6]
+        B = actions.shape[0]
+        if self.last_cql_gap is None or self.last_cql_gap.shape[0] != B:   # outside a capture: a new B recaptures
+            self.last_cql_gap = torch.empty(B, dtype=torch.float32, device=self.device)
+        support = None if self.quantile else self.support
+        if rows.dim() == 3:
+            cql_grad(rows, actions, weights, support, self.cql_alpha, grad, M, gap_out=self.last_cql_gap)
+        else:
+            cql_dueling_grad(rows, self.action_space, self.atoms, actions, weights, support, self.cql_alpha, grad, M,
+                             gap_out=self.last_cql_gap)
 
     def _hlg_sigma(self):
         """The sigma the HL-Gauss entries take, in return units: fl32(hl_gauss_sigma * delta_z)."""

@@ -388,6 +388,8 @@ def _meta(agent, mem):
         hyper["categorical_target"], hyper["hl_gauss_sigma"] = "hl_gauss", hlg
     if getattr(agent, "two_hot", False):   # two-hot targets record the switch alone
         hyper["categorical_target"] = "two_hot"
+    if getattr(agent, "cql_alpha", None) is not None:   # absent: CQL's regulariser off
+        hyper["cql_alpha"] = agent.cql_alpha
     if agent.bootstrap_truncation:   # absent: off
         hyper["bootstrap_truncation"] = True
     if agent.redo_interval or agent.redo_count:   # the index of the next recycling pass: the counter of its draws
@@ -560,6 +562,8 @@ def _validate(agent, mem, man):
         live = ("two_hot", None)
     if hlg != live:
         raise _Error(f"categorical target (categorical_target, hl_gauss_sigma) differs: checkpoint {hlg}, live {live}")
+    if hyper.get("cql_alpha") != getattr(agent, "cql_alpha", None):
+        raise _Error(f"cql_alpha differs: checkpoint {hyper.get('cql_alpha')}, live {getattr(agent, 'cql_alpha', None)}")
     # a ring with final-observation records means nothing to a replay that gathers without cutting windows at them
     if mem is not None and (man.get("replay") or {}).get("final_records") and not mem.bootstrap_truncation:
         raise _Error("the checkpoint's replay holds final-observation records (args.bootstrap_truncation) and this "

@@ -1445,6 +1445,28 @@ __device__ __forceinline__ void dueling_dz(float* __restrict__ dzi, const float*
   }
 }
 
+// dueling_dz for a gradient row on every action, g [A][Z], ADDED onto the dz row with all T threads:
+// dzv[c] += gv[c] = sum_a g[a][c] (action order from 0), dza[a][c] += g[a][c] - gv[c] / A.  gv is [Z] of shared scratch.
+// The caller synchronises before the call (g complete) and after it (before g or gv are written again).
+template <int T>
+__device__ __forceinline__ void dueling_dz_rows_add(float* __restrict__ dzi, const float* g, float* gv, int A, int Z) {
+  for (int c = threadIdx.x; c < Z; c += T) {
+    float acc = 0.0f;
+    for (int a = 0; a < A; ++a) acc = __fadd_rn(acc, g[a * Z + c]);
+    gv[c] = acc;
+  }
+  __syncthreads();
+  const float inv_a = 1.0f / (float)A;
+  for (int idx = threadIdx.x; idx < Z + A * Z; idx += T) {
+    if (idx < Z) {
+      dzi[idx] = __fadd_rn(dzi[idx], gv[idx]);
+    } else {
+      const int c = (idx - Z) % Z;
+      dzi[idx] = __fadd_rn(dzi[idx], __fsub_rn(g[idx - Z], __fmul_rn(gv[c], inv_a)));
+    }
+  }
+}
+
 // arg-max of s[0, n): the first maximum wins, like torch.argmax
 __device__ __forceinline__ int first_argmax(const float* s, int n) {
   int best = 0;
@@ -2563,6 +2585,126 @@ k_qr_munchausen(const float* __restrict__ q_on_s, const float* __restrict__ q_tg
     const int a = idx / N;
     gq[idx] = (a == act) ? s_g[idx - a * N] : 0.0f;
   }
+}
+
+// ---- CQL(H)'s regulariser (Kumar et al. 2020; DESIGN.md §22) ----
+// For copy j of sample i (row jB + i of the online net's rows of s) and its values Q_a -- the expected value over the
+// support with c51_expected_value's arithmetic (categorical head), or the mean quantile with qr_row_mean's (support NULL)
+// -- R = logsumexp_a Q_a - Q_act = -l_act of munchausen_policy at temperature 1, whose pi is softmax_a Q.  With
+// c = fl32(fl32(alpha w_i) / (M B)) and c_a = fl32(c (pi_a - [a == act])) the gradient on the logits of action a is
+//   categorical  g_ak = fl32(c_a fl32(p_ak fl32(z_k - Q_a))),  p_ak = softmax(q_a)_k;    quantile  g_ak = fl32(c_a / N),
+// ADDED onto the incoming gradient (through dueling_dz_rows_add on the fused head).  One CTA per sample walks its M rows
+// in j order (one CTA per row at M = 1):
+//   phase 0  (fused head) all threads stage the z row;
+//   phase 1  warp a forms action a's logits, Q_a and, categorical, p_ak (z_k - Q_a) into s_g;
+//   phase 2  thread 0 forms pi and R (munchausen_policy) and adds R to the gap in j order;
+//   phase 3  all threads scale s_g into g; phase 4 the gradient row += g.
+// gap_out[i] = fl32(sum_j R_ij / M).  No atomics: an eager launch and a graph replay agree bitwise.
+constexpr int CQL_T = 256;
+constexpr int CQL_WARPS = CQL_T / 32;
+
+template <int R, bool QUANTILE, bool DUELING>
+__device__ __forceinline__ void cql_sample(const float* __restrict__ rows, const int64_t* __restrict__ actions,
+                                           const float* __restrict__ weights, const float* __restrict__ support,
+                                           float alpha, int M, int B, int A, int Z, float* __restrict__ grad,
+                                           float* __restrict__ gap_out) {
+  extern __shared__ __align__(16) float s_dyn[];
+  const int N2 = DUELING ? Z + A * Z : A * Z;   // floats per row
+  float* zs = s_dyn;                            // [N2] the staged z row (fused head)
+  float* s_g = zs + (DUELING ? N2 : 0);         // [A][Z] logits (fused head), then dQ_a / dq_ak, then g
+  float* s_gv = s_g + A * Z;                    // [Z] dueling_dz_rows_add's scratch (fused head)
+  float* s_q = s_gv + (DUELING ? Z : 0);        // [A] Q_a
+  float* s_pi = s_q + A;                        // [A] softmax_a Q
+  const int i = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int act = (int)actions[i];
+  const float c = __fdiv_rn(__fmul_rn(alpha, __ldg(weights + i)), (float)(M * B));
+  float sup[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) sup[r] = (!QUANTILE && lane + 32 * r < Z) ? __ldg(support + lane + 32 * r) : 0.0f;
+  float gap = 0.0f;
+  for (int j = 0; j < M; ++j) {
+    const size_t row = (size_t)j * B + i;
+    const float* src = rows + row * N2;
+    if constexpr (DUELING) {  // phase 0: the one row (M = 1, K = 0) of copy j through the shared stager
+      stage_z_rows<CQL_T>(zs, rows + (size_t)j * B * N2, rows, i, B, N2, 1, 0);
+      __syncthreads();
+    }
+    {  // phase 1
+      float mean[R];
+#pragma unroll
+      for (int r = 0; r < R; ++r) mean[r] = (DUELING && lane + 32 * r < Z) ? dueling_mean(zs, A, Z, lane + 32 * r) : 0.0f;
+      for (int a = warp; a < A; a += CQL_WARPS) {
+        float* ga = s_g + (size_t)a * Z;
+        const float* qa = DUELING ? ga : src + (size_t)a * Z;
+        if constexpr (DUELING) {
+#pragma unroll
+          for (int r = 0; r < R; ++r) {
+            const int k = lane + 32 * r;
+            if (k < Z) ga[k] = dueling_q(zs[k], zs[Z + a * Z + k], mean[r]);
+          }
+          __syncwarp();
+        }
+        float q;
+        if constexpr (QUANTILE) {
+          float x[R];
+#pragma unroll
+          for (int r = 0; r < R; ++r) x[r] = (lane + 32 * r < Z) ? qa[lane + 32 * r] : 0.0f;
+          q = qr_row_mean<R>(x, Z);
+        } else {
+          float e[R], x[R], mx, sum;
+          softmax_row(qa, Z, lane, e, x, mx, sum);
+          q = c51_expected_value<R>(x, sup, Z, lane);
+#pragma unroll
+          for (int r = 0; r < R; ++r)
+            if (lane + 32 * r < Z) ga[lane + 32 * r] = __fmul_rn(__fdiv_rn(e[r], sum), __fsub_rn(sup[r], q));
+        }
+        if (lane == 0) s_q[a] = q;
+      }
+    }
+    __syncthreads();
+    if (tid == 0) {  // phase 2
+      const float Rj = __fsub_rn(0.0f, munchausen_policy(s_q, A, 1.0f, s_pi, nullptr, act));
+      gap = j == 0 ? Rj : __fadd_rn(gap, Rj);
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int a = tid; a < A; a += CQL_T) {  // phase 3: c_a (quantile: c_a / N) over s_q, then g
+      const float ca = __fmul_rn(c, __fsub_rn(s_pi[a], a == act ? 1.0f : 0.0f));
+      s_q[a] = QUANTILE ? __fdiv_rn(ca, (float)Z) : ca;
+    }
+    __syncthreads();
+    for (int idx = tid; idx < A * Z; idx += CQL_T) {
+      const float ca = s_q[idx / Z];
+      s_g[idx] = QUANTILE ? ca : __fmul_rn(ca, s_g[idx]);
+    }
+    __syncthreads();
+    float* gi = grad + row * N2;  // phase 4
+    if constexpr (DUELING) {
+      dueling_dz_rows_add<CQL_T>(gi, s_g, s_gv, A, Z);
+    } else {
+      for (int idx = tid; idx < A * Z; idx += CQL_T) gi[idx] = __fadd_rn(gi[idx], s_g[idx]);
+    }
+    __syncthreads();  // before the next row rewrites zs, s_g and s_gv
+  }
+  if (gap_out && tid == 0) gap_out[i] = __fdiv_rn(gap, (float)M);
+}
+
+// Fused-head entry: z_on rows [Z + A Z] as k_c51_dueling takes them (copy j of s at row jB + i); dz [M B][Z + A Z].
+template <int R, bool QUANTILE>
+__global__ void __launch_bounds__(CQL_T)
+k_cql_dueling(const float* __restrict__ z_on, const int64_t* __restrict__ actions, const float* __restrict__ weights,
+              const float* __restrict__ support, float alpha, int M, int B, int A, int Z, float* __restrict__ dz,
+              float* __restrict__ gap_out) {
+  cql_sample<R, QUANTILE, true>(z_on, actions, weights, support, alpha, M, B, A, Z, dz, gap_out);
+}
+
+// Library-head entry: logit rows [M B][A][Z] in k_c51's layout; grad [M B][A][Z].
+template <int R, bool QUANTILE>
+__global__ void __launch_bounds__(CQL_T)
+k_cql(const float* __restrict__ q_on_s, const int64_t* __restrict__ actions, const float* __restrict__ weights,
+      const float* __restrict__ support, float alpha, int M, int B, int A, int Z, float* __restrict__ grad,
+      float* __restrict__ gap_out) {
+  cql_sample<R, QUANTILE, false>(q_on_s, actions, weights, support, alpha, M, B, A, Z, grad, gap_out);
 }
 
 // Greedy values for acting / evaluation under quantiles: k_q_select with the mean over quantiles in place of
@@ -4078,6 +4220,49 @@ int rb_c51_dueling_twohot_vt_loss_grad(const float* z_online, const float* z_tar
   return c51_dueling_twohot_launch<true>("rb_c51_dueling_twohot_vt_loss_grad", z_online, z_target, actions_n, atoms,
                                          actions, returns, nonterminals, weights, support, vmin, vmax, delta_z, gamma_n, B,
                                          loss, dz, m_out, astar_out, y_out, support_q, eps, stream);
+}
+
+// The CQL entries: the loss entries' shape refusals (c51_check), alpha a positive normal fp32 (NaN, +-inf, 0, negatives
+// and subnormals refused), M in [1, RB_MAX_AUG_COPIES], then the shared-memory limit; k_cql_dueling / k_cql with one CTA
+// per sample.  A NULL support selects the quantile head.
+extern "C++" {
+template <bool DUELING>
+static int cql_launch(const char* name, const float* rows, const int64_t* actions, const float* weights,
+                      const float* support, float alpha, int M, int B, int A, int Z, float* grad, float* gap_out,
+                      rb_stream_t stream) {
+  int rc = c51_check(name, rows && actions && weights && grad, B, A, Z, "A", "Z");
+  if (rc == RB_OK && !(alpha >= FLT_MIN && alpha <= FLT_MAX)) {
+    char msg[128];
+    snprintf(msg, sizeof msg, "%s: alpha must be a positive finite normal fp32", name);
+    rc = fail(RB_ERR_INVAL, msg);
+  }
+  if (rc == RB_OK) rc = copies_check(name, M, 1);
+  if (rc != RB_OK) return rc;
+  const size_t smem = (size_t)((DUELING ? 2 * Z : 0) + 2 * A * Z + 2 * A) * sizeof(float);
+  rc = smem_check(name, smem, "A * Z too large");
+  const auto k2 = support ? (DUELING ? k_cql_dueling<2, false> : k_cql<2, false>)
+                          : (DUELING ? k_cql_dueling<2, true> : k_cql<2, true>);
+  const auto k4 = support ? (DUELING ? k_cql_dueling<4, false> : k_cql<4, false>)
+                          : (DUELING ? k_cql_dueling<4, true> : k_cql<4, true>);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k2, smem, name);
+  if (rc == RB_OK) rc = rbi::ensure_dynamic_smem(k4, smem, name);
+  if (rc != RB_OK) return rc;
+  { ProfScope prof_(DUELING ? RB_K_C51_DUELING : RB_K_C51, (cudaStream_t)stream);
+    (Z <= 64 ? k2 : k4)<<<B, CQL_T, smem, (cudaStream_t)stream>>>(rows, actions, weights, support, alpha, M, B, A, Z, grad,
+                                                                  gap_out); }
+  return check_launch(name);
+}
+}
+
+int rb_cql_grad(const float* q_online_s, const int64_t* actions, const float* weights, const float* support, float alpha,
+                int M, int B, int A, int Z, float* grad, float* gap_out, rb_stream_t stream) {
+  return cql_launch<false>("rb_cql_grad", q_online_s, actions, weights, support, alpha, M, B, A, Z, grad, gap_out, stream);
+}
+
+int rb_cql_dueling_grad(const float* z_online, const int64_t* actions, const float* weights, const float* support,
+                        float alpha, int M, int B, int A, int Z, float* dz, float* gap_out, rb_stream_t stream) {
+  return cql_launch<true>("rb_cql_dueling_grad", z_online, actions, weights, support, alpha, M, B, A, Z, dz, gap_out,
+                          stream);
 }
 
 extern "C++" {
