@@ -258,6 +258,24 @@ int rb_append_batch_trunc(float* tree, int64_t tree_start, int64_t size, uint8_t
                           const float* const* last_frames, const int32_t* actions, const float* rewards,
                           const int32_t* terminals, int k, rb_stream_t stream);
 
+/* Bytes of device scratch rb_append_bulk needs for k records (0 for k <= 0). */
+int rb_append_bulk_scratch_bytes(int64_t k);
+
+/* k consecutive appends of already-quantised records in one call (a dataset fill): the result is bitwise that of k
+ * rb_append_batch_trunc records in order -- frames, timestep, action, reward, nonterminal, every tree node, the running
+ * max (unchanged) and ring_state[0..3].  new_frames: uint8[k][84*84], device or pinned host memory, copied into slots
+ * head, head + 1, ... (mod size) by the copy engine (split in two at the wrap); head must be ring_state[0] as the stream
+ * will find it (the host mirror of the ring's head).  actions int32[k], rewards float32[k] and flags uint8[k] are device
+ * arrays: flag 0 = nonterminal, RB_NONTERMINAL_FINAL = a final-observation record (action 0, reward 0, leaf 0; actions[j]
+ * and rewards[j] are not read), any other value = terminal.  Timesteps continue ring_state[2] until the first nonzero
+ * flag.  scratch: device memory of at least rb_append_bulk_scratch_bytes(k) bytes, used by this call only.
+ * RB_ERR_INVAL: a NULL pointer or an odd size; RB_ERR_RANGE: k outside [1, size], head outside [0, size), a tree deeper
+ * than 30 levels or scratch_bytes too small.  A refused call launches nothing.  Profiled under RB_K_APPEND. */
+int rb_append_bulk(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
+                   float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max, int64_t head,
+                   const uint8_t* new_frames, const int32_t* actions, const float* rewards, const uint8_t* flags,
+                   int64_t k, void* scratch, int64_t scratch_bytes, rb_stream_t stream);
+
 /* agent.py:66-96 Agent.learn minus the three network bodies, given PRE-softmax logits [B,A,Z]
  * (model.py:75 `q`; the softmax / log_softmax of model.py:76-79 are folded in):
  * double-DQN argmax with the online net, target distribution, Tz clamp, l/u projection with the

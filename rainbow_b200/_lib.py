@@ -97,6 +97,10 @@ SIGNATURES = {
     "rb_append_batch": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
     "rb_append_batch_trunc": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32,
                                         _vp]),
+    # bulk append of quantised records: the replay's arrays, head, frames, actions, rewards, flags, k, scratch, its bytes
+    "rb_append_bulk_scratch_bytes": (C.c_int, [_i64]),
+    "rb_append_bulk": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp,
+                                 _i64, _vp]),
     "rb_c51_loss_grad": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i32, _i32, _i32,
                                    _vp, _vp, _vp, _vp, _vp]),
     "rb_noisy_resample": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp, _u64, _vp, _vp]),

@@ -1020,6 +1020,197 @@ k_append_batch_final(float* tree, int64_t tree_start, int64_t size, uint8_t* __r
 }
 
 // ================================================================================================
+// Bulk append (rb_append_bulk): k records of a dataset in one call, equal to k appends in order (DESIGN §23).  The frames
+// are copies issued by the entry; these kernels write the records, the leaves, the touched ancestors and the ring state.
+//   1. k_bulk_block_reset  : per tile of BULK_TILE records, the last index whose flag is nonzero (-1 if none);
+//   2. k_bulk_scan_tiles   : one CTA, exclusive max-scan of those over the tiles, in place, and the block's total;
+//   3. k_bulk_records      : r_j = the last index < j with a nonzero flag, t_j = r_j < 0 ? t_ep0 + j : j - r_j - 1; the
+//                            record at slot (head + j) mod size and its leaf (*running_max, 0 for a FINAL record);
+//   4. k_bulk_tree_level   : one grid-wide launch per wide level: each touched ancestor = fl32(left + right);
+//   5. k_bulk_tree_top     : one CTA finishes the narrow top levels, then advances the ring state once.
+// Every launch reads the head from ring_state[0]; only the last one writes it.  k <= size, so every record survives.
+// ================================================================================================
+constexpr int BULK_THREADS = 256;
+constexpr int BULK_ITEMS = 4;
+constexpr int BULK_TILE = BULK_THREADS * BULK_ITEMS;
+constexpr int BULK_TOP_THREADS = 1024;
+
+__device__ __forceinline__ int warp_max_int(int v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// Block-wide max of v over BULK_THREADS threads (the result in every thread).
+__device__ __forceinline__ int bulk_block_max(int v, int* s_warp) {
+  v = warp_max_int(v);
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int m = -1;
+#pragma unroll
+  for (int w = 0; w < BULK_THREADS / 32; ++w) m = max(m, s_warp[w]);
+  return m;
+}
+
+__global__ void __launch_bounds__(BULK_THREADS)
+k_bulk_block_reset(const uint8_t* __restrict__ flags, int k, int* __restrict__ tile_reset) {
+  __shared__ int s_warp[BULK_THREADS / 32];
+  const int base = blockIdx.x * BULK_TILE;
+  int r = -1;
+#pragma unroll
+  for (int u = 0; u < BULK_ITEMS; ++u) {
+    const int j = base + u * BULK_THREADS + threadIdx.x;
+    if (j < k && flags[j]) r = max(r, j);
+  }
+  r = bulk_block_max(r, s_warp);
+  if (threadIdx.x == 0) tile_reset[blockIdx.x] = r;
+}
+
+// tile_reset[0 .. tiles) -> the exclusive prefix max (-1 before tile 0); tile_reset[tiles] = the max over all tiles.
+__global__ void __launch_bounds__(BULK_TOP_THREADS)
+k_bulk_scan_tiles(int* tile_reset, int tiles) {
+  __shared__ int s_warp[BULK_TOP_THREADS / 32];
+  __shared__ int s_carry;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) s_carry = -1;
+  __syncthreads();
+  for (int base = 0; base < tiles; base += BULK_TOP_THREADS) {
+    const int i = base + threadIdx.x;
+    const int v = i < tiles ? tile_reset[i] : -1;
+    int inc = v;   // inclusive max within the warp
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc = max(inc, y);
+    }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    int before = s_carry, total = s_carry;
+    for (int w = 0; w < BULK_TOP_THREADS / 32; ++w) {
+      if (w < warp) before = max(before, s_warp[w]);
+      total = max(total, s_warp[w]);
+    }
+    const int prev = __shfl_up_sync(0xffffffffu, inc, 1);
+    const int excl = lane > 0 ? max(before, prev) : before;
+    __syncthreads();   // s_carry and s_warp read by every thread
+    if (i < tiles) tile_reset[i] = excl;
+    if (threadIdx.x == 0) s_carry = total;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) tile_reset[tiles] = s_carry;
+}
+
+__global__ void __launch_bounds__(BULK_THREADS)
+k_bulk_records(float* tree, int64_t tree_start, int64_t size, int32_t* timestep, int32_t* action, float* reward,
+               uint8_t* nonterminal, const int64_t* ring_state, const float* running_max,
+               const int32_t* __restrict__ actions, const float* __restrict__ rewards, const uint8_t* __restrict__ flags,
+               int k, const int* __restrict__ tile_reset) {
+  __shared__ int s_warp[BULK_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t head = ring_state[0];
+  const int64_t t_ep0 = ring_state[2];
+  const float leaf = *running_max;
+  // thread-contiguous items: thread x of tile b holds records base + BULK_ITEMS x + u
+  const int base = blockIdx.x * BULK_TILE + BULK_ITEMS * threadIdx.x;
+  uint8_t f[BULK_ITEMS];
+  int own = -1;
+#pragma unroll
+  for (int u = 0; u < BULK_ITEMS; ++u) {
+    const int j = base + u;
+    f[u] = j < k ? flags[j] : (uint8_t)0;
+    if (f[u]) own = j;
+  }
+  int inc = own;   // inclusive max over the threads of the warp, then exclusive over the block
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc = max(inc, y);
+  }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  int r = tile_reset[blockIdx.x];   // the last reset before this tile
+  for (int w = 0; w < warp; ++w) r = max(r, s_warp[w]);
+  const int prev = __shfl_up_sync(0xffffffffu, inc, 1);
+  if (lane > 0) r = max(r, prev);
+#pragma unroll
+  for (int u = 0; u < BULK_ITEMS; ++u) {
+    const int j = base + u;
+    if (j < k) {
+      const int64_t t = r < 0 ? t_ep0 + j : (int64_t)(j - r - 1);
+      int64_t slot = head + j;
+      if (slot >= size) slot -= size;
+      const bool fin = f[u] == RB_NONTERMINAL_FINAL;
+      timestep[slot] = (int32_t)t;
+      action[slot] = fin ? 0 : actions[j];
+      reward[slot] = fin ? 0.0f : rewards[j];
+      nonterminal[slot] = fin ? (uint8_t)RB_NONTERMINAL_FINAL : f[u] ? (uint8_t)0 : (uint8_t)1;
+      __stcg(tree + tree_start + slot, fin ? 0.0f : leaf);
+      if (f[u]) r = j;
+    }
+  }
+}
+
+// The touched nodes s levels above the leaves, as two disjoint intervals [a1, b1] and [a2, b2] of heap indices (the second
+// may be empty: b2 < a2).  The leaves are slots head .. head + k - 1 (mod size): [head, min(head + k, size)) and, after a
+// wrap, [0, head + k - size).  Both children of every such node lie inside the array (size is even).
+__device__ __forceinline__ void bulk_level_nodes(int64_t head, int64_t k, int64_t size, int64_t tree_start, int s,
+                                                 int64_t& a1, int64_t& b1, int64_t& a2, int64_t& b2) {
+  const int64_t end = head + k;
+  const int64_t hi1 = (end < size ? end : size) - 1;
+  a1 = ((tree_start + head + 1) >> s) - 1;
+  b1 = ((tree_start + hi1 + 1) >> s) - 1;
+  a2 = 0;
+  b2 = -1;
+  if (end > size) {
+    a2 = ((tree_start + 1) >> s) - 1;
+    b2 = ((tree_start + (end - size - 1) + 1) >> s) - 1;
+    if (b2 + 1 >= a1) {   // the wrapped range lies left of the first; merge where they meet or overlap
+      a1 = a2;
+      a2 = 0;
+      b2 = -1;
+    }
+  }
+}
+
+__device__ __forceinline__ void bulk_rebuild_node(float* tree, int64_t p) {
+  __stcg(tree + p, __fadd_rn(__ldcg(tree + 2 * p + 1), __ldcg(tree + 2 * p + 2)));
+}
+
+__global__ void __launch_bounds__(BULK_THREADS)
+k_bulk_tree_level(float* tree, int64_t tree_start, int64_t size, const int64_t* ring_state, int k, int s) {
+  int64_t a1, b1, a2, b2;
+  bulk_level_nodes(ring_state[0], k, size, tree_start, s, a1, b1, a2, b2);
+  const int64_t n2 = b2 - a2 + 1, n = n2 + (b1 - a1 + 1);
+  const int64_t i = (int64_t)blockIdx.x * BULK_THREADS + threadIdx.x;
+  if (i < n) bulk_rebuild_node(tree, i < n2 ? a2 + i : a1 + (i - n2));
+}
+
+__global__ void __launch_bounds__(BULK_TOP_THREADS)
+k_bulk_tree_top(float* tree, int64_t tree_start, int64_t size, int64_t* ring_state, int k, int s_first,
+                const int* tile_reset, int tiles) {
+  const int64_t head = ring_state[0];
+  const int L = tree_depth(tree_start);
+  for (int s = s_first; s <= L; ++s) {
+    int64_t a1, b1, a2, b2;
+    bulk_level_nodes(head, k, size, tree_start, s, a1, b1, a2, b2);
+    const int64_t n2 = b2 - a2 + 1, n = n2 + (b1 - a1 + 1);
+    for (int64_t i = threadIdx.x; i < n; i += BULK_TOP_THREADS) bulk_rebuild_node(tree, i < n2 ? a2 + i : a1 + (i - n2));
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {   // every earlier launch has read the old head
+    const int r_last = tile_reset[tiles];
+    int64_t nh = head + k;
+    if (nh >= size) {
+      nh -= size;
+      ring_state[1] = 1;
+    }
+    ring_state[2] = r_last < 0 ? ring_state[2] + k : (int64_t)(k - 1 - r_last);
+    ring_state[0] = nh;
+    ring_state[3] = ring_state[3] + k;
+  }
+}
+
+// ================================================================================================
 // Value rescaling (Pohlen et al. 2018): h(x) = sign(x) (sqrt(|x| + 1) - 1) + eps x and its inverse, in cancellation-free
 // forms (DESIGN.md §16): every step adds or multiplies nonnegative terms, each rounded explicitly (no contraction), with
 // IEEE sqrtf and __fdiv_rn.  0 <= eps <= 1 (the host entries refuse anything else).
@@ -3835,6 +4026,54 @@ int rb_append_batch_trunc(float* tree, int64_t tree_start, int64_t size, uint8_t
                           const int32_t* terminals, int k, rb_stream_t stream) {
   return append_batch_launch("rb_append_batch_trunc", true, tree, tree_start, size, frames, timestep, action, reward,
                              nonterminal, ring_state, running_max, last_frames, actions, rewards, terminals, k, stream);
+}
+
+int rb_append_bulk_scratch_bytes(int64_t k) {
+  if (k <= 0) return 0;
+  if (k > ((int64_t)1 << 30)) k = (int64_t)1 << 30;   // rb_append_bulk's largest k (size <= 2^30)
+  return (int)(sizeof(int) * ((k + BULK_TILE - 1) / BULK_TILE + 1));
+}
+
+int rb_append_bulk(float* tree, int64_t tree_start, int64_t size, uint8_t* frames, int32_t* timestep, int32_t* action,
+                   float* reward, uint8_t* nonterminal, int64_t* ring_state, float* running_max, int64_t head,
+                   const uint8_t* new_frames, const int32_t* actions, const float* rewards, const uint8_t* flags,
+                   int64_t k, void* scratch, int64_t scratch_bytes, rb_stream_t stream) {
+  if (!tree || !frames || !timestep || !action || !reward || !nonterminal || !ring_state || !running_max || !new_frames ||
+      !actions || !rewards || !flags || !scratch)
+    return fail(RB_ERR_INVAL, "rb_append_bulk: null pointer");
+  if (size <= 0 || (size & 1)) return fail(RB_ERR_INVAL, "rb_append_bulk: an even size is required");
+  if (tree_depth(tree_start) > 30) return fail(RB_ERR_RANGE, "rb_append_bulk: tree deeper than 30 levels");
+  if (k < 1 || k > size) return fail(RB_ERR_RANGE, "rb_append_bulk: 1 <= k <= size");
+  if (head < 0 || head >= size) return fail(RB_ERR_RANGE, "rb_append_bulk: head outside [0, size)");
+  if (scratch_bytes < rb_append_bulk_scratch_bytes(k))
+    return fail(RB_ERR_RANGE, "rb_append_bulk: scratch smaller than rb_append_bulk_scratch_bytes(k)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int kk = (int)k;   // k <= size <= 2^30
+  const int tiles = (kk + BULK_TILE - 1) / BULK_TILE;
+  int* tile_reset = static_cast<int*>(scratch);
+  { ProfScope prof_(RB_K_APPEND, st);
+    // frames: copy-engine copies (device or pinned host source), split at the wrap
+    const int64_t n1 = head + k <= size ? k : size - head;
+    cudaError_t e = cudaMemcpyAsync(frames + (size_t)head * RB_FRAME_BYTES, new_frames, (size_t)n1 * RB_FRAME_BYTES,
+                                    cudaMemcpyDefault, st);
+    if (e == cudaSuccess && n1 < k)
+      e = cudaMemcpyAsync(frames, new_frames + (size_t)n1 * RB_FRAME_BYTES, (size_t)(k - n1) * RB_FRAME_BYTES,
+                          cudaMemcpyDefault, st);
+    if (e != cudaSuccess) return fail(RB_ERR_CUDA, cudaGetErrorString(e));
+    k_bulk_block_reset<<<tiles, BULK_THREADS, 0, st>>>(flags, kk, tile_reset);
+    k_bulk_scan_tiles<<<1, BULK_TOP_THREADS, 0, st>>>(tile_reset, tiles);
+    k_bulk_records<<<tiles, BULK_THREADS, 0, st>>>(tree, tree_start, size, timestep, action, reward, nonterminal,
+                                                    ring_state, running_max, actions, rewards, flags, kk, tile_reset);
+    // a level s above the leaves holds at most (k >> s) + 4 touched nodes; the wide ones get a grid each
+    const int L = tree_depth(tree_start);
+    int s = 1;
+    for (; s <= L && (k >> s) + 4 > 4 * BULK_TOP_THREADS; ++s) {
+      const int64_t n = (k >> s) + 4;
+      k_bulk_tree_level<<<(unsigned)((n + BULK_THREADS - 1) / BULK_THREADS), BULK_THREADS, 0, st>>>(
+          tree, tree_start, size, ring_state, kk, s);
+    }
+    k_bulk_tree_top<<<1, BULK_TOP_THREADS, 0, st>>>(tree, tree_start, size, ring_state, kk, s, tile_reset, tiles); }
+  return check_launch("rb_append_bulk");
 }
 
 // The value-rescaled entries' own refusals: support_q (C51) given, 0 <= eps <= 1 (NaN refused).

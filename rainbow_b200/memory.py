@@ -14,6 +14,8 @@ called through the C ABI in include/rainbow_b200.h:
                           counterpart; rb_gather_aug with intensity > 0 or copies != (1, 1): shift and intensity
                           augmentation of M copies of s and K of s'; rb_gather_horizon with an annealed horizon, see
                           rainbow_b200.horizon; rb_gather_trunc with args.bootstrap_truncation)
+    extend             -> rb_append_bulk          (k appends of quantised arrays in one call: a dataset fill, no
+                                                   reference counterpart)
     update_priorities  -> rb_tree_update   (K4)   memory.py:157-159, 23-48
     __next__           -> rb_iter_states          memory.py:166-178
 
@@ -413,6 +415,148 @@ class ReplayMemory:
         self.t = 0
         if self.defer_appends and len(self._queue) >= self.APPEND_BATCH:
             self.flush_appends()
+
+    # ---- bulk fill from arrays ------------------------------------------------------------------
+    EXTEND_CHUNK_BYTES = 64 << 20   # frames per rb_append_bulk call and per pinned staging buffer (two of them)
+
+    def extend(self, frames, actions, rewards, terminals, final=None):
+        """Append k transitions given as arrays, bitwise as k calls of append() (and append_truncated() for the pairs
+        `final` marks) would leave the replay: frames, records, the whole sum tree, the running max, the ring state and
+        the host mirrors index, full and t.  With k > capacity only the last `capacity` records remain.
+
+        frames: uint8 [k, 84, 84] or [k, 7056], the newest frame of each state already quantised, as datasets store it:
+        numpy, a CPU tensor (pageable or pinned) or a CUDA tensor on this replay's device (read in stream order on the
+        current stream).  Float frames are refused; append's rounding is q = (uint8)(int)fl32(f * 255).
+        actions (integers that fit int32), rewards (rounded to fp32 as append rounds float(reward)), terminals: [k].
+        final (optional, [k] bool, needs args.bootstrap_truncation): record j is the final observation of a time-limited
+        episode, so records j - 1 and j are what append_truncated(state_{j-1}, a, r, final_state_j) writes.  Record j - 1
+        must be in the same call, neither terminal nor final; record j must have terminal False, action 0 and reward 0.
+
+        Everything is checked before anything is written, and a refused call writes nothing.  A non-empty defer_appends
+        queue is written first.  Host frames go through two owned pinned buffers of EXTEND_CHUNK_BYTES (a host copy into
+        one while the copy engine moves the other), so the caller may reuse its arrays as soon as this returns; the host
+        waits only on those buffers' events."""
+        fr, acts, rews, flags = self._check_extend(frames, actions, rewards, terminals, final)
+        k = flags.size
+        if k == 0:
+            return
+        self.flush_appends()
+        tr = self.transitions
+        chunk = max(1, min(tr.size, self.EXTEND_CHUNK_BYTES // FRAME))
+        stage = self._extend_stage(min(chunk, k), fr.is_cuda)
+        stream = torch.cuda.current_stream(self.device)
+        for c, j0 in enumerate(range(0, k, chunk)):
+            n = min(chunk, k - j0)
+            b = c % 2
+            if stage["evt"][b] is not None:
+                stage["evt"][b].synchronize()
+            stage["act"][b][:n].copy_(torch.from_numpy(acts[j0:j0 + n]))
+            stage["rew"][b][:n].copy_(torch.from_numpy(rews[j0:j0 + n]))
+            stage["flag"][b][:n].copy_(torch.from_numpy(flags[j0:j0 + n]))
+            if fr.is_cuda:
+                src = fr[j0:j0 + n]
+            else:
+                stage["frames"][b][:n].copy_(fr[j0:j0 + n])
+                src = stage["frames"][b]
+            dev = stage["dev"]
+            dev["act"][:n].copy_(stage["act"][b][:n], non_blocking=True)
+            dev["rew"][:n].copy_(stage["rew"][b][:n], non_blocking=True)
+            dev["flag"][:n].copy_(stage["flag"][b][:n], non_blocking=True)
+            _lib.check(self._lib.rb_append_bulk(
+                _lib.ptr(tr.tree), tr.tree_start, tr.size, _lib.ptr(tr.frames), _lib.ptr(tr.timestep),
+                _lib.ptr(tr.action), _lib.ptr(tr.reward), _lib.ptr(tr.nonterminal), _lib.ptr(tr.ring_state),
+                _lib.ptr(tr.running_max), tr.index, src.data_ptr(), _lib.ptr(dev["act"]), _lib.ptr(dev["rew"]),
+                _lib.ptr(dev["flag"]), n, _lib.ptr(dev["scratch"]), dev["scratch"].numel(), stream.cuda_stream))
+            evt = torch.cuda.Event()
+            evt.record(stream)
+            stage["evt"][b] = evt
+            tr.full = tr.full or tr.index + n >= tr.size
+            tr.index = (tr.index + n) % tr.size
+        resets = np.flatnonzero(flags)
+        self.t = self.t + k if resets.size == 0 else int(k - 1 - resets[-1])
+
+    def _extend_stage(self, chunk, cuda_frames):
+        """Pinned staging (two buffers of `chunk` records; frames only for host frames) and the device record buffers."""
+        st = getattr(self, "_bulk", None)
+        if st is None or st["chunk"] < chunk or (not cuda_frames and st["frames"] is None):
+            pin = lambda shape, dt: torch.empty(shape, dtype=dt).pin_memory()   # noqa: E731
+            st = dict(chunk=chunk, evt=[None, None],
+                      frames=None if cuda_frames else [pin((chunk, FRAME), torch.uint8) for _ in range(2)],
+                      act=[pin(chunk, torch.int32) for _ in range(2)], rew=[pin(chunk, torch.float32) for _ in range(2)],
+                      flag=[pin(chunk, torch.uint8) for _ in range(2)])
+            nbytes = int(self._lib.rb_append_bulk_scratch_bytes(chunk))
+            st["dev"] = dict(act=torch.empty(chunk, dtype=torch.int32, device=self.device),
+                             rew=torch.empty(chunk, dtype=torch.float32, device=self.device),
+                             flag=torch.empty(chunk, dtype=torch.uint8, device=self.device),
+                             scratch=torch.empty(nbytes, dtype=torch.uint8, device=self.device))
+            old = getattr(self, "_bulk", None)
+            if old is not None:   # the old buffers may still feed queued copies
+                for e in old["evt"]:
+                    if e is not None:
+                        e.synchronize()
+            self._bulk = st
+        return st
+
+    def _check_extend(self, frames, actions, rewards, terminals, final):
+        """extend()'s inputs checked and converted: (frames [k, 7056] uint8 tensor, int32, float32 and uint8 flag arrays)."""
+        if isinstance(frames, torch.Tensor):
+            fr = frames.detach()
+            if fr.is_cuda and fr.device != self.device:
+                raise ValueError(f"frames are on {fr.device}, the replay on {self.device}")
+        else:
+            fr = torch.from_numpy(np.ascontiguousarray(frames))
+        if fr.is_floating_point():
+            raise ValueError("extend takes uint8 frames, already quantised; quantise float frames f in [0, 1] as append "
+                             "does: q = (f.astype(np.float32) * np.float32(255)).astype(np.int32).astype(np.uint8)")
+        if fr.dtype != torch.uint8:
+            raise ValueError(f"frames must be uint8, got {fr.dtype}")
+        if not (fr.dim() == 2 and fr.shape[1] == FRAME) and not (fr.dim() == 3 and tuple(fr.shape[1:]) == (84, 84)):
+            raise ValueError(f"frames must be [k, 84, 84] or [k, {FRAME}], got {tuple(fr.shape)}")
+        k = fr.shape[0]
+        fr = fr.reshape(k, FRAME)
+        if fr.is_cuda:
+            fr = fr.contiguous()
+
+        def host(x, name):
+            a = x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+            if a.shape != (k,):
+                raise ValueError(f"{name} must have shape ({k},) like the frames, got {a.shape}")
+            return a
+
+        a, r, term = host(actions, "actions"), host(rewards, "rewards"), host(terminals, "terminals")
+        if a.dtype.kind not in "iu":
+            raise ValueError(f"actions must be integers, got {a.dtype}")
+        if k and (a.min() < -2 ** 31 or a.max() >= 2 ** 31):
+            raise ValueError("actions must fit int32")
+        if r.dtype.kind not in "iuf":
+            raise ValueError(f"rewards must be numbers, got {r.dtype}")
+        if term.dtype.kind not in "biu":
+            raise ValueError(f"terminals must be bool or integers, got {term.dtype}")
+        acts = a.astype(np.int32)
+        rews = r.astype(np.float64).astype(np.float32)   # float(reward) -> c_float, as append rounds it
+        flags = (term != 0).astype(np.uint8)
+        if final is not None:
+            if not self.bootstrap_truncation:
+                raise _lib.RainbowB200Error("extend(final=...) needs args.bootstrap_truncation = True: without it the "
+                                            "replay cannot store the final observation a time limit stopped the episode at")
+            fin = host(final, "final")
+            if fin.dtype.kind not in "biu":
+                raise ValueError(f"final must be bool, got {fin.dtype}")
+            fin = fin != 0
+            idx = np.flatnonzero(fin)
+            bad = [(j, why) for j, why in (
+                *((j, "is the first record of the call") for j in idx[idx == 0]),
+                *((j, "is also terminal") for j in idx[flags[idx] != 0]),
+                *((j, "has a nonzero action") for j in idx[acts[idx] != 0]),
+                *((j, "has a nonzero reward") for j in idx[rews[idx].view(np.uint32) != 0]),
+                *((j, "follows a terminal") for j in idx[(idx > 0) & (flags[idx - 1] != 0)]),
+                *((j, "follows another final record") for j in idx[(idx > 0) & fin[idx - 1]]))]
+            if bad:
+                j, why = min(bad)
+                raise ValueError(f"final record {j} {why}: a final observation follows its episode's last transition "
+                                 "and carries terminal False, action 0 and reward 0")
+            flags[fin] = FINAL
+        return fr, acts, rews, flags
 
     def flush_appends(self):
         """Write the queued transitions (defer_appends=True) with one rb_append_batch launch."""
